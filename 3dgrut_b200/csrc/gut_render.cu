@@ -11,9 +11,9 @@
 // shape is fixed by parity), 256 threads = 256 pixels, sorted particle lists consumed in batches staged in
 // shared memory as render-ready records (scale folded into the rotation rows once per staged particle
 // instead of once per pixel test).  Both kernels are FP32/SFU-issue bound, not HBM bound.
-// G7 reduces the 16 canonical per-particle sums (section comment "G7 backward") across a quarter of the warp with a
-// 16-value transposing butterfly (14 SHFL) and lands them with one 8-byte vector RED per lane into a [N,20]
-// accumulator that G8 maps to the final gradients and re-zeroes.
+// G7 sums the 16 canonical per-particle sums (+ 3 depth slots; section comment "G7 backward") over a quarter of the warp through a
+// per-warp shared-memory scratch and lands each 16-byte column with one vector RED into a [N,20] accumulator that G8 maps to the
+// final gradients and re-zeroes.
 #include "gut_common.cuh"
 #include "hit_math.cuh"
 #include "subtile_cull.cuh"
@@ -424,68 +424,44 @@ __global__ void __launch_bounds__(kTilePixels) render_forward_kernel(FrameCamera
 // staged record, 6 x float4:
 //   r0, r1, r2 = rows of quaternionWXYZToMatrix (columns of R); .w = canonical frame origin S^-1 R (o_f - mu) (FAST) | position (GENERAL)
 //   sc = scale.xyz, density     is = 1/scale.xyz, _     cl = clamped rgb, particle index bits
+// The rotation rows are kept apart from 1/scale (the forward stages M = S^-1 R^T): the backward's accept test applies 1/s after the
+// rotation, as the reference's adjoint does.  With the forward's record the test moves by the last bits, borderline pairs flip, and
+// on a 500-Gaussian scene the gradients drifted from 4.7e-4 to 1.8e-3 relative to the CPU restatement of the reference.
+//
+// The gradient rows of one lockstep iteration are summed through a per-warp scratch:
+//   every lane stores its row (g[0..15], the depth slots 16..18 when the warp carries a distance gradient; zeros without a hit) as
+//   float4 at a stride of kGradRow floats -- 8 consecutive lanes then hit 8 distinct 16-byte bank groups, so the stores are
+//   conflict-free --, and lane r (r < 5, or < 4 without depth slots) of each sub-block sums float4 column r over the sub-block's
+//   rows and lands it with one 16-byte vector RED.  For SUBL 8 and 16 the readers of one lane octet read two rows 4 lanes apart,
+//   columns 0..3: 16-byte groups 5 row + r and 5 row + 20 + r are again 8 distinct ones.
+// This replaced a transposing butterfly over the sub-block (14 SHFL + 14 FADD + ~28 SEL per lane, 3 more 5-level sums for the depth
+// slots and a second RED): 5 STS.128 + SUBL LDS.128 on the summing lanes, 5 REDs per flushed row instead of 9 (4 instead of 8 without
+// the depth slots).  render_backward on C2 (H100 80GB HBM3, 700 W, 1980 MHz, three runs each): 0.454-0.460 -> 0.417-0.422 ms; with the rgb / opacity
+// loss (no depth slots) unchanged at 0.354-0.358 ms.
 
 struct BwdSmem {
     float4 r0[kBatch], r1[kBatch], r2[kBatch], sc[kBatch], is[kBatch], cl[kBatch];
-    uint32_t hw[(kBatch / 32) * kWordsPerChunk];  // the forward's hit words of this batch, [chunk][warp][quarter]
+    uint32_t hw[(kBatch / 32) * kWordsPerChunk];        // the forward's hit words of this batch, [chunk][warp][quarter]
+    float4 rows[kTilePixels / 32][32 * kGradRow / 4];  // gradient rows of one lockstep iteration, [warp][lane * 5 + column]
 };
 
-// Transposing butterfly over the SUBL lanes of a sub-block (SUBL = 32: the warp, 16: half = 4x4 pixels, 8: quarter = 4x2 pixels; the
-// sub-block id uses lane bits b2 (and b4), the exchanges use the others).  Each level halves the number of values a lane carries:
-//   SUBL 32: 16 values -> 1 (both lanes of a pair hold it), component = lane >> 1                         16 SHFL
-//   SUBL 16: 16 values -> 1, component = 8 [lane & 16] + 4 [lane & 8] + 2 [lane & 2] + [lane & 1]          15 SHFL
-//   SUBL  8: 16 values -> 2 (v[0], v[1]), components 8 [lane & 8] + 4 [lane & 2] + 2 [lane & 1] + {0, 1}   14 SHFL
-template <int H>
-__device__ __forceinline__ void butterfly_level(float (&v)[16], bool up, int mask) {
-#pragma unroll
-    for (int i = 0; i < H; ++i) {
-        const float send = up ? v[i] : v[i + H];
-        const float keep = up ? v[i + H] : v[i];
-        v[i] = keep + __shfl_xor_sync(kFull, send, mask);
-    }
+// Sub-blocks of SUBL lanes (32: the warp, 16: half = 4x4 pixels, 8: quarter = 4x2 pixels): the sub-block id uses lane bits b2 (and
+// b4), the lanes within it the others.  sub_lane = the i-th lane of the sub-block whose lowest lane is `first`, sub_rank = its inverse.
+template <int SUBL>
+__device__ __forceinline__ int sub_first(int lane) { return SUBL == 32 ? 0 : SUBL == 16 ? (lane & 4) : (lane & 20); }
+
+template <int SUBL>
+__device__ __forceinline__ int sub_lane(int first, int i) {
+    if (SUBL == 32) return i;
+    if (SUBL == 16) return first | (i & 3) | ((i & 12) << 1);
+    return first | (i & 3) | ((i & 4) << 1);
 }
 
 template <int SUBL>
-__device__ __forceinline__ void sub_reduce16(float (&v)[16], int lane) {
-    if (SUBL == 32) {
-        butterfly_level<8>(v, lane & 16, 16);
-        butterfly_level<4>(v, lane & 8, 8);
-        butterfly_level<2>(v, lane & 4, 4);
-        butterfly_level<1>(v, lane & 2, 2);
-        v[0] += __shfl_xor_sync(kFull, v[0], 1);
-    } else if (SUBL == 16) {
-        butterfly_level<8>(v, lane & 16, 16);
-        butterfly_level<4>(v, lane & 8, 8);
-        butterfly_level<2>(v, lane & 2, 2);
-        butterfly_level<1>(v, lane & 1, 1);
-    } else {
-        butterfly_level<8>(v, lane & 8, 8);
-        butterfly_level<4>(v, lane & 2, 2);
-        butterfly_level<2>(v, lane & 1, 1);
-    }
-}
-
-// plain sum over the lanes of a sub-block (every lane receives it) and the lane that writes it
-template <int SUBL>
-__device__ __forceinline__ float sub_sum(float v) {
-    if (SUBL >= 16) v += __shfl_xor_sync(kFull, v, 16);
-    v += __shfl_xor_sync(kFull, v, 8);
-    if (SUBL == 32) v += __shfl_xor_sync(kFull, v, 4);
-    v += __shfl_xor_sync(kFull, v, 2);
-    v += __shfl_xor_sync(kFull, v, 1);
-    return v;
-}
-
-template <int SUBL>
-__device__ __forceinline__ bool sub_leader(int lane) {
-    return SUBL == 32 ? lane == 0 : SUBL == 16 ? (lane & 27) == 0 : (lane & 11) == 0;
-}
-
-template <int SUBL>
-__device__ __forceinline__ int sub_component(int lane) {
-    if (SUBL == 32) return lane >> 1;
-    if (SUBL == 16) return ((lane & 16) >> 1) | ((lane & 8) >> 1) | (lane & 3);
-    return (lane & 8) | ((lane & 2) << 1) | ((lane & 1) << 1);
+__device__ __forceinline__ int sub_rank(int lane) {
+    if (SUBL == 32) return lane;
+    if (SUBL == 16) return (lane & 3) | ((lane >> 1) & 12);
+    return (lane & 3) | ((lane >> 1) & 4);
 }
 
 // per-pixel backward state (initializeBackwardRay, kernels/cuda/common/rayPayloadBackward.cuh:31-73)
@@ -599,9 +575,12 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
     const float dox = ray.ox - ofx, doy = ray.oy - ofy, doz = ray.oz - ofz;   // zero in FAST tiles
     const bool depth_grads = __any_sync(kFull, alive && (st.Dgrad != 0.f));
     const int quarter = lane_quarter(lane);
-    // lanes of this lane's sub-block, and where its gradient components land after the reduction
+    // lanes of this lane's sub-block, and the float4 column of the gradient row this lane sums (columns >= 5 / 4: none)
     const unsigned sub_lanes = SUBL == 32 ? kFull : SUBL == 16 ? (quarter_lanes(quarter & 1) | quarter_lanes((quarter & 1) | 2)) : quarter_lanes(quarter);
-    const int comp = sub_component<SUBL>(lane);
+    const int first = sub_first<SUBL>(lane);
+    const int col = sub_rank<SUBL>(lane);
+    const int cols = depth_grads ? 5 : 4;
+    float4* rows = sm.rows[tid >> 5];
     for (uint32_t base = begin; base < end; base += kBatch) {
         if (__syncthreads_and(!alive)) break;
         const uint32_t k = base + tid;
@@ -659,23 +638,23 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
                 if (act && alive) hit = backward_pair<DEG, FAST>(cfg, sm, j, ray, dox, doy, doz, depth_grads, st, alive, g, ex);
                 const unsigned hits = __ballot_sync(kFull, hit);
                 if (hits) {
-                    sub_reduce16<SUBL>(g, lane);
-                    if (depth_grads) {  // warp-uniform: the depth branch's direct scale part, slots 16..18 of the row
-                        ex[0] = sub_sum<SUBL>(ex[0]); ex[1] = sub_sum<SUBL>(ex[1]); ex[2] = sub_sum<SUBL>(ex[2]);
-                        if ((hits & sub_lanes) && sub_leader<SUBL>(lane))
-                            atomicAdd(reinterpret_cast<float4*>(grad_acc + static_cast<size_t>(__float_as_uint(sm.cl[j].w)) * kGradRow + 16),
-                                      make_float4(ex[0], ex[1], ex[2], 0.f));
-                    }
-                    if (hits & sub_lanes) {  // this sub-block's particle received something
-                        float* row = grad_acc + static_cast<size_t>(__float_as_uint(sm.cl[j].w)) * kGradRow + comp;
-                        if (SUBL == 32) {
-                            if ((lane & 1) == 0) atomicAdd(row, g[0]);
-                        } else if (SUBL == 16) {
-                            atomicAdd(row, g[0]);
-                        } else {
-                            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(row), "f"(g[0]), "f"(g[1]) : "memory");
+                    float4* mine = rows + lane * (kGradRow / 4);
+                    mine[0] = make_float4(g[0], g[1], g[2], g[3]);
+                    mine[1] = make_float4(g[4], g[5], g[6], g[7]);
+                    mine[2] = make_float4(g[8], g[9], g[10], g[11]);
+                    mine[3] = make_float4(g[12], g[13], g[14], g[15]);
+                    if (depth_grads) mine[4] = make_float4(ex[0], ex[1], ex[2], 0.f);  // warp-uniform
+                    __syncwarp();
+                    if ((hits & sub_lanes) && col < cols) {  // this sub-block's particle received something
+                        float4 s = rows[sub_lane<SUBL>(first, 0) * (kGradRow / 4) + col];
+#pragma unroll
+                        for (int i = 1; i < SUBL; ++i) {
+                            const float4 v = rows[sub_lane<SUBL>(first, i) * (kGradRow / 4) + col];
+                            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
                         }
+                        atomicAdd(reinterpret_cast<float4*>(grad_acc + static_cast<size_t>(__float_as_uint(sm.cl[j].w)) * kGradRow) + col, s);
                     }
+                    __syncwarp();  // the next iteration overwrites the rows
                     if (__all_sync(kFull, !alive)) break;
                 }
             }
@@ -696,6 +675,9 @@ __device__ __forceinline__ bool frame_common_origin(const FrameCamera& cam, cons
     return __syncthreads_and(same);
 }
 
+// 3 CTAs per SM (72-80 registers, 45 KB of shared memory per CTA; 24 warps per SM).  4 CTAs would fit in shared memory but cap the
+// kernel at 64 registers, where every instantiation spills (36 B stores, 64 B loads per thread).  Measured at C2 on an H100 80GB HBM3
+// (700 W), bench.py --steps 50, three runs each, render_backward: 3 -> 0.417-0.422 ms, 4 (with the spills) -> 0.413-0.414 ms.
 template <int DEG, int SUBL>
 __global__ void __launch_bounds__(kTilePixels, 3) render_backward_kernel(FrameCamera cam, FrameConfig cfg,
                                                                       const float* __restrict__ rays_o,
