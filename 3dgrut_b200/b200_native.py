@@ -225,7 +225,11 @@ class GrtConfig(C.Structure):
     """grtb200_config"""
 
     _fields_ = [("kernel_degree", C.c_int32), ("min_response", C.c_float), ("min_alpha", C.c_float), ("max_alpha", C.c_float),
-                ("density_clamping", C.c_int32)]
+                ("density_clamping", C.c_int32), ("primitive", C.c_int32)]
+
+
+# grtb200_config.primitive (render.primitive_type)
+GRT_PRIMITIVES = {"instances": 0, "icosahedron": 1}
 
 
 GRT_EXPORTS = ["grtb200_default_config", "grtb200_create", "grtb200_destroy", "grtb200_last_error", "grtb200_build_bvh", "grtb200_trace",
@@ -265,6 +269,8 @@ class GrtContext:
         self._lib = _grt_lib()
         self._h = C.c_void_p()
         rc = self._lib.grtb200_create(C.byref(cfg), int(device), C.byref(self._h))
+        if rc == 5:
+            raise ValueError(f"grtb200_create: primitive {cfg.primitive} is not one of {GRT_PRIMITIVES}")
         if rc != 0 or not self._h:
             raise RuntimeError(f"grtb200_create failed (rc={rc}): a CUDA device is required, there is no CPU path")
         self.cfg = cfg

@@ -38,8 +38,8 @@ class OptixTracer:
             raise RuntimeError("threedgrt_tracer: CUDA device required; there is no CPU path")
         if pipeline not in ("reference",) or backward_pipeline not in ("referenceBwd",):
             raise NotImplementedError("only the default reference / referenceBwd pipelines are built")
-        if primitive != "instances":
-            raise NotImplementedError("only the default `instances` proxy is built (configs/render/3dgrt.yaml:11)")
+        if primitive not in native.GRT_PRIMITIVES:
+            raise NotImplementedError(f"primitive_type {primitive!r} is not built; built proxies: {', '.join(native.GRT_PRIMITIVES)}")
         if enable_normals:
             raise NotImplementedError("normals output is not built")
         if int(particle_radiance_sph_degree) != 3:
@@ -49,6 +49,7 @@ class OptixTracer:
         cfg.min_response = float(particle_kernel_min_response)
         cfg.max_alpha = float(particle_kernel_max_alpha)
         cfg.density_clamping = int(bool(particle_kernel_density_clamping))
+        cfg.primitive = native.GRT_PRIMITIVES[primitive]
         self._cfg = cfg
         self._ctx = {}
 

@@ -38,16 +38,23 @@ typedef struct grtb200_config {
     float min_alpha;         /* alphaMinThreshold 1/255 (optixTracer.cpp:928)            */
     float max_alpha;         /* render.particle_kernel_max_alpha 0.99                    */
     int32_t density_clamping; /* render.particle_kernel_density_clamping (true)          */
+    int32_t primitive;       /* render.primitive_type: 0 instances (default), 1 icosahedron */
 } grtb200_config;
+
+/* grtb200_config.primitive */
+#define GRTB200_PRIMITIVE_INSTANCES 0
+#define GRTB200_PRIMITIVE_ICOSAHEDRON 1
 
 typedef struct grtb200_ctx grtb200_ctx;
 
 void grtb200_default_config(grtb200_config* cfg);
+/* Returns 2 without a usable CUDA device and 5 when cfg->primitive is not one of GRTB200_PRIMITIVE_*. */
 int grtb200_create(const grtb200_config* cfg, int device, grtb200_ctx** out);
 void grtb200_destroy(grtb200_ctx* ctx);
 const char* grtb200_last_error(const grtb200_ctx* ctx);
 
-/* (Re)build the LBVH over the particles' bounding proxies.  `rebuild`/`allow_update` are accepted for API
+/* (Re)build the LBVH over the particles' bounding proxies (cfg->primitive: the instance box or the icosahedron; both are traced
+ * in the instance space of the particle, no triangles are stored).  `rebuild`/`allow_update` are accepted for API
  * compatibility; every call is a full rebuild (the reference's default config also rebuilds every step). */
 int grtb200_build_bvh(grtb200_ctx* ctx, void* stream, int64_t n, const float* pos, const float* rot, const float* scl,
                       const float* dns, int32_t rebuild, int32_t allow_update);
