@@ -260,8 +260,9 @@ void fill_frame(gutb200_ctx* c, const gutb200_camera* cam) {
     g.k_buffer_size = s.k_buffer_size;
 }
 
-int check_args(gutb200_ctx* c, const gutb200_camera* cam, int64_t n, const void* particles) {
+int check_args(gutb200_ctx* c, const gutb200_camera* cam, int64_t n, const void* particles, int32_t sph_degree) {
     if (!c) return 1;
+    if (sph_degree < 0 || sph_degree > 3) return fail(c, "sph_degree %d out of range (0..3)", sph_degree);
     if (!cam || cam->width <= 0 || cam->height <= 0) return fail(c, "invalid camera resolution");
     if (cam->rolling_shutter < 0 || cam->rolling_shutter > 4) return fail(c, "rolling_shutter %d out of range (0 global, 1..4 readout directions)", cam->rolling_shutter);
     if (cam->model < 0 || cam->model > 2) return fail(c, "camera model %d unknown (0 = OpenCV pinhole, 1 = OpenCV fisheye, 2 = f-theta)", cam->model);
@@ -269,6 +270,8 @@ int check_args(gutb200_ctx* c, const gutb200_camera* cam, int64_t n, const void*
     if (reinterpret_cast<uintptr_t>(particles) & 15) return fail(c, "particle buffer must be 16-byte aligned");
     if (c->cfg.k_buffer_size < 0 || c->cfg.k_buffer_size > 16) return fail(c, "k_buffer_size %d out of range (0..16)", c->cfg.k_buffer_size);
     if (c->cfg.kernel_degree != 2 && c->cfg.kernel_degree != 4) return fail(c, "kernel_degree %d not built (2 or 4)", c->cfg.kernel_degree);
+    if (((c->cfg.subtile_culling >> 4) & 3) == 3)
+        return fail(c, "subtile_culling sub-block code 3 (bits 4-5) not built (0 = quarter-warps, 1 = half-warps, 2 = whole warps)");
     return 0;
 }
 
@@ -391,7 +394,7 @@ int64_t gutb200_launch_count(const gutb200_ctx* c) { return c ? c->launches : 0;
 int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
                     int32_t sph_degree, const float* rays_o, const float* rays_d, float* out_rgba, float* out_dist, float* out_hits,
                     float* visibility) {
-    if (int rc = check_args(c, cam, n, particles)) return rc;
+    if (int rc = check_args(c, cam, n, particles, sph_degree)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     GUT_CUDA(c, cudaSetDevice(c->device));
     c->have_forward = false;
@@ -505,7 +508,7 @@ int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int
 static int backward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
                          int32_t sph_degree, const float* rays_o, const float* rays_d, const float* out_rgba, const float* d_rgba,
                          const float* out_dist, const float* d_dist, float* d_particles, float* d_sph, bool compact) {
-    if (int rc = check_args(c, cam, n, particles)) return rc;
+    if (int rc = check_args(c, cam, n, particles, sph_degree)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     // the backward replays the sorted lists of the immediately preceding forward (gutRenderer.cu:436-440)
     if (!c->have_forward || c->fwd_stream != s || c->n != n || c->cam.width != cam->width || c->cam.height != cam->height)

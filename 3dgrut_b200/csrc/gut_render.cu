@@ -994,7 +994,8 @@ void launch_render_backward(cudaStream_t s, const FrameCamera& cam, const FrameC
                             const uint32_t* ranges, const uint32_t* tile_order, const uint32_t* chunk_base, const uint32_t* hit_words,
                             const float* out_rgba, const float* d_rgba, const float* out_dist, const float* d_dist, float* grad_acc) {
     const unsigned grid = cam.grid_x * cam.grid_y;
-    // sub-block width of the backward walk: bits 4..5 of the switch (0 = default quarter-warps, 1 = half-warps, 2 = whole warp)
+    // sub-block width of the backward walk: bits 4..5 of the switch (0 = default quarter-warps, 1 = half-warps, 2 = whole warp;
+    // check_args rejects 3)
     const int sub = (cfg.subtile_culling >> 4) & 3;
 #define GUT_BWD(DEG_, SUB_) render_backward_kernel<DEG_, SUB_><<<grid, kTilePixels, 0, s>>>(cam, cfg, rays_o, rays_d, particles, rgb, sorted_values, ranges, tile_order, chunk_base, hit_words, out_rgba, d_rgba, out_dist, d_dist, grad_acc)
     if (cfg.kernel_degree == 4) {
