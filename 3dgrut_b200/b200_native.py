@@ -45,7 +45,7 @@ EXPORTS = [
     "gutb200_backward_compact", "gutb200_sph_grad_from_views", "gutb200_camera_position",
     "gutb200_debug_work_counters", "gutb200_debug_fma_peak",
     "gutb200_selective_adam_update", "gutb200_gaussian_adam_step",  # bound in optimizers/__init__.py
-    "gutb200_image_loss_scratch_bytes", "gutb200_image_loss",  # bound in losses.py
+    "gutb200_image_loss_scratch_bytes", "gutb200_image_loss", "gutb200_image_loss_rgb",  # bound in losses.py
 ]
 
 def camera_position(cam):
@@ -232,7 +232,8 @@ class GrtConfig(C.Structure):
 GRT_PRIMITIVES = {"instances": 0, "icosahedron": 1}
 
 
-GRT_EXPORTS = ["grtb200_default_config", "grtb200_create", "grtb200_destroy", "grtb200_last_error", "grtb200_build_bvh", "grtb200_trace",
+GRT_EXPORTS = ["grtb200_default_config", "grtb200_create", "grtb200_destroy", "grtb200_last_error", "grtb200_build_bvh",
+               "grtb200_build_bvh_packed", "grtb200_trace",
                "grtb200_trace_bwd", "grtb200_scene_aabb", "grtb200_launch_count", "grtb200_debug_trace_counters", "grtb200_set_replay"]
 
 
@@ -247,6 +248,7 @@ def _grt_lib():
         lib.grtb200_create.argtypes = [C.POINTER(GrtConfig), C.c_int, C.POINTER(vp)]
         lib.grtb200_destroy.argtypes = [vp]
         lib.grtb200_build_bvh.argtypes = [vp, vp, i64, vp, vp, vp, vp, i32, i32]
+        lib.grtb200_build_bvh_packed.argtypes = [vp, vp, i64, vp]
         lib.grtb200_trace.argtypes = [vp, vp, i64, vp, vp, i32, f32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.grtb200_trace_bwd.argtypes = [vp, vp, i64, vp, vp, i32, f32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.grtb200_scene_aabb.argtypes = [vp, vp]
@@ -292,6 +294,10 @@ class GrtContext:
 
     def build_bvh(self, stream, n, pos, rot, scl, dns, rebuild=True, allow_update=False):
         self._check(self._lib.grtb200_build_bvh(self._h, stream, n, pos, rot, scl, dns, int(rebuild), int(allow_update)), "grtb200_build_bvh")
+
+    def build_bvh_packed(self, stream, n, particles):
+        """The same build from the [N,12] particle record that trace reads (grtb200_build_bvh_packed)."""
+        self._check(self._lib.grtb200_build_bvh_packed(self._h, stream, n, particles), "grtb200_build_bvh_packed")
 
     def trace(self, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d, r2w_host, out_rgb, out_alpha,
               out_dist, out_hits, visibility):

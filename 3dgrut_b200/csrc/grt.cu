@@ -112,21 +112,24 @@ __device__ __forceinline__ float slab_dot(const float (&n)[3], float x, float y,
     return fmaf(n[0], x, fmaf(n[1], y, n[2] * z));
 }
 
+// PS, RS, SS, DS: floats between consecutive particles in pos / rot / scl / dns -- 3, 4, 3, 1 for the four separate arrays of
+// grtb200_build_bvh, 12 for all four when they point into the [N,12] particle record (grtb200_build_bvh_packed).  Only the loads differ.
+template <int PS, int RS, int SS, int DS>
 __global__ void __launch_bounds__(256) proxy_kernel(int n, const float* __restrict__ pos, const float* __restrict__ rot,
                                                     const float* __restrict__ scl, const float* __restrict__ dns, float min_response,
                                                     int clamping, float degree, int primitive, Proxy* __restrict__ proxies,
                                                     Box* __restrict__ boxes, int* __restrict__ scene /*[6] ordered ints*/) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float ks = kernel_scale(dns[i], min_response, clamping, degree);
-    const float kx = ks * scl[i * 3], ky = ks * scl[i * 3 + 1], kz = ks * scl[i * 3 + 2];
-    const float r = rot[i * 4], x = rot[i * 4 + 1], y = rot[i * 4 + 2], z = rot[i * 4 + 3];
+    const float ks = kernel_scale(dns[i * DS], min_response, clamping, degree);
+    const float kx = ks * scl[i * SS], ky = ks * scl[i * SS + 1], kz = ks * scl[i * SS + 2];
+    const float r = rot[i * RS], x = rot[i * RS + 1], y = rot[i * RS + 2], z = rot[i * RS + 3];
     const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, xz = x * z, yz = y * z, rx = r * x, ry = r * y, rz = r * z;
     // c0,c1,c2 = columns of R
     const float c0x = 1.f - 2.f * (yy + zz), c0y = 2.f * (xy + rz), c0z = 2.f * (xz - ry);
     const float c1x = 2.f * (xy - rz), c1y = 1.f - 2.f * (xx + zz), c1z = 2.f * (yz + rx);
     const float c2x = 2.f * (xz + ry), c2y = 2.f * (yz - rx), c2z = 1.f - 2.f * (xx + yy);
-    const float px = pos[i * 3], py = pos[i * 3 + 1], pz = pos[i * 3 + 2];
+    const float px = pos[i * PS], py = pos[i * PS + 1], pz = pos[i * PS + 2];
     Proxy p;
     p.a0 = make_float4(c0x / kx, c0y / kx, c0z / kx, px);
     p.a1 = make_float4(c1x / ky, c1y / ky, c1z / ky, py);
@@ -952,8 +955,9 @@ void grtb200_destroy(grtb200_ctx* c) {
 const char* grtb200_last_error(const grtb200_ctx* c) { return c ? c->error.c_str() : "null context"; }
 int64_t grtb200_launch_count(const grtb200_ctx* c) { return c ? c->launches : 0; }
 
-int grtb200_build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos, const float* rot, const float* scl, const float* dns,
-                      int32_t /*rebuild*/, int32_t /*allow_update*/) {
+// Both build entries: `packed` says that pos / rot / scl / dns point into the [N,12] particle record (row stride 12 floats).
+static int build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos, const float* rot, const float* scl, const float* dns,
+                     bool packed) {
     if (!c) return 1;
     if (n < 0 || n > 0x3FFFFFFF) return fail(c, "particle count %lld out of range", static_cast<long long>(n));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -996,8 +1000,16 @@ int grtb200_build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos,
     const int init[6] = {0x7F7FFFFF, 0x7F7FFFFF, 0x7F7FFFFF, static_cast<int>(0xFF7FFFFF ^ 0x7FFFFFFF), static_cast<int>(0xFF7FFFFF ^ 0x7FFFFFFF),
                          static_cast<int>(0xFF7FFFFF ^ 0x7FFFFFFF)};  // +FLT_MAX / ordered(-FLT_MAX)
     GRT_CUDA(c, cudaMemcpyAsync(c->scene, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    proxy_kernel<<<blocks, 256, 0, s>>>(ni, pos, rot, scl, dns, c->cfg.min_response, c->cfg.density_clamping, static_cast<float>(c->cfg.kernel_degree),
-                                        c->cfg.primitive, static_cast<Proxy*>(c->proxies), static_cast<Box*>(c->leaf_boxes), static_cast<int*>(c->scene));
+    if (packed)
+        proxy_kernel<12, 12, 12, 12><<<blocks, 256, 0, s>>>(ni, pos, rot, scl, dns, c->cfg.min_response, c->cfg.density_clamping,
+                                                            static_cast<float>(c->cfg.kernel_degree), c->cfg.primitive,
+                                                            static_cast<Proxy*>(c->proxies), static_cast<Box*>(c->leaf_boxes),
+                                                            static_cast<int*>(c->scene));
+    else
+        proxy_kernel<3, 4, 3, 1><<<blocks, 256, 0, s>>>(ni, pos, rot, scl, dns, c->cfg.min_response, c->cfg.density_clamping,
+                                                        static_cast<float>(c->cfg.kernel_degree), c->cfg.primitive,
+                                                        static_cast<Proxy*>(c->proxies), static_cast<Box*>(c->leaf_boxes),
+                                                        static_cast<int*>(c->scene));
     c->launches++;
     {
         int size_levels = 1;
@@ -1042,6 +1054,19 @@ int grtb200_build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos,
     }
     GRT_CUDA(c, cudaGetLastError());
     return 0;
+}
+
+int grtb200_build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos, const float* rot, const float* scl, const float* dns,
+                      int32_t /*rebuild*/, int32_t /*allow_update*/) {
+    return build_bvh(c, stream, n, pos, rot, scl, dns, false);
+}
+
+// The particle record [N,12] = pos3, density, quat(wxyz), scale3, pad is what grtb200_trace reads: a training step that keeps its
+// activated particles in that layout builds from it directly instead of copying out four arrays.
+int grtb200_build_bvh_packed(grtb200_ctx* c, void* stream, int64_t n, const float* particles) {
+    if (!c) return 1;
+    if (!particles && n > 0) return fail(c, "particles is null");
+    return build_bvh(c, stream, n, particles, particles + 4, particles + 8, particles + 3, true);
 }
 
 int grtb200_scene_aabb(grtb200_ctx* c, float* aabb6) {

@@ -12,6 +12,8 @@
 //                       d loss / d map (stored [H,W,9])
 //   loss_grad_kernel    convolves those maps and assembles d loss / d x, written as [H,W,4] with a zero alpha gradient -- directly the
 //                       d_rgba argument of gutb200_backward.
+// Both are templated on the pixel strides of the prediction and the gradient, so that gutb200_image_loss_rgb runs the same arithmetic on
+// the 3DGRT layout (rgb [H,W,3] in, d_rgb [H,W,3] out, directly the d_rgb argument of grtb200_trace_bwd).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -46,6 +48,8 @@ __device__ __forceinline__ float block_sum(float v, float* scratch) {
     return total;  // valid in thread (0,0)
 }
 
+// PS: floats per pixel of the prediction (4: the 3DGUT [H,W,4] image, 3: the 3DGRT rgb [H,W,3]); only the loads depend on it.
+template <int PS>
 __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
                                                              Window win, float g_scale /* -lambda_ssim / count */, float* __restrict__ dmaps,
                                                              float* __restrict__ sums /* [2]: sum |x-y|, sum of the valid SSIM map */) {
@@ -64,7 +68,7 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
             const int gx = x0 + lx - kR, gy = y0 + ly - kR;
             const bool in = (gx >= 0) && (gy >= 0) && (gx < W) && (gy < H);
             const int64_t p = static_cast<int64_t>(gy) * W + gx;
-            sx[ly][lx] = in ? pred_rgba[p * 4 + c] : 0.f;
+            sx[ly][lx] = in ? pred_rgba[p * PS + c] : 0.f;
             sy[ly][lx] = in ? target[p * 3 + c] : 0.f;
         }
         __syncthreads();
@@ -112,6 +116,8 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
     }
 }
 
+// GS: floats per pixel of the gradient (4: d_rgba with a zero alpha gradient, one 16-byte store; 3: d_rgb).
+template <int PS, int GS>
 __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
                                                             Window win, float l1_scale /* lambda_l1 / (H W 3) */, const float* __restrict__ dmaps,
                                                             float* __restrict__ d_rgba) {
@@ -152,14 +158,44 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
         }
         if (inside) {
             const int64_t p = static_cast<int64_t>(py) * W + px;
-            const float xv = pred_rgba[p * 4 + c], yv = target[p * 3 + c];
+            const float xv = pred_rgba[p * PS + c], yv = target[p * 3 + c];
             const float diff = xv - yv;
             const float sgn = diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f);
             grad[c] = c0 + 2.f * xv * c1 + yv * c2 + l1_scale * sgn;
         }
         __syncthreads();
     }
-    if (inside) reinterpret_cast<float4*>(d_rgba)[static_cast<int64_t>(py) * W + px] = make_float4(grad[0], grad[1], grad[2], 0.f);
+    if (!inside) return;
+    const int64_t p = static_cast<int64_t>(py) * W + px;
+    if (GS == 4) {
+        reinterpret_cast<float4*>(d_rgba)[p] = make_float4(grad[0], grad[1], grad[2], 0.f);
+    } else {
+        d_rgba[p * GS + 0] = grad[0];
+        d_rgba[p * GS + 1] = grad[1];
+        d_rgba[p * GS + 2] = grad[2];
+    }
+}
+
+template <int PS, int GS>
+int image_loss(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1, float lambda_ssim,
+               void* scratch, float* d_pred, float* sums2) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    Window win;
+    double g[11], total = 0.0;
+    for (int i = 0; i < 11; ++i) {
+        const double x = i - 5;
+        g[i] = exp(-(x * x) / (2.0 * 1.5 * 1.5));
+        total += g[i];
+    }
+    for (int i = 0; i < 11; ++i) win.w[i] = static_cast<float>(g[i] / total);
+    const double count = (height > 10 && width > 10) ? static_cast<double>(height - 10) * (width - 10) * 3.0 : 1.0;
+    if (cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s) != cudaSuccess) return 2;
+    const dim3 block(kT, kT), grid((width + kT - 1) / kT, (height + kT - 1) / kT);
+    float* dmaps = static_cast<float*>(scratch);
+    ssim_stats_kernel<PS><<<grid, block, 0, s>>>(height, width, pred, target_rgb, win, static_cast<float>(-lambda_ssim / count), dmaps, sums2);
+    loss_grad_kernel<PS, GS><<<grid, block, 0, s>>>(height, width, pred, target_rgb, win,
+                                                    static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)), dmaps, d_pred);
+    return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 
 }  // namespace
@@ -174,26 +210,16 @@ size_t gutb200_image_loss_scratch_bytes(int32_t height, int32_t width) {
 
 int gutb200_image_loss(void* stream, int32_t height, int32_t width, const float* pred_rgba, const float* target_rgb, float lambda_l1,
                        float lambda_ssim, void* scratch, float* d_rgba, float* sums2) {
-    using namespace gutb200;
     if (height <= 0 || width <= 0 || !pred_rgba || !target_rgb || !scratch || !d_rgba || !sums2) return 1;
     if ((reinterpret_cast<uintptr_t>(d_rgba) & 15) != 0) return 3;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    Window win;
-    double g[11], total = 0.0;
-    for (int i = 0; i < 11; ++i) {
-        const double x = i - 5;
-        g[i] = exp(-(x * x) / (2.0 * 1.5 * 1.5));
-        total += g[i];
-    }
-    for (int i = 0; i < 11; ++i) win.w[i] = static_cast<float>(g[i] / total);
-    const double count = (height > 10 && width > 10) ? static_cast<double>(height - 10) * (width - 10) * 3.0 : 1.0;
-    if (cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s) != cudaSuccess) return 2;
-    const dim3 block(kT, kT), grid((width + kT - 1) / kT, (height + kT - 1) / kT);
-    float* dmaps = static_cast<float*>(scratch);
-    ssim_stats_kernel<<<grid, block, 0, s>>>(height, width, pred_rgba, target_rgb, win, static_cast<float>(-lambda_ssim / count), dmaps, sums2);
-    loss_grad_kernel<<<grid, block, 0, s>>>(height, width, pred_rgba, target_rgb, win,
-                                            static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)), dmaps, d_rgba);
-    return cudaGetLastError() == cudaSuccess ? 0 : 2;
+    return gutb200::image_loss<4, 4>(stream, height, width, pred_rgba, target_rgb, lambda_l1, lambda_ssim, scratch, d_rgba, sums2);
+}
+
+// The same loss on the 3DGRT layout: prediction rgb [H,W,3] (alpha is a separate output there and takes no part), gradient d_rgb [H,W,3].
+int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const float* pred_rgb, const float* target_rgb, float lambda_l1,
+                           float lambda_ssim, void* scratch, float* d_rgb, float* sums2) {
+    if (height <= 0 || width <= 0 || !pred_rgb || !target_rgb || !scratch || !d_rgb || !sums2) return 1;
+    return gutb200::image_loss<3, 3>(stream, height, width, pred_rgb, target_rgb, lambda_l1, lambda_ssim, scratch, d_rgb, sums2);
 }
 
 }  // extern "C"

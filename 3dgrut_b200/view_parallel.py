@@ -3,7 +3,8 @@ cameras, sum the per-Gaussian gradients once per step.  The reference has no mul
 
 One process per GPU (torchrun); `torch.distributed` with NCCL over NVLink on a multi-GPU node, gloo in the CPU tests.
 The only exchange of the path is the gradient sum, so the only collective is one all-reduce over a single flat
-bucket holding [N,3]+[N,4]+[N,3]+[N,1]+[N,48] = 59 floats per Gaussian (236 B x N per rank)."""
+bucket holding [N,3]+[N,4]+[N,3]+[N,1]+[N,48] = 59 floats per Gaussian (236 B x N per rank).  The training steps use
+CompactGradientExchange (3DGUT, 64 B per Gaussian) and FlatGradientExchange (3DGRT, 240 B per Gaussian)."""
 from __future__ import annotations
 
 from typing import Iterable, List, Sequence
@@ -127,3 +128,32 @@ class CompactGradientExchange:
         """Bytes a rank receives + sends per step with ring collectives: all-reduce 2 (w-1)/w x 48 N, all-gathers (w-1) x 16 N per view."""
         w = self.world
         return int(2 * (w - 1) / w * 48 * self.n + self.views_per_rank * (w - 1) * 16 * self.n) if w > 1 else 0
+
+
+class FlatGradientExchange:
+    """The gradient exchange of the 3DGRT path: one SUM all-reduce of 60 floats per Gaussian (240 B x N).
+
+    d_particles [N,12] and d_sph [N,48] are views of one flat fp32 buffer; `OptixTracer.trace_bwd(..., out=self.out())` writes the view's
+    gradients straight into it, and `exchange` sums the buffer over the ranks in place.  The compact 64-byte exchange of the 3DGUT path does
+    not apply: there a Gaussian's SH gradient in one view is basis(one direction) x g, while 3DGRT evaluates the radiance along every ray
+    that hits the Gaussian, so its SH gradient is a sum over rays with different directions and has no 4-float summary."""
+
+    def __init__(self, n: int, device, group=None):
+        self.n, self.group = int(n), group
+        self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+        self.bucket = GradientBucket([(self.n, 12), (self.n, 48)], device)
+        self.d_particles, self.d_sph = self.bucket.views
+
+    def out(self):
+        """The (d_particles, d_sph) pair to pass as `out=` to OptixTracer.trace_bwd."""
+        return self.d_particles, self.d_sph
+
+    def exchange(self):
+        """Sums the buffer over the ranks (no-op on one rank); returns (d_particles [N,12], d_sph [N,48])."""
+        self.bucket.all_reduce(group=self.group)
+        return self.d_particles, self.d_sph
+
+    def bytes_on_wire(self) -> int:
+        """Bytes a rank sends + receives per step with a ring all-reduce: 2 (w-1)/w x 240 N."""
+        w = self.world
+        return int(2 * (w - 1) / w * 240 * self.n) if w > 1 else 0

@@ -7,6 +7,7 @@
  *
  *   grtb200_create / destroy   <- OptixTracer::OptixTracer / ~OptixTracer        (src/optixTracer.cpp:153-343)
  *   grtb200_build_bvh          <- OptixTracer::buildBVH                           (src/optixTracer.cpp:616-890)
+ *   grtb200_build_bvh_packed   the same build from the [N,12] particle record (ours: the no-autograd training step)
  *   grtb200_trace              <- OptixTracer::trace   -> __raygen__rg            (src/optixTracer.cpp:893-960, src/kernels/cuda/referenceOptix.cu:103-186)
  *   grtb200_trace_bwd          <- OptixTracer::traceBwd -> bwd __raygen__rg        (src/optixTracer.cpp:962-1031, src/kernels/cuda/referenceBwdOptix.cu:103-170)
  *
@@ -58,6 +59,11 @@ const char* grtb200_last_error(const grtb200_ctx* ctx);
  * compatibility; every call is a full rebuild (the reference's default config also rebuilds every step). */
 int grtb200_build_bvh(grtb200_ctx* ctx, void* stream, int64_t n, const float* pos, const float* rot, const float* scl,
                       const float* dns, int32_t rebuild, int32_t allow_update);
+
+/* The same build from the [N,12] particle record that grtb200_trace reads (pos = cols 0-2, density = col 3, quat = cols 4-7, scale =
+ * cols 8-10): the same proxies, scene box and LBVH as grtb200_build_bvh on the same values, bit for bit, without copying the four
+ * arrays out first.  Every call is a full rebuild. */
+int grtb200_build_bvh_packed(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles);
 
 int grtb200_trace(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
                   float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,

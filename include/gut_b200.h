@@ -131,6 +131,11 @@ int gutb200_gaussian_adam_step(void* stream, int64_t n, float* const* params6, f
 size_t gutb200_image_loss_scratch_bytes(int32_t height, int32_t width);
 int gutb200_image_loss(void* stream, int32_t height, int32_t width, const float* pred_rgba, const float* target_rgb, float lambda_l1,
                        float lambda_ssim, void* scratch, float* d_rgba, float* sums2);
+/* The same loss on the 3DGRT layout: pred_rgb [H,W,3] (grtb200_trace's out_rgb; alpha takes no part), d_rgb [H,W,3] (directly the d_rgb
+ * of grtb200_trace_bwd).  sums2, the rgb gradient and the scratch contents are bit-identical to gutb200_image_loss on the [H,W,4]
+ * concatenation of rgb and alpha. */
+int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const float* pred_rgb, const float* target_rgb, float lambda_l1,
+                           float lambda_ssim, void* scratch, float* d_rgb, float* sums2);
 
 int gutb200_forward_host(gutb200_ctx* ctx, const gutb200_camera* cam, int64_t n, const float* particles,
                          const float* sph, int32_t sph_degree, const float* rays_o, const float* rays_d,
