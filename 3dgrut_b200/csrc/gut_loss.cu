@@ -14,6 +14,12 @@
 //                       d_rgba argument of gutb200_backward.
 // Both are templated on the pixel strides of the prediction and the gradient, so that gutb200_image_loss_rgb runs the same arithmetic on
 // the 3DGRT layout (rgb [H,W,3] in, d_rgb [H,W,3] out, directly the d_rgb argument of grtb200_trace_bwd).
+//
+// gutb200_image_loss_composited adds the two image-side parts of the training loss (threedgrut/model/background.py:80-93,
+// trainer.py:691-694) where the kernels load x and y, and their chain rule where loss_grad_kernel writes:
+//     x = (rgb + bg (1 - alpha)) m,  y = target m          bg: constant colour or [H,W,3] image; m: optional [H,W] mask
+//     d rgb_c = m dL/dx_c,  d alpha = -sum_c bg_c m dL/dx_c
+// The background mode (BG) and the mask (MASK) are template parameters beside the strides; BG = 0 (black) with no mask is the plain loss.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -32,6 +38,35 @@ struct Window {
     float w[11];
 };
 
+// Extra inputs and outputs of the composited loss; unused (all null) by the plain entries.
+struct Composite {
+    const float* alpha;     // [H,W]: the prediction's alpha when it is not channel 3 of the prediction (PS == 3)
+    const float* bg_image;  // [H,W,3] background (BG == 2)
+    const float* mask;      // [H,W] (MASK)
+    float* d_alpha;         // [H,W]: d loss / d alpha when the gradient has no alpha channel (GS == 3)
+    double* acc;            // [2] fp64 sums of the composited kernels (the head of the scratch), copied to sums2 by loss_grad_kernel
+    float* sums;            // sums2
+    float bg[3];            // constant background (BG == 1)
+};
+
+// x and y of pixel p, channel c, as the loss sees them: the prediction composited onto the background, both multiplied by the mask.
+template <int PS, int BG, bool MASK>
+__device__ __forceinline__ void load_xy(const float* __restrict__ pred, const float* __restrict__ target, const Composite& cp, int64_t p, int c,
+                                        float& x, float& y) {
+    x = pred[p * PS + c];
+    y = target[p * 3 + c];
+    if constexpr (BG != 0) {
+        const float a = PS == 4 ? pred[p * 4 + 3] : cp.alpha[p];
+        const float b = BG == 1 ? cp.bg[c] : cp.bg_image[p * 3 + c];
+        x = x + b * (1.0f - a);
+    }
+    if constexpr (MASK) {
+        const float m = cp.mask[p];
+        x = x * m;
+        y = y * m;
+    }
+}
+
 __device__ __forceinline__ float block_sum(float v, float* scratch) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
@@ -49,9 +84,10 @@ __device__ __forceinline__ float block_sum(float v, float* scratch) {
 }
 
 // PS: floats per pixel of the prediction (4: the 3DGUT [H,W,4] image, 3: the 3DGRT rgb [H,W,3]); only the loads depend on it.
-template <int PS>
+template <int PS, int BG = 0, bool MASK = false>
 __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
-                                                             Window win, float g_scale /* -lambda_ssim / count */, float* __restrict__ dmaps,
+                                                             Composite cp, Window win, float g_scale /* -lambda_ssim / count */,
+                                                             float* __restrict__ dmaps,
                                                              float* __restrict__ sums /* [2]: sum |x-y|, sum of the valid SSIM map */) {
     __shared__ float sx[kS][kS + 1], sy[kS][kS + 1];
     __shared__ float hz[5][kS][kT + 1];
@@ -68,8 +104,10 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
             const int gx = x0 + lx - kR, gy = y0 + ly - kR;
             const bool in = (gx >= 0) && (gy >= 0) && (gx < W) && (gy < H);
             const int64_t p = static_cast<int64_t>(gy) * W + gx;
-            sx[ly][lx] = in ? pred_rgba[p * PS + c] : 0.f;
-            sy[ly][lx] = in ? target[p * 3 + c] : 0.f;
+            float xv = 0.f, yv = 0.f;
+            if (in) load_xy<PS, BG, MASK>(pred_rgba, target, cp, p, c, xv, yv);
+            sx[ly][lx] = xv;
+            sy[ly][lx] = yv;
         }
         __syncthreads();
         // horizontal pass: kS rows x kT columns x 5 quantities
@@ -111,22 +149,34 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
     const float l1_block = block_sum(l1_acc, scratch);
     const float ss_block = block_sum(ssim_acc, scratch);
     if (tid == 0) {
-        atomicAdd(sums + 0, l1_block);
-        atomicAdd(sums + 1, ss_block);
+        if constexpr (BG != 0 || MASK) {  // fp64 totals: the 1e-6 bar of the means holds at 800x800 with masked (partly constant) images
+            atomicAdd(cp.acc + 0, static_cast<double>(l1_block));
+            atomicAdd(cp.acc + 1, static_cast<double>(ss_block));
+        } else {
+            atomicAdd(sums + 0, l1_block);
+            atomicAdd(sums + 1, ss_block);
+        }
     }
 }
 
-// GS: floats per pixel of the gradient (4: d_rgba with a zero alpha gradient, one 16-byte store; 3: d_rgb).
-template <int PS, int GS>
+// GS: floats per pixel of the gradient (4: d_rgba, one 16-byte store, its alpha gradient zero unless BG != 0; 3: d_rgb, plus cp.d_alpha
+// in the composited entry).
+template <int PS, int GS, int BG = 0, bool MASK = false>
 __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
-                                                            Window win, float l1_scale /* lambda_l1 / (H W 3) */, const float* __restrict__ dmaps,
-                                                            float* __restrict__ d_rgba) {
+                                                            Composite cp, Window win, float l1_scale /* lambda_l1 / (H W 3) */,
+                                                            const float* __restrict__ dmaps, float* __restrict__ d_rgba) {
     __shared__ float sm[3][kS][kS + 1];
     __shared__ float hz[3][kS][kT + 1];
     const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * kT + tx;
     const int x0 = blockIdx.x * kT, y0 = blockIdx.y * kT;
     const int px = x0 + tx, py = y0 + ty;
     const bool inside = (px < W) && (py < H);
+    if constexpr (BG != 0 || MASK) {
+        if (blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) {  // every block of ssim_stats_kernel has finished (stream order)
+            cp.sums[0] = static_cast<float>(cp.acc[0]);
+            cp.sums[1] = static_cast<float>(cp.acc[1]);
+        }
+    }
     float grad[3] = {0.f, 0.f, 0.f};
     for (int c = 0; c < 3; ++c) {
         for (int i = tid; i < kS * kS; i += kT * kT) {
@@ -158,7 +208,8 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
         }
         if (inside) {
             const int64_t p = static_cast<int64_t>(py) * W + px;
-            const float xv = pred_rgba[p * PS + c], yv = target[p * 3 + c];
+            float xv, yv;
+            load_xy<PS, BG, MASK>(pred_rgba, target, cp, p, c, xv, yv);
             const float diff = xv - yv;
             const float sgn = diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f);
             grad[c] = c0 + 2.f * xv * c1 + yv * c2 + l1_scale * sgn;
@@ -167,18 +218,30 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
     }
     if (!inside) return;
     const int64_t p = static_cast<int64_t>(py) * W + px;
+    // chain rule through the mask and the composite: grad is d loss / d x of the masked composite
+    if constexpr (MASK) {
+        const float m = cp.mask[p];
+        grad[0] *= m; grad[1] *= m; grad[2] *= m;
+    }
+    float d_alpha = 0.f;
+    if constexpr (BG == 1) d_alpha = -(cp.bg[0] * grad[0] + cp.bg[1] * grad[1] + cp.bg[2] * grad[2]);
+    if constexpr (BG == 2) {
+        const float* b = cp.bg_image + p * 3;
+        d_alpha = -(b[0] * grad[0] + b[1] * grad[1] + b[2] * grad[2]);
+    }
     if (GS == 4) {
-        reinterpret_cast<float4*>(d_rgba)[p] = make_float4(grad[0], grad[1], grad[2], 0.f);
+        reinterpret_cast<float4*>(d_rgba)[p] = make_float4(grad[0], grad[1], grad[2], d_alpha);
     } else {
         d_rgba[p * GS + 0] = grad[0];
         d_rgba[p * GS + 1] = grad[1];
         d_rgba[p * GS + 2] = grad[2];
+        if constexpr (BG != 0 || MASK) cp.d_alpha[p] = d_alpha;
     }
 }
 
-template <int PS, int GS>
+template <int PS, int GS, int BG = 0, bool MASK = false>
 int image_loss(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1, float lambda_ssim,
-               void* scratch, float* d_pred, float* sums2) {
+               void* scratch, float* d_pred, float* sums2, Composite cp = Composite{}) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     Window win;
     double g[11], total = 0.0;
@@ -189,13 +252,43 @@ int image_loss(void* stream, int32_t height, int32_t width, const float* pred, c
     }
     for (int i = 0; i < 11; ++i) win.w[i] = static_cast<float>(g[i] / total);
     const double count = (height > 10 && width > 10) ? static_cast<double>(height - 10) * (width - 10) * 3.0 : 1.0;
-    if (cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s) != cudaSuccess) return 2;
     const dim3 block(kT, kT), grid((width + kT - 1) / kT, (height + kT - 1) / kT);
     float* dmaps = static_cast<float*>(scratch);
-    ssim_stats_kernel<PS><<<grid, block, 0, s>>>(height, width, pred, target_rgb, win, static_cast<float>(-lambda_ssim / count), dmaps, sums2);
-    loss_grad_kernel<PS, GS><<<grid, block, 0, s>>>(height, width, pred, target_rgb, win,
-                                                    static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)), dmaps, d_pred);
+    if constexpr (BG != 0 || MASK) {
+        // the composited kernels keep their two sums in fp64 at the head of the scratch (its 16 spare bytes), the maps after them
+        cp.acc = static_cast<double*>(scratch);
+        cp.sums = sums2;
+        dmaps = reinterpret_cast<float*>(static_cast<char*>(scratch) + 16);
+        if (cudaMemsetAsync(cp.acc, 0, 2 * sizeof(double), s) != cudaSuccess) return 2;
+    } else {
+        if (cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s) != cudaSuccess) return 2;
+    }
+    ssim_stats_kernel<PS, BG, MASK><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win, static_cast<float>(-lambda_ssim / count),
+                                                           dmaps, sums2);
+    loss_grad_kernel<PS, GS, BG, MASK><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win,
+                                                              static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)), dmaps,
+                                                              d_pred);
     return cudaGetLastError() == cudaSuccess ? 0 : 2;
+}
+
+template <int L>
+int image_loss_composited(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1,
+                          float lambda_ssim, void* scratch, float* d_pred, float* sums2, const Composite& cp, int bg_mode, bool mask) {
+    if (bg_mode == 0 && !mask) {
+        // black, no mask: the plain loss; the split layout's alpha gradient is zero
+        if (L == 3 && cudaMemsetAsync(cp.d_alpha, 0, static_cast<size_t>(height) * width * sizeof(float), static_cast<cudaStream_t>(stream)) != cudaSuccess)
+            return 2;
+        return image_loss<L, L>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2);
+    }
+#define GUT_LOSS_CASE(BG_, M_) \
+    if (bg_mode == BG_ && mask == M_) return image_loss<L, L, BG_, M_>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp);
+    GUT_LOSS_CASE(0, true)
+    GUT_LOSS_CASE(1, false)
+    GUT_LOSS_CASE(1, true)
+    GUT_LOSS_CASE(2, false)
+    GUT_LOSS_CASE(2, true)
+#undef GUT_LOSS_CASE
+    return 1;
 }
 
 }  // namespace
@@ -220,6 +313,37 @@ int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const fl
                            float lambda_ssim, void* scratch, float* d_rgb, float* sums2) {
     if (height <= 0 || width <= 0 || !pred_rgb || !target_rgb || !scratch || !d_rgb || !sums2) return 1;
     return gutb200::image_loss<3, 3>(stream, height, width, pred_rgb, target_rgb, lambda_l1, lambda_ssim, scratch, d_rgb, sums2);
+}
+
+// The loss on the composited, masked prediction (see the top of this file), for either layout:
+//   layout 4: pred [H,W,4] rgba, d_pred [H,W,4] = d_rgba with its alpha gradient (16-byte aligned); pred_alpha / d_alpha unused
+//   layout 3: pred [H,W,3] rgb + pred_alpha [H,W], d_pred [H,W,3] = d_rgb + d_alpha [H,W]
+// background_rgb: 3 host floats, or NULL (black); background_image: [H,W,3] device image (takes precedence), or NULL.  A black background
+// is skipped entirely: no alpha gradient.  mask: [H,W] device floats, or NULL.
+int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                                  const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                                  float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2) {
+    if (height <= 0 || width <= 0 || !pred || !target_rgb || !scratch || !d_pred || !sums2) return 1;
+    if (layout != 3 && layout != 4) return 1;
+    if (layout == 3 && (!pred_alpha || !d_alpha)) return 1;
+    if (layout == 4 && (reinterpret_cast<uintptr_t>(d_pred) & 15) != 0) return 3;
+    gutb200::Composite cp{};
+    cp.alpha = pred_alpha;
+    cp.d_alpha = d_alpha;
+    cp.mask = mask;
+    int bg_mode = 0;
+    if (background_image) {
+        cp.bg_image = background_image;
+        bg_mode = 2;
+    } else if (background_rgb && (background_rgb[0] != 0.f || background_rgb[1] != 0.f || background_rgb[2] != 0.f)) {
+        for (int c = 0; c < 3; ++c) cp.bg[c] = background_rgb[c];
+        bg_mode = 1;
+    }
+    if (layout == 4)
+        return gutb200::image_loss_composited<4>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp,
+                                                 bg_mode, mask != nullptr);
+    return gutb200::image_loss_composited<3>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp, bg_mode,
+                                             mask != nullptr);
 }
 
 }  // extern "C"

@@ -9,6 +9,9 @@
 //                           autograd (threedgrut/model/model.py:102-118 with utils/misc.py:46-50: density = sigmoid(raw),
 //                           scale = exp(raw), rotation = normalize(raw)) followed by the Adam update, either torch.optim.Adam's
 //                           (bias-corrected, model.py:807-810) or the selective one.
+// gutb200_gaussian_adam_step_reg adds the opacity and scale regularisers of the reference loss (trainer.py:722-736:
+// lambda_opacity mean|sigmoid(raw density)| + lambda_scale mean|exp(raw scale)|) to the activated density / scale gradients before the
+// chain rule: + lambda_opacity / N and + lambda_scale / (3 N).  They are a template flag (REG) of the kernel, so the plain entry is unchanged.
 // Both are streaming kernels: every byte is read and written once, coalesced (element-wise index space; the quaternion rows as
 // float4).  Algorithmic bytes per Gaussian of the fused step: 59 x (4 param r + 4 param w + 8 moments r + 8 moments w) + 240
 // gradient + 4 visibility = 1660 B.
@@ -59,23 +62,31 @@ struct GaussianAdamArgs {
     const float* visibility;   // [N] float bits (the renderer's output) or nullptr
     int64_t n;
     AdamHyper h;
+    float reg_density;         // lambda_opacity / N, added to d density (REG only)
+    float reg_scale;           // lambda_scale / (3 N), added to every d scale (REG only)
 };
 
 // gradient of element (row, col) of group G w.r.t. the RAW parameter value p
-template <int G>
+template <int G, bool REG>
 __device__ __forceinline__ float raw_gradient(const GaussianAdamArgs& a, int64_t row, int col, float p) {
     if (G == 0) return a.d_particles[row * 12 + col];
     if (G == 1) {
         const float s = 1.0f / (1.0f + expf(-p));   // density = sigmoid(raw)
-        return a.d_particles[row * 12 + 3] * s * (1.0f - s);
+        float g = a.d_particles[row * 12 + 3];
+        if constexpr (REG) g = g + a.reg_density;
+        return g * s * (1.0f - s);
     }
-    if (G == 3) return a.d_particles[row * 12 + 8 + col] * expf(p);   // scale = exp(raw)
+    if (G == 3) {
+        float g = a.d_particles[row * 12 + 8 + col];
+        if constexpr (REG) g = g + a.reg_scale;
+        return g * expf(p);   // scale = exp(raw)
+    }
     if (G == 4) return a.d_sph[row * 48 + col];                        // features = cat(albedo [N,3], specular [N,45])  (model.py:94-96)
     return a.d_sph[row * 48 + 3 + col];
 }
 
 // flat groups: a thread owns 4 consecutive floats of the [N*W] array (16-byte loads and stores of param / moments)
-template <int G, int W>
+template <int G, int W, bool REG>
 __device__ __forceinline__ void flat_group(const GaussianAdamArgs& a, int64_t t) {
     const int64_t total = a.n * W, e0 = t * 4;
     if (e0 >= total) return;
@@ -94,7 +105,7 @@ __device__ __forceinline__ void flat_group(const GaussianAdamArgs& a, int64_t t)
             const int col = static_cast<int>(e - row * W);
             if (masked && (__float_as_uint(a.visibility[row]) == 0u)) continue;
             any = true;
-            pe[k] = adam_update(pe[k], raw_gradient<G>(a, row, col, pe[k]), me[k], ve[k], lr, a.h);
+            pe[k] = adam_update(pe[k], raw_gradient<G, REG>(a, row, col, pe[k]), me[k], ve[k], lr, a.h);
         }
         if (!any) return;  // nothing visible: leave the 48 bytes alone
         *reinterpret_cast<float4*>(P) = make_float4(pe[0], pe[1], pe[2], pe[3]);
@@ -107,13 +118,14 @@ __device__ __forceinline__ void flat_group(const GaussianAdamArgs& a, int64_t t)
             if (masked && (__float_as_uint(a.visibility[row]) == 0u)) continue;
             float m = a.m[G][e], v = a.v[G][e];
             const float p = a.param[G][e];
-            a.param[G][e] = adam_update(p, raw_gradient<G>(a, row, col, p), m, v, lr, a.h);
+            a.param[G][e] = adam_update(p, raw_gradient<G, REG>(a, row, col, p), m, v, lr, a.h);
             a.m[G][e] = m;
             a.v[G][e] = v;
         }
     }
 }
 
+template <bool REG>
 __global__ void __launch_bounds__(256, 4) gaussian_adam_kernel(GaussianAdamArgs a) {
     const unsigned blk = blockIdx.x;
     int group = 0;
@@ -122,11 +134,11 @@ __global__ void __launch_bounds__(256, 4) gaussian_adam_kernel(GaussianAdamArgs 
     const unsigned first = group == 0 ? 0u : a.block_end[group - 1];
     const int64_t t = static_cast<int64_t>(blk - first) * blockDim.x + threadIdx.x;
     switch (group) {
-        case 0: flat_group<0, 3>(a, t); break;
-        case 1: flat_group<1, 1>(a, t); break;
-        case 3: flat_group<3, 3>(a, t); break;
-        case 4: flat_group<4, 3>(a, t); break;
-        case 5: flat_group<5, 45>(a, t); break;
+        case 0: flat_group<0, 3, REG>(a, t); break;
+        case 1: flat_group<1, 1, REG>(a, t); break;
+        case 3: flat_group<3, 3, REG>(a, t); break;
+        case 4: flat_group<4, 3, REG>(a, t); break;
+        case 5: flat_group<5, 45, REG>(a, t); break;
         default: {
             // rotation = normalize(raw): d raw = (g - q (q . g)) / max(|raw|, 1e-12)   (torch.nn.functional.normalize, eps 1e-12)
             const int64_t row = t;
@@ -167,6 +179,45 @@ AdamHyper make_hyper(float b1, float b2, float eps, int64_t step, int selective)
     return h;
 }
 
+int gaussian_adam_step(void* stream, int64_t n, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6, const float* lr6,
+                       float b1, float b2, float eps, int64_t step, int32_t selective, const float* d_particles, const float* d_sph,
+                       const float* visibility, float reg_density, float reg_scale) {
+    if (n < 0 || !params6 || !exp_avg6 || !exp_avg_sq6 || !lr6 || !d_particles || !d_sph) return 1;
+    if (!selective && step < 1) return 1;
+    if (n == 0) return 0;
+    GaussianAdamArgs a;
+    for (int k = 0; k < 6; ++k) {
+        if (!params6[k] || !exp_avg6[k] || !exp_avg_sq6[k]) return 1;
+        a.param[k] = params6[k];
+        a.m[k] = exp_avg6[k];
+        a.v[k] = exp_avg_sq6[k];
+        a.lr[k] = lr6[k];
+    }
+    for (int k = 0; k < 6; ++k) {  // parameters and moments are accessed 16 bytes at a time
+        if ((reinterpret_cast<uintptr_t>(a.param[k]) | reinterpret_cast<uintptr_t>(a.m[k]) | reinterpret_cast<uintptr_t>(a.v[k])) & 15) return 3;
+    }
+    if (reinterpret_cast<uintptr_t>(d_particles) & 15) return 3;
+    a.d_particles = d_particles;
+    a.d_sph = d_sph;
+    a.visibility = visibility;
+    a.n = n;
+    a.h = make_hyper(b1, b2, eps, step, selective);
+    a.reg_density = reg_density;
+    a.reg_scale = reg_scale;
+    const int widths[6] = {3, 1, 4, 3, 3, 45};
+    unsigned blocks = 0;
+    for (int k = 0; k < 6; ++k) {
+        const int64_t threads = k == 2 ? n : (n * widths[k] + 3) / 4;  // rotation: one row per thread; flat groups: 4 floats per thread
+        blocks += static_cast<unsigned>((threads + 255) / 256);
+        a.block_end[k] = blocks;
+    }
+    if (reg_density == 0.f && reg_scale == 0.f)
+        gaussian_adam_kernel<false><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    else
+        gaussian_adam_kernel<true><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    return cudaGetLastError() == cudaSuccess ? 0 : 2;
+}
+
 }  // namespace
 
 }  // namespace gutb200
@@ -190,36 +241,15 @@ int gutb200_selective_adam_update(void* stream, float* param, const float* grad,
 int gutb200_gaussian_adam_step(void* stream, int64_t n, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6,
                                const float* lr6, float b1, float b2, float eps, int64_t step, int32_t selective, const float* d_particles,
                                const float* d_sph, const float* visibility) {
-    using namespace gutb200;
-    if (n < 0 || !params6 || !exp_avg6 || !exp_avg_sq6 || !lr6 || !d_particles || !d_sph) return 1;
-    if (!selective && step < 1) return 1;
-    if (n == 0) return 0;
-    GaussianAdamArgs a;
-    for (int k = 0; k < 6; ++k) {
-        if (!params6[k] || !exp_avg6[k] || !exp_avg_sq6[k]) return 1;
-        a.param[k] = params6[k];
-        a.m[k] = exp_avg6[k];
-        a.v[k] = exp_avg_sq6[k];
-        a.lr[k] = lr6[k];
-    }
-    for (int k = 0; k < 6; ++k) {  // parameters and moments are accessed 16 bytes at a time
-        if ((reinterpret_cast<uintptr_t>(a.param[k]) | reinterpret_cast<uintptr_t>(a.m[k]) | reinterpret_cast<uintptr_t>(a.v[k])) & 15) return 3;
-    }
-    if (reinterpret_cast<uintptr_t>(d_particles) & 15) return 3;
-    a.d_particles = d_particles;
-    a.d_sph = d_sph;
-    a.visibility = visibility;
-    a.n = n;
-    a.h = make_hyper(b1, b2, eps, step, selective);
-    const int widths[6] = {3, 1, 4, 3, 3, 45};
-    unsigned blocks = 0;
-    for (int k = 0; k < 6; ++k) {
-        const int64_t threads = k == 2 ? n : (n * widths[k] + 3) / 4;  // rotation: one row per thread; flat groups: 4 floats per thread
-        blocks += static_cast<unsigned>((threads + 255) / 256);
-        a.block_end[k] = blocks;
-    }
-    gaussian_adam_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
-    return cudaGetLastError() == cudaSuccess ? 0 : 2;
+    return gutb200::gaussian_adam_step(stream, n, params6, exp_avg6, exp_avg_sq6, lr6, b1, b2, eps, step, selective, d_particles, d_sph,
+                                       visibility, 0.f, 0.f);
+}
+
+int gutb200_gaussian_adam_step_reg(void* stream, int64_t n, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6,
+                                   const float* lr6, float b1, float b2, float eps, int64_t step, int32_t selective, const float* d_particles,
+                                   const float* d_sph, const float* visibility, float reg_density, float reg_scale) {
+    return gutb200::gaussian_adam_step(stream, n, params6, exp_avg6, exp_avg_sq6, lr6, b1, b2, eps, step, selective, d_particles, d_sph,
+                                       visibility, reg_density, reg_scale);
 }
 
 }  // extern "C"

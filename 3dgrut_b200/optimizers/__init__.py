@@ -26,6 +26,8 @@ def _lib():
         lib.gutb200_gaussian_adam_step.argtypes = [vp, i64, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(f32), f32, f32, f32, i64, i32,
                                                    vp, vp, vp]
         lib.gutb200_gaussian_adam_step.restype = C.c_int
+        lib.gutb200_gaussian_adam_step_reg.argtypes = lib.gutb200_gaussian_adam_step.argtypes + [f32, f32]
+        lib.gutb200_gaussian_adam_step_reg.restype = C.c_int
         lib._optim_bound = True
     return lib
 
@@ -83,7 +85,9 @@ class FusedGaussianAdam:
 
     params: dict name -> raw (pre-activation) leaf tensor for the six GROUPS; lrs: dict name -> learning rate (mutable: schedulers
     write `opt.lrs["positions"] = ...`).  step(d_particles, d_sph, visibility=None) consumes the renderer's gradients
-    (Tracer / SplatRaster.trace_bwd outputs, or the view-parallel exchange's) -- no autograd pass over the activations is needed."""
+    (Tracer / SplatRaster.trace_bwd outputs, or the view-parallel exchange's) -- no autograd pass over the activations is needed.
+    lambda_opacity / lambda_scale add the reference's regularisers lambda_opacity mean(sigmoid(density)) + lambda_scale mean(exp(scale))
+    (trainer.py:722-736) to the gradient inside the same launch."""
 
     def __init__(self, params: dict, lrs: dict, betas=(0.9, 0.999), eps=1e-15, selective=False):
         # the dict itself is kept (not copied) when it holds exactly the six groups: densification replaces the tensors inside it
@@ -115,7 +119,8 @@ class FusedGaussianAdam:
         return arr
 
     @torch.no_grad()
-    def step(self, d_particles: torch.Tensor, d_sph: torch.Tensor, visibility: torch.Tensor | None = None):
+    def step(self, d_particles: torch.Tensor, d_sph: torch.Tensor, visibility: torch.Tensor | None = None, lambda_opacity: float = 0.0,
+             lambda_scale: float = 0.0):
         _check(d_particles, "d_particles")
         _check(d_sph, "d_sph")
         self._validate()  # the tensors may have been replaced (densification); moments must have followed
@@ -138,9 +143,13 @@ class FusedGaussianAdam:
         dev = d_particles.device
         lr = (C.c_float * 6)(*[self.lrs[k] for k in GROUPS])
         stream = torch.cuda.current_stream(dev).cuda_stream
+        args = (stream, self.n, self._array({k: t.data for k, t in self.params.items()}), self._array(self.exp_avg), self._array(self.exp_avg_sq),
+                lr, self.betas[0], self.betas[1], self.eps, self.steps, int(self.selective), d_particles.data_ptr(), d_sph.data_ptr(), vis_ptr)
+        if lambda_opacity == 0.0 and lambda_scale == 0.0:
+            entry, extra = "gutb200_gaussian_adam_step", ()
+        else:  # d mean(sigmoid(raw)) / d density = 1 / N, d mean(exp(raw)) / d scale = 1 / (3 N)
+            entry, extra = "gutb200_gaussian_adam_step_reg", (float(lambda_opacity) / max(self.n, 1), float(lambda_scale) / (3 * max(self.n, 1)))
         with torch.cuda.device(dev):
-            rc = _lib().gutb200_gaussian_adam_step(stream, self.n, self._array({k: t.data for k, t in self.params.items()}),
-                                                   self._array(self.exp_avg), self._array(self.exp_avg_sq), lr, self.betas[0], self.betas[1],
-                                                   self.eps, self.steps, int(self.selective), d_particles.data_ptr(), d_sph.data_ptr(), vis_ptr)
+            rc = getattr(_lib(), entry)(*args, *extra)
         if rc != 0:
-            raise RuntimeError(f"gutb200_gaussian_adam_step failed ({rc})")
+            raise RuntimeError(f"{entry} failed ({rc})")

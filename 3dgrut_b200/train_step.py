@@ -4,8 +4,10 @@ Replaces the render + backward + optimizer part of Trainer.run_train_iter (three
 repository wired together -- no autograd graph, no per-parameter all-reduce, no separate activation backward:
 
     activations (sigmoid / exp / normalize, model.py:102-118)  ->  SplatRaster.trace
-    -> loss gradient on the image (L1, trainer.py:698-704 + losses.py:20-21)  ->  SplatRaster.trace_bwd_compact
-    -> CompactGradientExchange (all-reduce [N,12], all-gather [N,4], rebuild [N,48])  ->  FusedGaussianAdam.step
+    -> loss gradient on the image (L1, trainer.py:698-704 + losses.py:20-21; or L1 + SSIM, with the background composited and the mask
+       applied, by losses.image_loss)  ->  SplatRaster.trace_bwd_compact
+    -> CompactGradientExchange (all-reduce [N,12], all-gather [N,4], rebuild [N,48])  ->  FusedGaussianAdam.step (+ the opacity and
+       scale regularisers, once per step after the exchange)
 
 Every rank holds a replica of the parameters and renders its own camera of the step's batch; the loss is normalised by the global
 batch (number of ranks), so the replicas stay identical.  The trainer, datasets, densification and logging of the reference stay out
@@ -16,6 +18,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+import losses
 import optimizers
 import view_parallel
 from threedgut_tracer.tracer import SplatRaster
@@ -23,10 +26,13 @@ from threedgut_tracer.tracer import SplatRaster
 
 class GaussianTrainStep:
     def __init__(self, params: dict, lrs: dict, conf=None, sph_degree: int = 3, selective: bool = False, group=None, eps: float = 1e-15,
-                 densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0):
+                 densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0, background="black",
+                 background_seed: int = 0, lambda_opacity: float = 0.0, lambda_scale: float = 0.0):
         """params: raw leaf tensors for optimizers.GROUPS (positions, density, rotation, scale, features_albedo, features_specular).
         densify_conf: a densify.DensifyConfig (GS strategy: clone / split / prune / reset) or densify.MCMCConfig (relocate / add / perturb)
-        turns on the replica-consistent strategy."""
+        turns on the replica-consistent strategy.  background: "black", "white", "random" or (r, g, b), composited onto the render before
+        the loss (model.background.color); "random" draws from a generator seeded background_seed + rank.  lambda_opacity / lambda_scale:
+        the regularisers of the loss (loss.lambda_opacity / loss.lambda_scale when use_opacity / use_scale)."""
         self.params = {k: params[k] for k in optimizers.GROUPS}  # ONE dict shared with the optimizer and the densifier
         self.device = self.params["positions"].device
         self.sph_degree = int(sph_degree)
@@ -37,6 +43,9 @@ class GaussianTrainStep:
         self.exchange = view_parallel.CompactGradientExchange(self.raster, self.n, self.device, group=group)
         self.frame = 0
         self.lambda_l1, self.lambda_ssim = float(lambda_l1), float(lambda_ssim)  # reference defaults: 0.8 / 0.2 (configs/base_gs.yaml:172-179)
+        self.lambda_opacity, self.lambda_scale = float(lambda_opacity), float(lambda_scale)
+        rank = dist.get_rank(group) if self.world > 1 else 0
+        self.background = losses.Background(background, seed=int(background_seed) + rank, device=self.device)
         self.scene_extent = float(scene_extent)
         self.densifier = None
         if densify_conf is not None:
@@ -66,15 +75,21 @@ class GaussianTrainStep:
         return rgba, dist_, hits, vis
 
     @torch.no_grad()
-    def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None):
+    def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view.  target_rgb: [H,W,3].  all_sensor_positions: [world,3] sensor positions of every
-        rank's view of this step in rank order (omit on a single GPU).  Returns this view's loss (a device scalar)."""
+        rank's view of this step in rank order (omit on a single GPU).  mask: optional [H,W] ([H,W,1], [1,H,W,1]) float CUDA tensor that
+        multiplies prediction and target before the loss.  Returns this view's loss (a device scalar), the regularisers included."""
         H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
+        if mask is not None:
+            mask = losses.mask_hw(mask, H, W)
         particles, sph = self.activated()
         rgba, dst, hits, vis = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
-        if self.lambda_ssim != 0.0:
-            import losses
-
+        if not self.background.black or mask is not None:
+            # composited onto the background, masked; d_rgba carries the alpha gradient (gut_loss.cu); global-batch normalisation
+            loss, _, _, d_rgba = losses.image_loss(rgba, target_rgb.contiguous(), self.lambda_l1 / self.world, self.lambda_ssim / self.world,
+                                                   background=self.background.draw(H, W), mask=mask)
+            loss = loss * self.world
+        elif self.lambda_ssim != 0.0:
             # lambda_l1 L1 + lambda_ssim (1 - SSIM) and its image gradient in two launches (gut_loss.cu); global-batch normalisation
             loss, _, _, d_rgba = losses.image_loss(rgba, target_rgb.contiguous(), self.lambda_l1 / self.world, self.lambda_ssim / self.world)
             loss = loss * self.world
@@ -98,7 +113,12 @@ class GaussianTrainStep:
         d_particles, d_sph = self.exchange.exchange(self.sph_degree, particles, np.asarray(all_sensor_positions, np.float32))
         if self.optimizer.selective and self.world > 1:
             dist.all_reduce(vis, op=dist.ReduceOp.MAX, group=self.group)  # visible in any view of the batch (SURVEY 8e)
-        self.optimizer.step(d_particles, d_sph, visibility=vis if self.optimizer.selective else None)
+        # the regularisers belong to the step once (every rank holds the same parameters): added after the exchange, no 1 / world
+        reg = {}
+        if self.lambda_opacity != 0.0 or self.lambda_scale != 0.0:
+            loss = loss + regulariser_loss(particles, self.lambda_opacity, self.lambda_scale)
+            reg = dict(lambda_opacity=self.lambda_opacity, lambda_scale=self.lambda_scale)
+        self.optimizer.step(d_particles, d_sph, visibility=vis if self.optimizer.selective else None, **reg)
         self.frame += 1
         if self.densifier is not None and self.densifier.post_optimizer_step(self.frame, self.scene_extent, positions_lr=self.optimizer.lrs["positions"]):
             # the number of Gaussians may have changed (identically on every rank): re-capacity the exchange buffers; the renderer's
@@ -106,3 +126,13 @@ class GaussianTrainStep:
             if self.exchange.n != self.n:
                 self.exchange = view_parallel.CompactGradientExchange(self.raster, self.n, self.device, group=self.group)
         return loss
+
+
+def regulariser_loss(particles, lambda_opacity: float, lambda_scale: float):
+    """lambda_opacity mean|density| + lambda_scale mean|scale| on the activated [N,12] record (trainer.py:722-736); 0 when both are 0."""
+    reg = 0.0
+    if lambda_opacity != 0.0:
+        reg = reg + lambda_opacity * particles[:, 3].abs().mean()
+    if lambda_scale != 0.0:
+        reg = reg + lambda_scale * particles[:, 8:11].abs().mean()
+    return reg

@@ -122,6 +122,12 @@ int gutb200_selective_adam_update(void* stream, float* param, const float* grad,
 int gutb200_gaussian_adam_step(void* stream, int64_t n, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6,
                                const float* lr6, float b1, float b2, float eps, int64_t step, int32_t selective, const float* d_particles,
                                const float* d_sph, const float* visibility);
+/* The same step with the opacity and scale regularisers of the reference loss (threedgrut/trainer.py:722-736): reg_density =
+ * lambda_opacity / n is added to every d density and reg_scale = lambda_scale / (3 n) to every d scale (w.r.t. the activated values)
+ * before the chain rule.  Both zero: exactly gutb200_gaussian_adam_step.  The selective rule still skips invisible rows. */
+int gutb200_gaussian_adam_step_reg(void* stream, int64_t n, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6,
+                                   const float* lr6, float b1, float b2, float eps, int64_t step, int32_t selective, const float* d_particles,
+                                   const float* d_sph, const float* visibility, float reg_density, float reg_scale);
 
 /* Image loss of the training step and its gradient (SURVEY.md 8f row 3): loss = lambda_l1 mean|x - y| + lambda_ssim (1 - SSIM(x, y))
  * (threedgrut/trainer.py:698-739, model/losses.py:20-33 -> fused_ssim(..., padding="valid"), third-party fused-ssim @ 1272e21).
@@ -136,6 +142,15 @@ int gutb200_image_loss(void* stream, int32_t height, int32_t width, const float*
  * concatenation of rgb and alpha. */
 int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const float* pred_rgb, const float* target_rgb, float lambda_l1,
                            float lambda_ssim, void* scratch, float* d_rgb, float* sums2);
+/* The loss on the prediction composited onto a background and multiplied by a mask (threedgrut/model/background.py:80-93,
+ * trainer.py:691-694): x = (rgb + bg (1 - alpha)) m, y = target m.  layout 4: pred [H,W,4] rgba and d_pred [H,W,4] = d_rgba with a live
+ * alpha gradient (16-byte aligned; pred_alpha / d_alpha unused); layout 3: pred [H,W,3] rgb + pred_alpha [H,W] and d_pred [H,W,3] = d_rgb
+ * + d_alpha [H,W] (the d_rgb / d_alpha of grtb200_trace_bwd).  background_rgb: 3 host floats or NULL (black); background_image: [H,W,3]
+ * device floats or NULL (used instead of background_rgb when given); black is skipped (zero alpha gradient).  mask: [H,W] or NULL.
+ * d rgb = m dL/dx, d alpha = -sum_c bg_c m dL/dx_c.  Black with no mask runs gutb200_image_loss / _rgb's kernels. */
+int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                                  const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                                  float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2);
 
 int gutb200_forward_host(gutb200_ctx* ctx, const gutb200_camera* cam, int64_t n, const float* particles,
                          const float* sph, int32_t sph_degree, const float* rays_o, const float* rays_d,
