@@ -332,3 +332,47 @@ class GrtContext:
 
     def launch_count(self) -> int:
         return int(self._lib.grtb200_launch_count(self._h))
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# include/nht_b200.h (NHT feature decoder: fused tensor-core MLP), same shared library
+
+class NhtConfig(C.Structure):
+    """nhtb200_config"""
+
+    _fields_ = [("n_features", C.c_int32), ("sh_degree", C.c_int32), ("n_hidden_layers", C.c_int32), ("width", C.c_int32),
+                ("output_activation", C.c_int32), ("sh_scale", C.c_float)]
+
+
+# nhtb200_config.output_activation (FeatureDecoder output_activation)
+NHT_ACTIVATIONS = {"None": 0, "ReLU": 1, "Sigmoid": 2}
+NHT_UNSUPPORTED = 1
+
+NHT_EXPORTS = ["nhtb200_last_error", "nhtb200_n_params", "nhtb200_backward_workspace_bytes", "nhtb200_forward", "nhtb200_backward"]
+
+
+def nht_lib():
+    lib = load()
+    if not getattr(lib, "_nht_ready", False):
+        vp, i64 = C.c_void_p, C.c_int64
+        cfg = C.POINTER(NhtConfig)
+        lib.nhtb200_last_error.restype = C.c_char_p
+        lib.nhtb200_last_error.argtypes = []
+        lib.nhtb200_n_params.restype = i64
+        lib.nhtb200_n_params.argtypes = [cfg]
+        lib.nhtb200_backward_workspace_bytes.restype = C.c_size_t
+        lib.nhtb200_backward_workspace_bytes.argtypes = [cfg, i64]
+        lib.nhtb200_forward.argtypes = [cfg, vp, i64, vp, vp, vp, vp]
+        lib.nhtb200_backward.argtypes = [cfg, vp, i64, vp, vp, vp, vp, vp, vp, vp]
+        lib._nht_ready = True
+    return lib
+
+
+def nht_check(rc: int, what: str):
+    """Raise for a non-zero nhtb200_* return code: NotImplementedError for a configuration that is not built."""
+    if rc == 0:
+        return
+    msg = f"{what}: {nht_lib().nhtb200_last_error().decode()}"
+    if rc == NHT_UNSUPPORTED:
+        raise NotImplementedError(msg)
+    raise RuntimeError(msg)

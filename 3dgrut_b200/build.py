@@ -30,6 +30,8 @@ UNITS = {
     "gut_optim.cu": [],
     "gut_loss.cu": [],
     "gut_debug.cu": [],
+    # NHT feature decoder: fp16 tensor-core MLP, IEEE fp32 encoding and epilogues
+    "nht_decoder.cu": [],
 }
 
 
@@ -41,7 +43,8 @@ def _nvcc() -> str:
 
 
 def sources():
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "gut_b200.h"), os.path.join(HERE, "..", "include", "grt_b200.h"), os.path.abspath(__file__)]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "gut_b200.h"), os.path.join(HERE, "..", "include", "grt_b200.h"),
+                                                                os.path.join(HERE, "..", "include", "nht_b200.h"), os.path.abspath(__file__)]
     return deps
 
 
