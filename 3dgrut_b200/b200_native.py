@@ -1,5 +1,5 @@
-"""ctypes binding of include/gut_b200.h (libgut_b200.so).  There is NO CPU or PyTorch fallback: if the CUDA
-extension cannot be built/loaded, or no GPU is present when a context is created, this raises."""
+"""ctypes binding of include/gut_b200.h, grt_b200.h and nht_b200.h (one shared library, libgut_b200.so).  There is NO CPU or PyTorch
+fallback: if the CUDA extension cannot be built/loaded, or no GPU is present when a context is created, this raises."""
 from __future__ import annotations
 
 import ctypes as C
@@ -38,15 +38,89 @@ class Config(C.Structure):
     ]
 
 
-EXPORTS = [
-    "gutb200_version", "gutb200_default_config", "gutb200_create", "gutb200_destroy", "gutb200_last_error",
-    "gutb200_forward", "gutb200_backward", "gutb200_forward_host", "gutb200_backward_host", "gutb200_last_stats",
-    "gutb200_debug_copy", "gutb200_collect_times", "gutb200_collect_stage_times", "gutb200_set_timings", "gutb200_launch_count",
-    "gutb200_backward_compact", "gutb200_sph_grad_from_views", "gutb200_camera_position",
-    "gutb200_debug_work_counters", "gutb200_debug_fma_peak",
-    "gutb200_selective_adam_update", "gutb200_gaussian_adam_step", "gutb200_gaussian_adam_step_reg",  # bound in optimizers/__init__.py
-    "gutb200_image_loss_scratch_bytes", "gutb200_image_loss", "gutb200_image_loss_rgb", "gutb200_image_loss_composited",  # bound in losses.py
-]
+class GrtConfig(C.Structure):
+    """grtb200_config"""
+
+    _fields_ = [("kernel_degree", C.c_int32), ("min_response", C.c_float), ("min_alpha", C.c_float), ("max_alpha", C.c_float),
+                ("density_clamping", C.c_int32), ("primitive", C.c_int32)]
+
+
+# grtb200_config.primitive (render.primitive_type)
+GRT_PRIMITIVES = {"instances": 0, "icosahedron": 1}
+
+
+class NhtConfig(C.Structure):
+    """nhtb200_config"""
+
+    _fields_ = [("n_features", C.c_int32), ("sh_degree", C.c_int32), ("n_hidden_layers", C.c_int32), ("width", C.c_int32),
+                ("output_activation", C.c_int32), ("sh_scale", C.c_float)]
+
+
+# nhtb200_config.output_activation (FeatureDecoder output_activation)
+NHT_ACTIVATIONS = {"None": 0, "ReLU": 1, "Sigmoid": 2}
+NHT_UNSUPPORTED = 1
+
+_vp, _i32, _i64, _f32, _int, _sz, _str = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_int, C.c_size_t, C.c_char_p
+_cam, _vpp, _i64p, _f32p = C.POINTER(Camera), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_float)
+_adam = [_vp, _i64, _vpp, _vpp, _vpp, _f32p, _f32, _f32, _f32, _i64, _i32, _vp, _vp, _vp]
+_grt_trace = [_vp, _vp, _i64, _vp, _vp, _i32, _f32, _i32, _i32, _i32, _vp, _vp, _vp]  # ctx ... ray_to_world_host
+_nht = C.POINTER(NhtConfig)
+
+# C function -> (restype, argtypes) for every function the three headers declare; load() applies it once.  None = void.
+# tests/test_cabi_bindings.py checks each entry against its prototype, type for type.
+SIGNATURES = {
+    # include/gut_b200.h
+    "gutb200_default_config": (None, [C.POINTER(Config)]),
+    "gutb200_create": (_int, [C.POINTER(Config), _int, _vpp]),
+    "gutb200_destroy": (None, [_vp]),
+    "gutb200_last_error": (_str, [_vp]),
+    "gutb200_version": (_str, []),
+    "gutb200_forward": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_backward": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_backward_compact": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_sph_grad_from_views": (_int, [_vp, _vp, _i64, _vp, _i32, _i32, _vp, _vp, _vp]),
+    "gutb200_camera_position": (_int, [_cam, _vp]),
+    "gutb200_selective_adam_update": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i64, _i64]),
+    "gutb200_gaussian_adam_step": (_int, _adam),
+    "gutb200_gaussian_adam_step_reg": (_int, _adam + [_f32, _f32]),
+    "gutb200_image_loss_scratch_bytes": (_sz, [_i32, _i32]),
+    "gutb200_image_loss": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
+    "gutb200_image_loss_rgb": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
+    "gutb200_image_loss_composited": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp]),
+    "gutb200_forward_host": (_int, [_vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_backward_host": (_int, [_vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_last_stats": (_int, [_vp, _i64p, _i64p, _i64p, _i64p]),
+    "gutb200_debug_copy": (_int, [_vp, _int, _vp, _sz]),
+    "gutb200_collect_times": (_int, [_vp, _f32p, _f32p]),
+    "gutb200_set_timings": (_int, [_vp, _int]),
+    "gutb200_collect_stage_times": (_int, [_vp, _f32p]),
+    "gutb200_debug_work_counters": (_int, [_vp, _vp, _vp, _vp, _vp]),
+    "gutb200_debug_fma_peak": (_int, [_vp, _int, _f32p]),
+    "gutb200_launch_count": (_i64, [_vp]),
+    # include/grt_b200.h (3DGRT: LBVH build + ordered ray tracing)
+    "grtb200_default_config": (None, [C.POINTER(GrtConfig)]),
+    "grtb200_create": (_int, [C.POINTER(GrtConfig), _int, _vpp]),
+    "grtb200_destroy": (None, [_vp]),
+    "grtb200_last_error": (_str, [_vp]),
+    "grtb200_build_bvh": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _i32]),
+    "grtb200_build_bvh_packed": (_int, [_vp, _vp, _i64, _vp]),
+    "grtb200_trace": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp]),
+    "grtb200_trace_bwd": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "grtb200_scene_aabb": (_int, [_vp, _vp]),
+    "grtb200_launch_count": (_i64, [_vp]),
+    "grtb200_set_replay": (_int, [_vp, _i32]),
+    "grtb200_debug_trace_counters": (_int, _grt_trace + [_vp, _vp]),
+    # include/nht_b200.h (NHT feature decoder: fused tensor-core MLP)
+    "nhtb200_last_error": (_str, []),
+    "nhtb200_n_params": (_i64, [_nht]),
+    "nhtb200_backward_workspace_bytes": (_sz, [_nht, _i64]),
+    "nhtb200_forward": (_int, [_nht, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "nhtb200_backward": (_int, [_nht, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+}
+EXPORTS = [k for k in SIGNATURES if k.startswith("gutb200_")]
+GRT_EXPORTS = [k for k in SIGNATURES if k.startswith("grtb200_")]
+NHT_EXPORTS = [k for k in SIGNATURES if k.startswith("nhtb200_")]
+
 
 def camera_position(cam):
     """Sensor position in world space as the kernels compute it (gutb200_camera_position): numpy float32 [3]."""
@@ -66,7 +140,7 @@ def lib_path() -> str:
 
 
 def load():
-    """Load (building in-tree if sources are newer) the sm_90a shared library."""
+    """Load (building in-tree if sources are newer) the sm_90a shared library, with every function of SIGNATURES bound."""
     global _LIB
     if _LIB is not None:
         return _LIB
@@ -77,31 +151,25 @@ def load():
     if not os.path.exists(_SO):
         raise RuntimeError(f"{_SO} is missing: the CUDA extension was not built (no fallback path exists)")
     lib = C.CDLL(_SO)
-    lib.gutb200_version.restype = C.c_char_p
-    lib.gutb200_last_error.restype = C.c_char_p
-    lib.gutb200_last_error.argtypes = [C.c_void_p]
-    lib.gutb200_launch_count.restype = C.c_int64
-    lib.gutb200_launch_count.argtypes = [C.c_void_p]
-    lib.gutb200_create.argtypes = [C.POINTER(Config), C.c_int, C.POINTER(C.c_void_p)]
-    lib.gutb200_destroy.argtypes = [C.c_void_p]
-    vp, i64, i32 = C.c_void_p, C.c_int64, C.c_int32
-    cam = C.POINTER(Camera)
-    lib.gutb200_forward.argtypes = [vp, vp, cam, i64, vp, vp, i32, vp, vp, vp, vp, vp, vp]
-    lib.gutb200_backward.argtypes = [vp, vp, cam, i64, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gutb200_backward_compact.argtypes = [vp, vp, cam, i64, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gutb200_sph_grad_from_views.argtypes = [vp, vp, i64, vp, i32, i32, vp, vp, vp]
-    lib.gutb200_camera_position.argtypes = [cam, vp]
-    lib.gutb200_forward_host.argtypes = [vp, cam, i64, vp, vp, i32, vp, vp, vp, vp, vp, vp]
-    lib.gutb200_backward_host.argtypes = [vp, cam, i64, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gutb200_last_stats.argtypes = [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]
-    lib.gutb200_debug_copy.argtypes = [vp, C.c_int, vp, C.c_size_t]
-    lib.gutb200_collect_times.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
-    lib.gutb200_collect_stage_times.argtypes = [vp, C.POINTER(C.c_float)]
-    lib.gutb200_set_timings.argtypes = [vp, C.c_int]
-    lib.gutb200_debug_work_counters.argtypes = [vp, vp, vp, vp, vp]
-    lib.gutb200_debug_fma_peak.argtypes = [vp, C.c_int, C.POINTER(C.c_float)]
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _LIB = lib
     return lib
+
+
+def cfg_get(conf, path, default):
+    """conf's value at the dotted `path` (dict keys or attributes), `default` where it is missing or None."""
+    cur = conf
+    for key in path.split("."):
+        if cur is None:
+            return default
+        cur = cur.get(key, None) if isinstance(cur, dict) else getattr(cur, key, None)
+    return default if cur is None else cur
+
+
+def ptr(t) -> int:
+    return t.data_ptr()
 
 
 def default_config() -> Config:
@@ -110,20 +178,26 @@ def default_config() -> Config:
     return cfg
 
 
-class Context:
-    """Owning wrapper of a gutb200_ctx*."""
+class _Handle:
+    """Owning wrapper of a `<PREFIX>_ctx*`: created by `<PREFIX>_create`, released by `close` (or garbage collection); `_check` raises
+    with `<PREFIX>_last_error` for a non-zero return code."""
 
-    def __init__(self, cfg: Config, device: int = 0):
+    PREFIX = ""
+
+    def __init__(self, cfg, device: int = 0):
         self._lib = load()
         self._h = C.c_void_p()
-        rc = self._lib.gutb200_create(C.byref(cfg), int(device), C.byref(self._h))
-        if rc != 0 or not self._h:
-            raise RuntimeError(f"gutb200_create failed (rc={rc}): a CUDA device is required, there is no CPU path")
+        rc = getattr(self._lib, self.PREFIX + "_create")(C.byref(cfg), int(device), C.byref(self._h))
+        self._check_create(rc, cfg)
         self.cfg = cfg
+
+    def _check_create(self, rc: int, cfg):
+        if rc != 0 or not self._h:
+            raise RuntimeError(f"{self.PREFIX}_create failed (rc={rc}): a CUDA device is required, there is no CPU path")
 
     def close(self):
         if getattr(self, "_h", None):
-            self._lib.gutb200_destroy(self._h)
+            getattr(self._lib, self.PREFIX + "_destroy")(self._h)
             self._h = None
 
     def __del__(self):
@@ -134,7 +208,13 @@ class Context:
 
     def _check(self, rc: int, what: str):
         if rc != 0:
-            raise RuntimeError(f"{what} failed: {self._lib.gutb200_last_error(self._h).decode()}")
+            raise RuntimeError(f"{what} failed: {getattr(self._lib, self.PREFIX + '_last_error')(self._h).decode()}")
+
+
+class Context(_Handle):
+    """Owning wrapper of a gutb200_ctx*."""
+
+    PREFIX = "gutb200"
 
     def forward(self, stream, cam, n, particles, sph, sph_degree, rays_o, rays_d, out_rgba, out_dist, out_hits, visibility):
         self._check(self._lib.gutb200_forward(self._h, stream, C.byref(cam), n, particles, sph, sph_degree, rays_o, rays_d,
@@ -221,76 +301,21 @@ class Context:
 # ---------------------------------------------------------------------------------------------------------------
 # include/grt_b200.h (3DGRT: LBVH build + ordered ray tracing), same shared library
 
-class GrtConfig(C.Structure):
-    """grtb200_config"""
-
-    _fields_ = [("kernel_degree", C.c_int32), ("min_response", C.c_float), ("min_alpha", C.c_float), ("max_alpha", C.c_float),
-                ("density_clamping", C.c_int32), ("primitive", C.c_int32)]
-
-
-# grtb200_config.primitive (render.primitive_type)
-GRT_PRIMITIVES = {"instances": 0, "icosahedron": 1}
-
-
-GRT_EXPORTS = ["grtb200_default_config", "grtb200_create", "grtb200_destroy", "grtb200_last_error", "grtb200_build_bvh",
-               "grtb200_build_bvh_packed", "grtb200_trace",
-               "grtb200_trace_bwd", "grtb200_scene_aabb", "grtb200_launch_count", "grtb200_debug_trace_counters", "grtb200_set_replay"]
-
-
-def _grt_lib():
-    lib = load()
-    if not getattr(lib, "_grt_ready", False):
-        vp, i64, i32, f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_float
-        lib.grtb200_last_error.restype = C.c_char_p
-        lib.grtb200_last_error.argtypes = [vp]
-        lib.grtb200_launch_count.restype = i64
-        lib.grtb200_launch_count.argtypes = [vp]
-        lib.grtb200_create.argtypes = [C.POINTER(GrtConfig), C.c_int, C.POINTER(vp)]
-        lib.grtb200_destroy.argtypes = [vp]
-        lib.grtb200_build_bvh.argtypes = [vp, vp, i64, vp, vp, vp, vp, i32, i32]
-        lib.grtb200_build_bvh_packed.argtypes = [vp, vp, i64, vp]
-        lib.grtb200_trace.argtypes = [vp, vp, i64, vp, vp, i32, f32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-        lib.grtb200_trace_bwd.argtypes = [vp, vp, i64, vp, vp, i32, f32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-        lib.grtb200_scene_aabb.argtypes = [vp, vp]
-        lib.grtb200_set_replay.argtypes = [vp, i32]
-        lib.grtb200_debug_trace_counters.argtypes = [vp, vp, i64, vp, vp, i32, f32, i32, i32, i32, vp, vp, vp, vp, vp]
-        lib._grt_ready = True
-    return lib
-
-
 def grt_default_config() -> GrtConfig:
     cfg = GrtConfig()
-    _grt_lib().grtb200_default_config(C.byref(cfg))
+    load().grtb200_default_config(C.byref(cfg))
     return cfg
 
 
-class GrtContext:
+class GrtContext(_Handle):
     """Owning wrapper of a grtb200_ctx*."""
 
-    def __init__(self, cfg: GrtConfig, device: int = 0):
-        self._lib = _grt_lib()
-        self._h = C.c_void_p()
-        rc = self._lib.grtb200_create(C.byref(cfg), int(device), C.byref(self._h))
+    PREFIX = "grtb200"
+
+    def _check_create(self, rc: int, cfg):
         if rc == 5:
             raise ValueError(f"grtb200_create: primitive {cfg.primitive} is not one of {GRT_PRIMITIVES}")
-        if rc != 0 or not self._h:
-            raise RuntimeError(f"grtb200_create failed (rc={rc}): a CUDA device is required, there is no CPU path")
-        self.cfg = cfg
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.grtb200_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _check(self, rc, what):
-        if rc != 0:
-            raise RuntimeError(f"{what} failed: {self._lib.grtb200_last_error(self._h).decode()}")
+        super()._check_create(rc, cfg)
 
     def build_bvh(self, stream, n, pos, rot, scl, dns, rebuild=True, allow_update=False):
         self._check(self._lib.grtb200_build_bvh(self._h, stream, n, pos, rot, scl, dns, int(rebuild), int(allow_update)), "grtb200_build_bvh")
@@ -337,35 +362,7 @@ class GrtContext:
 # ---------------------------------------------------------------------------------------------------------------
 # include/nht_b200.h (NHT feature decoder: fused tensor-core MLP), same shared library
 
-class NhtConfig(C.Structure):
-    """nhtb200_config"""
-
-    _fields_ = [("n_features", C.c_int32), ("sh_degree", C.c_int32), ("n_hidden_layers", C.c_int32), ("width", C.c_int32),
-                ("output_activation", C.c_int32), ("sh_scale", C.c_float)]
-
-
-# nhtb200_config.output_activation (FeatureDecoder output_activation)
-NHT_ACTIVATIONS = {"None": 0, "ReLU": 1, "Sigmoid": 2}
-NHT_UNSUPPORTED = 1
-
-NHT_EXPORTS = ["nhtb200_last_error", "nhtb200_n_params", "nhtb200_backward_workspace_bytes", "nhtb200_forward", "nhtb200_backward"]
-
-
-def nht_lib():
-    lib = load()
-    if not getattr(lib, "_nht_ready", False):
-        vp, i64 = C.c_void_p, C.c_int64
-        cfg = C.POINTER(NhtConfig)
-        lib.nhtb200_last_error.restype = C.c_char_p
-        lib.nhtb200_last_error.argtypes = []
-        lib.nhtb200_n_params.restype = i64
-        lib.nhtb200_n_params.argtypes = [cfg]
-        lib.nhtb200_backward_workspace_bytes.restype = C.c_size_t
-        lib.nhtb200_backward_workspace_bytes.argtypes = [cfg, i64]
-        lib.nhtb200_forward.argtypes = [cfg, vp, i64, vp, vp, vp, vp]
-        lib.nhtb200_backward.argtypes = [cfg, vp, i64, vp, vp, vp, vp, vp, vp, vp]
-        lib._nht_ready = True
-    return lib
+nht_lib = load  # the feature decoder's name for the library; load() binds the nhtb200_* entries with the rest
 
 
 def nht_check(rc: int, what: str):

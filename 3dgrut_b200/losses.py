@@ -18,22 +18,6 @@ import b200_native as native
 _scratch = {}
 
 
-def _lib():
-    lib = native.load()
-    if not getattr(lib, "_loss_bound", False):
-        vp, i32, f32 = C.c_void_p, C.c_int32, C.c_float
-        lib.gutb200_image_loss_scratch_bytes.argtypes = [i32, i32]
-        lib.gutb200_image_loss_scratch_bytes.restype = C.c_size_t
-        lib.gutb200_image_loss.argtypes = [vp, i32, i32, vp, vp, f32, f32, vp, vp, vp]
-        lib.gutb200_image_loss.restype = C.c_int
-        lib.gutb200_image_loss_rgb.argtypes = [vp, i32, i32, vp, vp, f32, f32, vp, vp, vp]
-        lib.gutb200_image_loss_rgb.restype = C.c_int
-        lib.gutb200_image_loss_composited.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, f32, f32, vp, vp, vp, vp]
-        lib.gutb200_image_loss_composited.restype = C.c_int
-        lib._loss_bound = True
-    return lib
-
-
 def _check_image(t, what, ch):
     if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 3 and t.shape[2] == ch):
         raise RuntimeError(f"{what}: expected a contiguous float32 CUDA tensor [H,W,{ch}] (there is no CPU fallback)")
@@ -61,7 +45,7 @@ def _run(entry, pred, tgt, ch_pred, lambda_l1, lambda_ssim, d_pred, name):
     if tuple(tgt.shape[:2]) != (H, W):
         raise RuntimeError("prediction and target resolutions differ")
     dev = pred.device
-    lib = _lib()
+    lib = native.load()
     scratch = _scratch_for(lib, dev, H, W)
     if d_pred is None:
         d_pred = torch.empty((H, W, ch_pred), dtype=torch.float32, device=dev)
@@ -98,7 +82,7 @@ def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background
         mask = mask_hw(mask, H, W)
         if mask.device != dev:
             raise RuntimeError("mask: expected a tensor on the prediction's device")
-    lib = _lib()
+    lib = native.load()
     scratch = _scratch_for(lib, dev, H, W)
     if d_pred is None:
         d_pred = torch.empty((H, W, layout), dtype=torch.float32, device=dev)

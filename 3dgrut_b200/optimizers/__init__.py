@@ -17,21 +17,6 @@ GROUPS = ("positions", "density", "rotation", "scale", "features_albedo", "featu
 WIDTHS = (3, 1, 4, 3, 3, 45)
 
 
-def _lib():
-    lib = native.load()
-    if not getattr(lib, "_optim_bound", False):
-        vp, i64, i32, f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_float
-        lib.gutb200_selective_adam_update.argtypes = [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, i64, i64]
-        lib.gutb200_selective_adam_update.restype = C.c_int
-        lib.gutb200_gaussian_adam_step.argtypes = [vp, i64, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(f32), f32, f32, f32, i64, i32,
-                                                   vp, vp, vp]
-        lib.gutb200_gaussian_adam_step.restype = C.c_int
-        lib.gutb200_gaussian_adam_step_reg.argtypes = lib.gutb200_gaussian_adam_step.argtypes + [f32, f32]
-        lib.gutb200_gaussian_adam_step_reg.restype = C.c_int
-        lib._optim_bound = True
-    return lib
-
-
 def _check(t: torch.Tensor, what: str):
     if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
         raise RuntimeError(f"{what}: expected a contiguous float32 CUDA tensor (there is no CPU fallback)")
@@ -48,7 +33,7 @@ def selective_adam_update(param, param_grad, exp_avg, exp_avg_sq, visibility, lr
         raise RuntimeError("visibility must have one entry per row of param")
     stream = torch.cuda.current_stream(param.device).cuda_stream
     with torch.cuda.device(param.device):
-        rc = _lib().gutb200_selective_adam_update(stream, param.data_ptr(), param_grad.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+        rc = native.load().gutb200_selective_adam_update(stream, param.data_ptr(), param_grad.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
                                                   vis.data_ptr(), float(lr), float(beta1), float(beta2), float(eps), n, m)
     if rc != 0:
         raise RuntimeError(f"gutb200_selective_adam_update failed ({rc})")
@@ -59,7 +44,7 @@ class SelectiveAdam(torch.optim.Adam):
 
     def __init__(self, params, lr=0.001, betas=(0.9, 0.999), eps=1e-08):
         super().__init__(params=params, lr=lr, eps=eps, betas=betas)
-        _lib()  # fail now if the library is missing
+        native.load()  # fail now if the library is missing
 
     @torch.no_grad()
     def step(self, visibility):
@@ -98,7 +83,7 @@ class FusedGaussianAdam:
         self.exp_avg = {k: torch.zeros_like(t.data) for k, t in self.params.items()}
         self.exp_avg_sq = {k: torch.zeros_like(t.data) for k, t in self.params.items()}
         self.steps = 0
-        _lib()
+        native.load()
 
     @property
     def n(self) -> int:
@@ -150,6 +135,6 @@ class FusedGaussianAdam:
         else:  # d mean(sigmoid(raw)) / d density = 1 / N, d mean(exp(raw)) / d scale = 1 / (3 N)
             entry, extra = "gutb200_gaussian_adam_step_reg", (float(lambda_opacity) / max(self.n, 1), float(lambda_scale) / (3 * max(self.n, 1)))
         with torch.cuda.device(dev):
-            rc = getattr(_lib(), entry)(*args, *extra)
+            rc = getattr(native.load(), entry)(*args, *extra)
         if rc != 0:
             raise RuntimeError(f"{entry} failed ({rc})")

@@ -13,19 +13,7 @@ import numpy as np
 import torch
 
 import b200_native as native
-
-
-def _cfg_get(conf, path, default):
-    cur = conf
-    for key in path.split("."):
-        if cur is None:
-            return default
-        cur = cur.get(key, None) if isinstance(cur, dict) else getattr(cur, key, None)
-    return default if cur is None else cur
-
-
-def _ptr(t: torch.Tensor) -> int:
-    return t.data_ptr()
+from b200_native import cfg_get, ptr
 
 
 class OptixTracer:
@@ -65,7 +53,7 @@ class OptixTracer:
         pos, rot, scl, dns = (t.detach().contiguous().float() for t in (mog_pos, mog_rot, mog_scl, mog_dns))
         self._keep = (pos, rot, scl, dns)  # keep alive until the stream has consumed them
         stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).build_bvh(stream, int(pos.shape[0]), _ptr(pos), _ptr(rot), _ptr(scl), _ptr(dns), rebuild, allow_update)
+        self._context(dev).build_bvh(stream, int(pos.shape[0]), ptr(pos), ptr(rot), ptr(scl), ptr(dns), rebuild, allow_update)
 
     def build_bvh_packed(self, particles):
         """The same build from the [N,12] particle record that `trace` reads (grtb200_build_bvh_packed; no reference twin): bit-identical
@@ -76,7 +64,7 @@ class OptixTracer:
             raise RuntimeError("particles: expected a contiguous float32 CUDA tensor [N,12]")
         self._keep = (particles,)  # keep alive until the stream has consumed it
         dev = particles.device
-        self._context(dev).build_bvh_packed(torch.cuda.current_stream(dev).cuda_stream, int(particles.shape[0]), _ptr(particles))
+        self._context(dev).build_bvh_packed(torch.cuda.current_stream(dev).cuda_stream, int(particles.shape[0]), ptr(particles))
 
     @staticmethod
     def _r2w(ray_to_world) -> np.ndarray:
@@ -97,8 +85,8 @@ class OptixTracer:
         vis = torch.empty((max(n, 1), 1), **opts)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).trace(stream, n, _ptr(particle_density), _ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
-                                 _ptr(ray_ori), _ptr(ray_dir), r2w.ctypes.data, _ptr(feat), _ptr(alpha), _ptr(hit), _ptr(hits), _ptr(vis))
+        self._context(dev).trace(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
+                                 ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(feat), ptr(alpha), ptr(hit), ptr(hits), ptr(vis))
         return feat, alpha, hit, nrm, hits, vis[:n]
 
     def set_replay(self, enable, device):
@@ -118,8 +106,8 @@ class OptixTracer:
         vis = torch.empty((max(n, 1), 1), dtype=torch.float32, device=dev)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        return self._context(dev).trace_counters(stream, n, _ptr(particle_density), _ptr(particle_features), int(sph_degree), float(min_transmittance),
-                                                 b, h, w, _ptr(ray_ori), _ptr(ray_dir), r2w.ctypes.data, _ptr(vis))
+        return self._context(dev).trace_counters(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance),
+                                                 b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(vis))
 
     def trace_bwd(self, frame_id, ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, ray_normals, particle_density,
                   particle_features, ray_features_grd, ray_density_grd, ray_hit_distance_grd, ray_normals_grd, render_opts, sph_degree,
@@ -146,9 +134,9 @@ class OptixTracer:
                     raise RuntimeError(f"out: {name} must be a contiguous float32 CUDA tensor [{n},{k}]")
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).trace_bwd(stream, n, _ptr(particle_density), _ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
-                                     _ptr(ray_ori), _ptr(ray_dir), r2w.ctypes.data, _ptr(rf), _ptr(rd_), _ptr(rh), _ptr(g_f), _ptr(g_a),
-                                     _ptr(g_d), _ptr(d_density), _ptr(d_features))
+        self._context(dev).trace_bwd(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
+                                     ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(rf), ptr(rd_), ptr(rh), ptr(g_f), ptr(g_a),
+                                     ptr(g_d), ptr(d_density), ptr(d_features))
         return d_density[:n], d_features[:n]
 
     def native_context(self, device=None) -> native.GrtContext:
@@ -190,7 +178,7 @@ class Tracer:
         self.conf = conf
         self.num_update_bvh = 0
         torch.zeros(1, device=self.device)
-        g = lambda k, d: _cfg_get(conf, "render." + k, d)  # noqa: E731
+        g = lambda k, d: cfg_get(conf, "render." + k, d)  # noqa: E731
         self.tracer_wrapper = OptixTracer(
             None, None, g("pipeline_type", "reference"), g("backward_pipeline_type", "referenceBwd"), g("primitive_type", "instances"),
             g("particle_kernel_degree", 4), g("particle_kernel_min_response", 0.0113), g("particle_kernel_max_alpha", 0.99),

@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 import b200_native as native
+from b200_native import cfg_get, ptr
 
 
 class ShutterType(enum.IntEnum):  # bindings.cpp:36-42
@@ -102,47 +103,31 @@ def _so3_matrix_to_quat_xyzw(R: np.ndarray) -> np.ndarray:
     return (q / np.sqrt(np.sum(q * q, dtype=np.float32), dtype=np.float32)).astype(np.float32)
 
 
-def _cfg_get(conf, path, default):
-    cur = conf
-    for key in path.split("."):
-        if cur is None:
-            return default
-        if isinstance(cur, dict):
-            cur = cur.get(key, None)
-        else:
-            cur = getattr(cur, key, None)
-    return default if cur is None else cur
-
-
 def _native_config(conf) -> native.Config:
     """Config -> what the reference bakes in as -D constants (setup_3dgut.py:64-95)."""
     cfg = native.default_config()
-    cfg.kernel_degree = int(_cfg_get(conf, "render.particle_kernel_degree", 2))
-    cfg.min_kernel_density = float(_cfg_get(conf, "render.particle_kernel_min_response", 0.0113))
-    cfg.min_alpha = float(_cfg_get(conf, "render.particle_kernel_min_alpha", 1.0 / 255.0))
-    cfg.max_alpha = float(_cfg_get(conf, "render.particle_kernel_max_alpha", 0.99))
-    cfg.min_transmittance = float(_cfg_get(conf, "render.min_transmittance", 0.0001))
-    a = float(_cfg_get(conf, "render.splat.ut_alpha", 1.0))
-    k = float(_cfg_get(conf, "render.splat.ut_kappa", 0.0))
-    cfg.ut_alpha, cfg.ut_beta, cfg.ut_kappa = a, float(_cfg_get(conf, "render.splat.ut_beta", 2.0)), k
+    cfg.kernel_degree = int(cfg_get(conf, "render.particle_kernel_degree", 2))
+    cfg.min_kernel_density = float(cfg_get(conf, "render.particle_kernel_min_response", 0.0113))
+    cfg.min_alpha = float(cfg_get(conf, "render.particle_kernel_min_alpha", 1.0 / 255.0))
+    cfg.max_alpha = float(cfg_get(conf, "render.particle_kernel_max_alpha", 0.99))
+    cfg.min_transmittance = float(cfg_get(conf, "render.min_transmittance", 0.0001))
+    a = float(cfg_get(conf, "render.splat.ut_alpha", 1.0))
+    k = float(cfg_get(conf, "render.splat.ut_kappa", 0.0))
+    cfg.ut_alpha, cfg.ut_beta, cfg.ut_kappa = a, float(cfg_get(conf, "render.splat.ut_beta", 2.0)), k
     cfg.ut_delta = math.sqrt(a * a * (3 + k))
-    cfg.ut_margin = float(_cfg_get(conf, "render.splat.ut_in_image_margin_factor", 0.1))
-    cfg.rect_bounding = int(bool(_cfg_get(conf, "render.splat.rect_bounding", True)))
-    cfg.tight_opacity_bounding = int(bool(_cfg_get(conf, "render.splat.tight_opacity_bounding", True)))
-    cfg.tile_culling = int(bool(_cfg_get(conf, "render.splat.tile_based_culling", True)))
-    cfg.global_z_order = int(bool(_cfg_get(conf, "render.splat.global_z_order", True)))
-    cfg.enable_timings = int(bool(_cfg_get(conf, "render.enable_kernel_timings", False)))
-    cfg.n_rolling_shutter_iterations = int(_cfg_get(conf, "render.splat.n_rolling_shutter_iterations", 5))
-    cfg.k_buffer_size = int(_cfg_get(conf, "render.splat.k_buffer_size", 0))
+    cfg.ut_margin = float(cfg_get(conf, "render.splat.ut_in_image_margin_factor", 0.1))
+    cfg.rect_bounding = int(bool(cfg_get(conf, "render.splat.rect_bounding", True)))
+    cfg.tight_opacity_bounding = int(bool(cfg_get(conf, "render.splat.tight_opacity_bounding", True)))
+    cfg.tile_culling = int(bool(cfg_get(conf, "render.splat.tile_based_culling", True)))
+    cfg.global_z_order = int(bool(cfg_get(conf, "render.splat.global_z_order", True)))
+    cfg.enable_timings = int(bool(cfg_get(conf, "render.enable_kernel_timings", False)))
+    cfg.n_rolling_shutter_iterations = int(cfg_get(conf, "render.splat.n_rolling_shutter_iterations", 5))
+    cfg.k_buffer_size = int(cfg_get(conf, "render.splat.k_buffer_size", 0))
     if not (0 <= cfg.k_buffer_size <= 16):
         raise NotImplementedError("k_buffer_size must be within 0..16 (configs/paper/3dgut/sorted_*.yaml use 16)")
-    if int(_cfg_get(conf, "render.particle_radiance_sph_degree", 3)) != 3:
+    if int(cfg_get(conf, "render.particle_radiance_sph_degree", 3)) != 3:
         raise NotImplementedError("this build stores 16 SH coefficients per particle (particle_radiance_sph_degree=3)")
     return cfg
-
-
-def _ptr(t: torch.Tensor) -> int:
-    return t.data_ptr()
 
 
 def _c(t: torch.Tensor) -> torch.Tensor:
@@ -226,8 +211,8 @@ class SplatRaster:
         vis = torch.empty((n, 1), dtype=torch.float32, device=dev)
         cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
         stream = _raw_stream(dev)
-        self._context(dev).forward(stream, cam, n, _ptr(particle_density), _ptr(particle_radiance), int(n_active_features),
-                                   _ptr(ray_ori), _ptr(ray_dir), _ptr(rgba), _ptr(dist), _ptr(hits), _ptr(vis))
+        self._context(dev).forward(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features),
+                                   ptr(ray_ori), ptr(ray_dir), ptr(rgba), ptr(dist), ptr(hits), ptr(vis))
         return rgba, dist, hits, vis
 
     def trace_bwd(self, frame_id, n_active_features, particle_density, particle_radiance, ray_ori, ray_dir, ray_time, sensor_params,
@@ -250,9 +235,9 @@ class SplatRaster:
             d_radiance = torch.empty((n, 48), dtype=torch.float32, device=dev)
         cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
         stream = _raw_stream(dev)
-        self._context(dev).backward(stream, cam, n, _ptr(particle_density), _ptr(particle_radiance), int(n_active_features),
-                                    _ptr(ray_ori), _ptr(ray_dir), _ptr(rgba), _ptr(d_rgba), _ptr(dist), _ptr(d_dist),
-                                    _ptr(d_density), _ptr(d_radiance))
+        self._context(dev).backward(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features),
+                                    ptr(ray_ori), ptr(ray_dir), ptr(rgba), ptr(d_rgba), ptr(dist), ptr(d_dist),
+                                    ptr(d_density), ptr(d_radiance))
         return d_density, d_radiance
 
     # ---- view-parallel extensions (no reference twin: the reference trains on one GPU) -----------------------------------------
@@ -277,9 +262,9 @@ class SplatRaster:
             g = torch.empty((n, 4), dtype=torch.float32, device=dev)
         cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
         stream = _raw_stream(dev)
-        self._context(dev).backward_compact(stream, cam, n, _ptr(particle_density), _ptr(particle_radiance), int(n_active_features),
-                                            _ptr(ray_ori), _ptr(ray_dir), _ptr(rgba), _ptr(d_rgba), _ptr(dist), _ptr(d_dist),
-                                            _ptr(d_density), _ptr(g))
+        self._context(dev).backward_compact(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features),
+                                            ptr(ray_ori), ptr(ray_dir), ptr(rgba), ptr(d_rgba), ptr(dist), ptr(d_dist),
+                                            ptr(d_density), ptr(g))
         return d_density, g
 
     def sensor_position(self, sensor_params, pose_start, pose_end, width, height):
@@ -297,8 +282,8 @@ class SplatRaster:
         d_radiance = out if out is not None else torch.empty((n, 48), dtype=torch.float32, device=dev)
         assert d_radiance.shape == (n, 48) and d_radiance.is_contiguous()
         stream = _raw_stream(dev)
-        self._context(dev).sph_grad_from_views(stream, n, _ptr(particle_density), int(n_active_features),
-                                               np.asarray(view_positions, np.float32).reshape(-1, 3), _ptr(g_all), _ptr(d_radiance))
+        self._context(dev).sph_grad_from_views(stream, n, ptr(particle_density), int(n_active_features),
+                                               np.asarray(view_positions, np.float32).reshape(-1, 3), ptr(g_all), ptr(d_radiance))
         return d_radiance
 
     def collect_times(self):

@@ -16,69 +16,50 @@ from __future__ import annotations
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 import losses
-import optimizers
 import view_parallel
 from threedgrt_tracer.tracer import Tracer
-from train_step import regulariser_loss
+from train_step import TrainStep
 
 PHASES = ("build", "trace", "loss", "backward", "exchange", "adam", "densify")
 
 
-class GaussianTrainStepGRT:
-    def __init__(self, params: dict, lrs: dict, conf=None, sph_degree: int = 3, selective: bool = False, group=None, eps: float = 1e-15,
-                 densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0, background="black",
-                 background_seed: int = 0, lambda_opacity: float = 0.0, lambda_scale: float = 0.0):
-        """params: raw leaf tensors for optimizers.GROUPS.  conf: a config with a `render:` section read as threedgrt_tracer.Tracer reads
-        it (primitive_type, particle_kernel_degree, particle_kernel_density_clamping, max_consecutive_bvh_update, min_transmittance,
-        particle_kernel_max_alpha, ...).  densify_conf: densify.DensifyConfig (GS) or densify.MCMCConfig turns densification on.
-        background / background_seed / lambda_opacity / lambda_scale: as in train_step.GaussianTrainStep."""
-        self.params = {k: params[k] for k in optimizers.GROUPS}  # ONE dict shared with the optimizer and the densifier
-        self.device = self.params["positions"].device
-        self.sph_degree = int(sph_degree)
-        self.group = group
-        self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+class GaussianTrainStepGRT(TrainStep):
+    """Constructor as train_step.TrainStep's; conf is read as threedgrt_tracer.Tracer reads it (primitive_type, particle_kernel_degree,
+    particle_kernel_density_clamping, max_consecutive_bvh_update, min_transmittance, particle_kernel_max_alpha, ...).  `phase_events`
+    records every phase of PHASES."""
+
+    def _init_renderer(self, conf):
         with torch.cuda.device(self.device):
-            self.tracer = Tracer(conf if conf is not None else {"render": {}})
+            self.tracer = Tracer(conf)
         self.tracer.tracer_wrapper.set_replay(True, self.device)
         self.min_transmittance = self.tracer._min_transmittance
-        self.optimizer = optimizers.FusedGaussianAdam(self.params, lrs, eps=eps, selective=selective)
-        self.exchange = view_parallel.FlatGradientExchange(self.n, self.device, group=group)
-        self.frame = 0
-        self.lambda_l1, self.lambda_ssim = float(lambda_l1), float(lambda_ssim)  # reference defaults: 0.8 / 0.2 (configs/base_gs.yaml:172-179)
-        self.lambda_opacity, self.lambda_scale = float(lambda_opacity), float(lambda_scale)
-        rank = dist.get_rank(group) if self.world > 1 else 0
-        self.background = losses.Background(background, seed=int(background_seed) + rank, device=self.device)
-        self.scene_extent = float(scene_extent)
-        self.densifier = None
-        if densify_conf is not None:
-            import densify
-
-            cls = densify.MCMCDensifier if isinstance(densify_conf, densify.MCMCConfig) else densify.GSDensifier
-            self.densifier = cls(self.params, [self.optimizer.exp_avg, self.optimizer.exp_avg_sq], densify_conf, group=group)
         self._rebuild = True   # the first build, and the first after densification, is a rebuild (build_acc(rebuild=True))
         self._zeros = {}       # zero d_alpha / d_dist / d_normals per resolution: the loss has no depth term, and no alpha term on black
-        self.phase_events = None  # set to [] to record (phase, cuda event) pairs at the end of each phase of `step`
 
-    @property
-    def n(self) -> int:
-        return int(self.params["positions"].shape[0])
+    def _new_exchange(self):
+        return view_parallel.FlatGradientExchange(self.n, self.device, group=self.group)
+
+    def _image_loss(self, pred, target, lambda_l1, lambda_ssim, background, mask):
+        rgb, alpha, zero1 = pred
+        if background is None and mask is None:  # black, unmasked: the rgb loss, no alpha gradient
+            loss, _, _, d_rgb = losses.image_loss_rgb(rgb, target, lambda_l1, lambda_ssim)
+            return loss, (d_rgb, zero1)
+        # composited onto the background, masked: rgb and alpha gradients (gut_loss.cu)
+        loss, _, _, d_rgb, d_alpha = losses.image_loss_rgb_alpha(rgb, alpha, target, lambda_l1, lambda_ssim, background=background, mask=mask)
+        return loss, (d_rgb, d_alpha)
+
+    def _l1_grads(self, pred, diff):
+        return self._d_l1(diff), pred[2]
+
+    def _densified(self):
+        self._rebuild = True  # the Gaussians changed: rebuild the BVH from scratch next step
+        super()._densified()
 
     @property
     def num_update_bvh(self) -> int:
         return self.tracer.num_update_bvh
-
-    @torch.no_grad()
-    def activated(self):
-        """[N,12] = pos3, sigmoid(density), normalize(rotation) (wxyz), exp(scale), 0 and [N,48] = cat(albedo, specular)
-        (threedgrt_tracer/tracer.py:61, model.py:94-118)"""
-        p = self.params
-        particles = torch.cat([p["positions"], torch.sigmoid(p["density"]), torch.nn.functional.normalize(p["rotation"]), torch.exp(p["scale"]),
-                               torch.zeros_like(p["density"])], dim=1).contiguous()
-        sph = torch.cat([p["features_albedo"], p["features_specular"]], dim=1).contiguous()
-        return particles, sph
 
     def _build(self, particles):
         """Tracer.build_acc's cadence: with density clamping every build is a rebuild, otherwise the update path is taken until
@@ -95,12 +76,6 @@ class GaussianTrainStepGRT:
             self._zeros = {key: (torch.zeros((1, H, W, 1), dtype=torch.float32, device=self.device),
                                  torch.zeros((1, H, W, 3), dtype=torch.float32, device=self.device))}
         return self._zeros[key]
-
-    def _mark(self, phase):
-        if self.phase_events is not None:
-            ev = torch.cuda.Event(enable_timing=True)
-            ev.record()
-            self.phase_events.append((phase, ev))
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, T_to_world):
@@ -134,52 +109,14 @@ class GaussianTrainStepGRT:
         rgb, alpha, dst, nrm, hits, vis = ot.trace(self.frame, T_to_world, rays_o, rays_d, particles, sph, 0, self.sph_degree,
                                                    self.min_transmittance)
         self._mark("trace")
-        target = target_rgb.reshape(H, W, 3)
         zero1, zero3 = self._zero_grads(H, W)
-        d_alpha = zero1
-        if not self.background.black or mask is not None:
-            # composited onto the background, masked: rgb and alpha gradients (gut_loss.cu); global-batch normalisation
-            loss, _, _, d_rgb, d_alpha = losses.image_loss_rgb_alpha(rgb, alpha, target.contiguous(), self.lambda_l1 / self.world,
-                                                                     self.lambda_ssim / self.world, background=self.background.draw(H, W),
-                                                                     mask=mask)
-            loss = loss * self.world
-        elif self.lambda_ssim != 0.0:
-            # lambda_l1 L1 + lambda_ssim (1 - SSIM) and its rgb gradient in two launches (gut_loss.cu); global-batch normalisation
-            loss, _, _, d_rgb = losses.image_loss_rgb(rgb, target.contiguous(), self.lambda_l1 / self.world, self.lambda_ssim / self.world)
-            loss = loss * self.world
-        else:
-            diff = rgb[0] - target
-            loss = self.lambda_l1 * diff.abs().mean()
-            d_rgb = self.lambda_l1 * torch.sign(diff) / (diff.numel() * self.world)  # d mean|.| / d rgb, global-batch normalisation
+        loss, (d_rgb, d_alpha) = self._loss((rgb, alpha, zero1), rgb[0], target_rgb.reshape(H, W, 3), H, W, mask)
         self._mark("loss")
         ot.trace_bwd(self.frame, T_to_world, rays_o, rays_d, rgb, alpha, dst, nrm, particles, sph, d_rgb, d_alpha, zero1, zero3, 0,
                      self.sph_degree, self.min_transmittance, out=self.exchange.out())
         self._mark("backward")
-        if all_sensor_positions is None and self.world != 1:
-            raise RuntimeError("all_sensor_positions is required when more than one rank trains")
-        if self.densifier is not None:
-            # this view's own position gradient, before the exchange (weighted by the distance to THIS view's sensor, gs.py:127-137);
-            # x world undoes the global-batch normalisation so that the thresholds keep their per-view meaning
-            self.densifier.update_gradient_buffer(self.exchange.d_particles[:, 0:3] * float(self.world), self.sensor_position(T_to_world))
-        d_particles, d_sph = self.exchange.exchange()
-        if self.optimizer.selective and self.world > 1:
-            dist.all_reduce(vis, op=dist.ReduceOp.MAX, group=self.group)  # visible in any view of the batch (SURVEY 8e)
-        self._mark("exchange")
-        # the regularisers belong to the step once (every rank holds the same parameters): added after the exchange, no 1 / world
-        reg = {}
-        if self.lambda_opacity != 0.0 or self.lambda_scale != 0.0:
-            loss = loss + regulariser_loss(particles, self.lambda_opacity, self.lambda_scale)
-            reg = dict(lambda_opacity=self.lambda_opacity, lambda_scale=self.lambda_scale)
-        self.optimizer.step(d_particles, d_sph, visibility=vis if self.optimizer.selective else None, **reg)
-        self._mark("adam")
-        self.frame += 1
-        if self.densifier is not None and self.densifier.post_optimizer_step(self.frame, self.scene_extent, positions_lr=self.optimizer.lrs["positions"]):
-            # the Gaussians changed (identically on every rank): re-capacity the exchange buffer, rebuild the BVH from scratch next step
-            self._rebuild = True
-            if self.exchange.n != self.n:
-                self.exchange = view_parallel.FlatGradientExchange(self.n, self.device, group=self.group)
-        self._mark("densify")
-        return loss
+        my_position = self.sensor_position(T_to_world) if self.densifier is not None else None
+        return self._update(loss, particles, vis, all_sensor_positions, my_position)
 
     def bytes_on_wire(self) -> int:
         return self.exchange.bytes_on_wire()

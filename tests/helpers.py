@@ -1,8 +1,30 @@
-"""Shared helpers of the parity tests."""
+"""Shared helpers of the tests."""
+import os
+import re
+
 import numpy as np
 
 import scenes
 from oracle import gut_oracle as go
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def prototypes(header):
+    """{name: (return type, [parameter types])} of the functions include/<header> declares, comments stripped; a parameter type keeps
+    its `const` and `*` ("const float*", "float* const*"), `(void)` is no parameters."""
+    text = open(os.path.join(ROOT, "include", header)).read()
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", "", text, flags=re.S)
+    out = {}
+    for ret, name, params in re.findall(r"^[ \t]*([A-Za-z_][\w \t*]*?)\s*\b([a-z]+b200_\w+)\s*\(([^;]*?)\)\s*;", text, re.M):
+        types = [re.sub(r"\s*\b\w+\s*$", "", p.strip()) for p in params.split(",") if p.strip() not in ("", "void")]
+        out[name] = (ret.strip(), types)
+    return out
+
+
+def declared(header):
+    """Names of the functions include/<header> declares."""
+    return set(prototypes(header))
 
 
 def oracle_camera(sc, c2w, pose=None):

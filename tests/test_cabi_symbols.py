@@ -2,30 +2,23 @@
 path fails loudly (no CPU fallback) when no CUDA device is present."""
 import ctypes
 import os
-import re
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _declared(header="gut_b200.h", prefix="gutb200_"):
-    text = open(os.path.join(ROOT, "include", header)).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(" + prefix + r"[a-z_0-9]+)\s*\(", text)))
+from helpers import ROOT, declared
 
 
 def test_library_exports_every_declared_symbol():
     import b200_native as nat
 
     lib = nat.load()
-    names = _declared()
+    names = declared("gut_b200.h")
     assert len(names) >= 14
     for name in names:
         assert hasattr(lib, name), f"{name} declared in include/gut_b200.h but not exported"
     assert set(nat.EXPORTS) == set(names)
     assert b"sm_90a" in lib.gutb200_version()
-    grt = _declared("grt_b200.h", "grtb200_")
+    grt = declared("grt_b200.h")
     assert len(grt) >= 9 and set(nat.GRT_EXPORTS) == set(grt)
     for name in grt:
         assert hasattr(lib, name), f"{name} declared in include/grt_b200.h but not exported"

@@ -1,21 +1,13 @@
 """The entry points the 3DGRT training step adds to the C ABI are declared, exported and bound (no GPU needed)."""
-import os
-import re
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _declared(header):
-    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", header)).read(), flags=re.S)
-    return set(re.findall(r"\b((?:gutb200|grtb200)_[a-z_0-9]+)\s*\(", text))
+from helpers import declared
 
 
 def test_training_step_entry_points_are_exported():
     import b200_native as nat
 
     lib = nat.load()
-    assert "grtb200_build_bvh_packed" in _declared("grt_b200.h") and "grtb200_build_bvh_packed" in nat.GRT_EXPORTS
-    assert "gutb200_image_loss_rgb" in _declared("gut_b200.h") and "gutb200_image_loss_rgb" in nat.EXPORTS
+    assert "grtb200_build_bvh_packed" in declared("grt_b200.h") and "grtb200_build_bvh_packed" in nat.GRT_EXPORTS
+    assert "gutb200_image_loss_rgb" in declared("gut_b200.h") and "gutb200_image_loss_rgb" in nat.EXPORTS
     for name in ("grtb200_build_bvh_packed", "gutb200_image_loss_rgb", "grtb200_build_bvh", "gutb200_image_loss"):
         assert hasattr(lib, name), name
     assert hasattr(nat.GrtContext, "build_bvh_packed")

@@ -107,6 +107,7 @@ def test_all_zeros_mask_gives_a_zero_gradient():
 def test_composited_loss_rejects_bad_arguments():
     import ctypes
 
+    import b200_native as nat
     import losses
 
     dev = torch.device("cuda", 0)
@@ -121,7 +122,7 @@ def test_composited_loss_rejects_bad_arguments():
         losses.image_loss_rgb_alpha(rgb, alpha, tgt, background=torch.rand((16, 16, 3)))
     with pytest.raises(ValueError):
         losses.Background("grey")
-    lib = losses._lib()
+    lib = nat.load()
     scratch = torch.empty(int(lib.gutb200_image_loss_scratch_bytes(16, 16)) // 4 + 1, device=dev)
     sums = torch.empty(2, device=dev)
     d = torch.empty(16 * 16 * 4 + 1, device=dev)

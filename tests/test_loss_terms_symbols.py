@@ -1,29 +1,21 @@
 """The entry points the composited loss and the regularised Adam step add to the C ABI are declared, exported and bound, and the training
 steps' new arguments are there (no GPU needed)."""
 import inspect
-import os
-import re
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import declared
+
 NEW = ("gutb200_image_loss_composited", "gutb200_gaussian_adam_step_reg")
-
-
-def _declared(header):
-    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", header)).read(), flags=re.S)
-    return set(re.findall(r"\b((?:gutb200|grtb200)_[a-z_0-9]+)\s*\(", text))
 
 
 def test_loss_terms_entry_points_are_exported():
     import b200_native as nat
-    import losses
-    import optimizers
 
     lib = nat.load()
     for name in NEW:
-        assert name in _declared("gut_b200.h") and name in nat.EXPORTS, name
+        assert name in declared("gut_b200.h") and name in nat.EXPORTS, name
         assert hasattr(lib, name), name
-    assert losses._lib().gutb200_image_loss_composited.argtypes is not None
-    assert optimizers._lib().gutb200_gaussian_adam_step_reg.argtypes is not None
+    assert lib.gutb200_image_loss_composited.argtypes is not None
+    assert lib.gutb200_gaussian_adam_step_reg.argtypes is not None
 
 
 def test_new_arguments_without_a_gpu():

@@ -2,23 +2,21 @@
 has the reference class's keys and shapes.  No GPU needed."""
 import ctypes as C
 import os
-import re
 
 import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import ROOT, declared
 
 
 def test_every_nhtb200_symbol_is_exported_and_bound():
     import b200_native as nat
 
-    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "nht_b200.h")).read(), flags=re.S)
-    declared = set(re.findall(r"\b(nhtb200_[a-z_0-9]+)\s*\(", text))
-    assert declared == set(nat.NHT_EXPORTS)
+    names = declared("nht_b200.h")
+    assert names == set(nat.NHT_EXPORTS)
     lib = nat.nht_lib()
-    for name in declared:
+    for name in names:
         assert hasattr(lib, name) and getattr(lib, name).argtypes is not None, name
 
 
