@@ -77,6 +77,8 @@ SIGNATURES = {
     "gutb200_version": (_str, []),
     "gutb200_forward": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_backward": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_forward_nht": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_backward_nht": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_backward_compact": (_int, [_vp, _vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_sph_grad_from_views": (_int, [_vp, _vp, _i64, _vp, _i32, _i32, _vp, _vp, _vp]),
     "gutb200_camera_position": (_int, [_cam, _vp]),
@@ -224,6 +226,19 @@ class Context(_Handle):
                  d_particles, d_sph):
         self._check(self._lib.gutb200_backward(self._h, stream, C.byref(cam), n, particles, sph, sph_degree, rays_o, rays_d,
                                                out_rgba, d_rgba, out_dist, d_dist, d_particles, d_sph), "gutb200_backward")
+
+    def forward_nht(self, stream, cam, n, particles, features, feature_dim, features_half, rays_o, rays_d, out_features_alpha, out_dist,
+                    out_hits, visibility):
+        """NHT features instead of SH radiance: out_features_alpha [H,W,feature_dim/2 + 1] (gutb200_forward_nht)."""
+        self._check(self._lib.gutb200_forward_nht(self._h, stream, C.byref(cam), n, particles, features, feature_dim, features_half, rays_o,
+                                                  rays_d, out_features_alpha, out_dist, out_hits, visibility), "gutb200_forward_nht")
+
+    def backward_nht(self, stream, cam, n, particles, features, feature_dim, features_half, rays_o, rays_d, out_features_alpha,
+                     d_features_alpha, out_dist, d_dist, d_particles, d_features):
+        """Adjoint of forward_nht: d_particles [N,12], d_features [N,feature_dim] fp32 (gutb200_backward_nht)."""
+        self._check(self._lib.gutb200_backward_nht(self._h, stream, C.byref(cam), n, particles, features, feature_dim, features_half, rays_o,
+                                                   rays_d, out_features_alpha, d_features_alpha, out_dist, d_dist, d_particles, d_features),
+                    "gutb200_backward_nht")
 
     def backward_compact(self, stream, cam, n, particles, sph, sph_degree, rays_o, rays_d, out_rgba, d_rgba, out_dist, d_dist,
                          d_particles, d_radiance):

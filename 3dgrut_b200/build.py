@@ -23,6 +23,7 @@ UNITS = {
     # compositing kernels: same numerics mode as the reference build (-use_fast_math, setup_3dgut.py:108-109):
     # flush-to-zero, approximate div/sqrt/exp; parity is tolerance-based for these (DESIGN.md section 5)
     "gut_render.cu": ["--use_fast_math"],
+    "gut_render_nht.cu": ["--use_fast_math"],
     "gut_render_kbuffer.cu": ["--use_fast_math", "--extended-lambda"],
     "gut_api.cu": ["-fmad=false"],
     "grt.cu": ["--use_fast_math"],

@@ -163,6 +163,7 @@ struct gutb200_ctx {
     FrameConfig fcfg{};
     int64_t n = -1, num_isect = 0, num_tiles = 0;
     bool have_forward = false;
+    bool fwd_nht = false;          // the forward rendered NHT features (gutb200_forward_nht): only gutb200_backward_nht may follow
     cudaStream_t fwd_stream = nullptr;
 
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -391,10 +392,23 @@ const char* gutb200_last_error(const gutb200_ctx* c) { return c ? c->error.c_str
 
 int64_t gutb200_launch_count(const gutb200_ctx* c) { return c ? c->launches : 0; }
 
-int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
-                    int32_t sph_degree, const float* rays_o, const float* rays_d, float* out_rgba, float* out_dist, float* out_hits,
-                    float* visibility) {
-    if (int rc = check_args(c, cam, n, particles, sph_degree)) return rc;
+}  // extern "C"
+
+namespace {
+
+// NHT features: the configuration the kernels build (48 features = 4 vertices x 12, barycentric, sincos x 1)
+int check_nht_args(gutb200_ctx* c, const void* features, int32_t feature_dim, int32_t features_half) {
+    if (feature_dim != 48) return fail(c, "NHT feature_dim %d not built (48 = 4 tetrahedron vertices x 12 features)", feature_dim);
+    if (features_half != 0 && features_half != 1) return fail(c, "features_half must be 0 (fp32) or 1 (fp16), got %d", features_half);
+    if (reinterpret_cast<uintptr_t>(features) & 15) return fail(c, "feature buffer must be 16-byte aligned");
+    if (c->cfg.k_buffer_size > 0) return fail(c, "NHT features are not built with the k-buffer (k_buffer_size %d > 0)", c->cfg.k_buffer_size);
+    return 0;
+}
+
+// nht = false: SH radiance (`sph`, `sph_degree`, out [H,W,4]); nht = true: NHT features (`sph` = features, `half`, out [H,W,25])
+int forward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const void* sph,
+                 int32_t sph_degree, bool nht, bool half, const float* rays_o, const float* rays_d, float* out_rgba, float* out_dist,
+                 float* out_hits, float* visibility) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     GUT_CUDA(c, cudaSetDevice(c->device));
     c->have_forward = false;
@@ -452,7 +466,11 @@ int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int
             StageTimer t(c, 5, s);
             if (c->fcfg.k_buffer_size == 0)  // chunks a forward warp never reaches must read as "no hit" in the backward
                 GUT_CUDA(c, cudaMemsetAsync(c->hit_words.ptr, 0, hit_words_capacity(capacity, tiles) * 4, s));
-            if (c->fcfg.k_buffer_size > 0)  // sorted 3DGUT (gut_render_kbuffer.cu)
+            if (nht)
+                launch_render_forward_nht(s, c->cam, c->fcfg, rays_o, rays_d, particles, sph, half, c->vals_out.as<uint32_t>(),
+                                          c->ranges.as<uint32_t>(), c->tile_order.as<uint32_t>(), c->chunk_base.as<uint32_t>(),
+                                          c->hit_words.as<uint32_t>(), out_rgba, out_dist, out_hits);
+            else if (c->fcfg.k_buffer_size > 0)  // sorted 3DGUT (gut_render_kbuffer.cu)
                 launch_render_forward_kbuffer(s, c->cam, c->fcfg, c->fcfg.k_buffer_size, rays_o, rays_d, particles, c->rgb.as<float>(),
                                               c->vals_out.as<uint32_t>(), c->ranges.as<uint32_t>(), out_rgba, out_dist, out_hits);
             else
@@ -468,8 +486,8 @@ int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int
     GUT_CUDA(c, cudaMemsetAsync(c->tile_hist.ptr, 0, tt * kTileSubs * 4, s));
     if (n > 0) {
         StageTimer t(c, 0, s);
-        launch_project(s, c->cam, c->fcfg, n, particles, sph, sph_degree, c->tiles_count.as<uint32_t>(), c->proj.as<ProjRecord>(),
-                       c->depth.as<float>(), c->rgb.as<float>(), visibility, c->tile_hist.as<uint32_t>());
+        launch_project(s, c->cam, c->fcfg, n, particles, static_cast<const float*>(sph), sph_degree, c->tiles_count.as<uint32_t>(),
+                       c->proj.as<ProjRecord>(), c->depth.as<float>(), c->rgb.as<float>(), visibility, c->tile_hist.as<uint32_t>(), !nht);
         c->launches++;
     }
     GUT_CUDA(c, c->vals_out.reserve(16, s));
@@ -501,14 +519,35 @@ int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int
     c->num_tiles = tiles;
     c->fwd_stream = s;
     c->fwd_camera = *cam;
+    c->fwd_nht = nht;
     c->have_forward = true;
     return 0;
 }
 
-static int backward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
-                         int32_t sph_degree, const float* rays_o, const float* rays_d, const float* out_rgba, const float* d_rgba,
-                         const float* out_dist, const float* d_dist, float* d_particles, float* d_sph, bool compact) {
+}  // namespace
+
+extern "C" {
+
+int gutb200_forward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
+                    int32_t sph_degree, const float* rays_o, const float* rays_d, float* out_rgba, float* out_dist, float* out_hits,
+                    float* visibility) {
     if (int rc = check_args(c, cam, n, particles, sph_degree)) return rc;
+    return forward_impl(c, stream, cam, n, particles, sph, sph_degree, false, false, rays_o, rays_d, out_rgba, out_dist, out_hits, visibility);
+}
+
+int gutb200_forward_nht(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const void* features,
+                        int32_t feature_dim, int32_t features_half, const float* rays_o, const float* rays_d, float* out_features_alpha,
+                        float* out_dist, float* out_hits, float* visibility) {
+    if (int rc = check_args(c, cam, n, particles, 0)) return rc;
+    if (int rc = check_nht_args(c, features, feature_dim, features_half)) return rc;
+    return forward_impl(c, stream, cam, n, particles, features, 0, true, features_half != 0, rays_o, rays_d, out_features_alpha, out_dist,
+                        out_hits, visibility);
+}
+
+// `nht`: the adjoint of gutb200_forward_nht (`sph` = the features, `half`, out / d_rgba [H,W,25], d_sph = d_features [N,48])
+static int backward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const void* sph,
+                         int32_t sph_degree, bool nht, bool half, const float* rays_o, const float* rays_d, const float* out_rgba,
+                         const float* d_rgba, const float* out_dist, const float* d_dist, float* d_particles, float* d_sph, bool compact) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     // the backward replays the sorted lists of the immediately preceding forward (gutRenderer.cu:436-440)
     if (!c->have_forward || c->fwd_stream != s || c->n != n || c->cam.width != cam->width || c->cam.height != cam->height)
@@ -516,15 +555,24 @@ static int backward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam
     // the lists, the projection and the hit words are those of the forward's camera: a different view in between is an error, not a silent mix
     if (memcmp(&c->fwd_camera, cam, sizeof(gutb200_camera)) != 0)
         return fail(c, "backward was called with a camera that differs from the immediately preceding forward's (poses / intrinsics)");
+    if (c->fwd_nht != nht)
+        return fail(c, nht ? "gutb200_backward_nht needs a gutb200_forward_nht before it (the preceding forward rendered SH radiance)"
+                           : "the preceding forward rendered NHT features: its adjoint is gutb200_backward_nht");
     GUT_CUDA(c, cudaSetDevice(c->device));
     if (c->cfg.enable_timings) {
         GUT_CUDA(c, cudaEventRecord(c->ev[2], s));
     }
     const size_t nn = static_cast<size_t>(n > 0 ? n : 1);
     GUT_CUDA(c, c->grad_acc.reserve(nn * kGradRow * 4, s, /*zero=*/true));
+    if (nht && n > 0) GUT_CUDA(c, cudaMemsetAsync(d_sph, 0, static_cast<size_t>(n) * 48 * sizeof(float), s));  // the feature adjoint adds into it
     if (c->num_isect > 0) {
         StageTimer t(c, 6, s);
-        if (c->fcfg.k_buffer_size > 0)
+        if (nht)
+            GUT_CUDA(c, launch_render_backward_nht(s, c->cam, c->fcfg, rays_o, rays_d, particles, sph, half, c->vals_out.as<uint32_t>(),
+                                                   c->ranges.as<uint32_t>(), c->tile_order.as<uint32_t>(), c->chunk_base.as<uint32_t>(),
+                                                   c->hit_words.as<uint32_t>(), out_rgba, d_rgba, out_dist, d_dist, c->grad_acc.as<float>(),
+                                                   d_sph));
+        else if (c->fcfg.k_buffer_size > 0)
             launch_render_backward_kbuffer(s, c->cam, c->fcfg, c->fcfg.k_buffer_size, rays_o, rays_d, particles, c->rgb.as<float>(),
                                            c->vals_out.as<uint32_t>(), c->ranges.as<uint32_t>(), out_rgba, d_rgba, out_dist, d_dist,
                                            c->grad_acc.as<float>());
@@ -536,8 +584,9 @@ static int backward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam
     }
     if (n > 0) {
         StageTimer t(c, 7, s);
-        launch_project_backward(s, c->cam, n, particles, sph, sph_degree, c->rgb.as<float>(), c->tiles_count.as<uint32_t>(), rays_o,
-                                c->grad_acc.as<float>(), d_particles, d_sph, compact, /*canon=*/c->fcfg.k_buffer_size == 0);
+        launch_project_backward(s, c->cam, n, particles, static_cast<const float*>(sph), sph_degree, c->rgb.as<float>(),
+                                c->tiles_count.as<uint32_t>(), rays_o, c->grad_acc.as<float>(), d_particles, d_sph, compact,
+                                /*canon=*/c->fcfg.k_buffer_size == 0, /*radiance=*/!nht);
         c->launches++;
     }
     GUT_CUDA(c, cudaGetLastError());
@@ -551,14 +600,26 @@ static int backward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam
 int gutb200_backward(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
                      int32_t sph_degree, const float* rays_o, const float* rays_d, const float* out_rgba, const float* d_rgba,
                      const float* out_dist, const float* d_dist, float* d_particles, float* d_sph) {
-    return backward_impl(c, stream, cam, n, particles, sph, sph_degree, rays_o, rays_d, out_rgba, d_rgba, out_dist, d_dist, d_particles, d_sph, false);
+    if (int rc = check_args(c, cam, n, particles, sph_degree)) return rc;
+    return backward_impl(c, stream, cam, n, particles, sph, sph_degree, false, false, rays_o, rays_d, out_rgba, d_rgba, out_dist, d_dist, d_particles,
+                         d_sph, false);
+}
+
+int gutb200_backward_nht(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const void* features,
+                         int32_t feature_dim, int32_t features_half, const float* rays_o, const float* rays_d, const float* out_features_alpha,
+                         const float* d_features_alpha, const float* out_dist, const float* d_dist, float* d_particles, float* d_features) {
+    if (int rc = check_args(c, cam, n, particles, 0)) return rc;
+    if (int rc = check_nht_args(c, features, feature_dim, features_half)) return rc;
+    return backward_impl(c, stream, cam, n, particles, features, 0, true, features_half != 0, rays_o, rays_d, out_features_alpha, d_features_alpha,
+                         out_dist, d_dist, d_particles, d_features, false);
 }
 
 int gutb200_backward_compact(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const float* sph,
                              int32_t sph_degree, const float* rays_o, const float* rays_d, const float* out_rgba, const float* d_rgba,
                              const float* out_dist, const float* d_dist, float* d_particles, float* d_radiance) {
-    return backward_impl(c, stream, cam, n, particles, sph, sph_degree, rays_o, rays_d, out_rgba, d_rgba, out_dist, d_dist, d_particles, d_radiance,
-                         true);
+    if (int rc = check_args(c, cam, n, particles, sph_degree)) return rc;
+    return backward_impl(c, stream, cam, n, particles, sph, sph_degree, false, false, rays_o, rays_d, out_rgba, d_rgba, out_dist, d_dist, d_particles,
+                         d_radiance, true);
 }
 
 int gutb200_sph_grad_from_views(gutb200_ctx* c, void* stream, int64_t n, const float* particles, int32_t sph_degree, int32_t views,
@@ -708,6 +769,7 @@ int gutb200_debug_copy(gutb200_ctx* c, int what, void* dst, size_t bytes) {
 int gutb200_debug_work_counters(gutb200_ctx* c, const float* particles, const float* rays_o, const float* rays_d, uint64_t* counters16) {
     if (!c || !c->have_forward) return fail(c, "no forward context");
     if (c->fcfg.k_buffer_size != 0) return fail(c, "work counters exist for the unsorted path (k_buffer_size 0) only");
+    if (c->fwd_nht) return fail(c, "work counters exist for the SH radiance forward only");
     GUT_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t s = c->fwd_stream;
     unsigned long long* dctr = nullptr;

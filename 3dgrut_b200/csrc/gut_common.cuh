@@ -57,7 +57,7 @@ constexpr int kGradRow = 20;
 
 void launch_project(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, int64_t n, const float* particles,
                     const float* sph, int sph_degree, uint32_t* tiles_count, ProjRecord* proj, float* depth, float* rgb,
-                    float* visibility, uint32_t* tile_hist);
+                    float* visibility, uint32_t* tile_hist, bool radiance = true);
 void launch_expand_place(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, int64_t n, const ProjRecord* proj, const float* depth,
                          const uint32_t* tile_hist, const uint32_t* sub_base, const uint32_t* totals, uint32_t capacity, uint32_t* fill,
                          unsigned long long* keys);
@@ -83,6 +83,17 @@ void launch_render_backward(cudaStream_t s, const FrameCamera& cam, const FrameC
                             const float* rays_d, const float* particles, const float* rgb, const uint32_t* sorted_values,
                             const uint32_t* ranges, const uint32_t* tile_order, const uint32_t* chunk_base, const uint32_t* hit_words,
                             const float* out_rgba, const float* d_rgba, const float* out_dist, const float* d_dist, float* grad_acc);
+// gut_render_nht.cu: Neural Harmonic Texture features (48 per particle, barycentric, sincos) -> [H,W,25] features + opacity, and the
+// adjoint: canonical sums into grad_acc (G8 with radiance = false maps them) and the feature gradient into d_features (zeroed by the caller)
+void launch_render_forward_nht(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, const float* rays_o, const float* rays_d,
+                               const float* particles, const void* features, bool half, const uint32_t* sorted_values, const uint32_t* ranges,
+                               const uint32_t* tile_order, const uint32_t* chunk_base, uint32_t* hit_words, float* out_features_alpha,
+                               float* out_dist, float* out_hits);
+cudaError_t launch_render_backward_nht(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, const float* rays_o, const float* rays_d,
+                                       const float* particles, const void* features, bool half, const uint32_t* sorted_values,
+                                       const uint32_t* ranges, const uint32_t* tile_order, const uint32_t* chunk_base, const uint32_t* hit_words,
+                                       const float* out_features_alpha, const float* d_features_alpha, const float* out_dist, const float* d_dist,
+                                       float* grad_acc, float* d_features);
 void launch_fma_peak(cudaStream_t s, int blocks, int iters, float* sink);
 void launch_render_forward_kbuffer(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, int K, const float* rays_o, const float* rays_d,
                                    const float* particles, const float* rgb, const uint32_t* sorted_values, const uint32_t* ranges,
@@ -92,7 +103,7 @@ void launch_render_backward_kbuffer(cudaStream_t s, const FrameCamera& cam, cons
                                     const float* out_rgba, const float* d_rgba, const float* out_dist, const float* d_dist, float* grad_acc);
 void launch_project_backward(cudaStream_t s, const FrameCamera& cam, int64_t n, const float* particles, const float* sph,
                              int sph_degree, const float* rgb, const uint32_t* tiles_count, const float* rays_o, float* grad_acc,
-                             float* d_particles, float* d_sph, bool compact, bool canon);
+                             float* d_particles, float* d_sph, bool compact, bool canon, bool radiance = true);
 void launch_sph_from_views(cudaStream_t s, int64_t n, const float* particles, int sph_degree, int views, const float* view_positions,
                            const float* d_radiance_all, float* d_sph);
 

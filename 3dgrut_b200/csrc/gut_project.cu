@@ -292,8 +292,9 @@ __device__ __forceinline__ void sph_radiance(int deg, const float* __restrict__ 
 }
 
 // G1: one thread per particle (projectOnTiles -> GUTProjector::eval, gutProjector.cuh:217-322)
-// ROLLING = false is the global-shutter instantiation (no pose interpolation code, no stack frame)
-template <bool ROLLING>
+// ROLLING = false is the global-shutter instantiation (no pose interpolation code, no stack frame); RGB = false skips the SH -> radiance
+// work (NHT features are evaluated per hit in gut_render_nht.cu) and leaves `rgb` and `sph` untouched
+template <bool ROLLING, bool RGB>
 __global__ void __launch_bounds__(kProjThreads) project_kernel(FrameCamera cam, FrameConfig cfg, int64_t n,
                                                                const float* __restrict__ particles,
                                                                const float* __restrict__ sph, int sph_degree,
@@ -470,13 +471,14 @@ __global__ void __launch_bounds__(kProjThreads) project_kernel(FrameCamera cam, 
     } else {
         const float sx = px - cam.cam_pos[0], sy = py - cam.cam_pos[1], sz = pz - cam.cam_pos[2];
         const float dist = sqrtf(sx * sx + sy * sy + sz * sz);
-        sph_radiance(sph_degree, sph + i * 48, sx / dist, sy / dist, sz / dist, col);
+        if (RGB) sph_radiance(sph_degree, sph + i * 48, sx / dist, sy / dist, sz / dist, col);
         pr.cx = pcx; pr.cy = pcy; pr.ex = ex; pr.ey = ey;
         pr.ca = ca; pr.cb = cb; pr.cc = cc; pr.op = op;
         zdepth = cfg.global_z_order ? zc : dist;
     }
     proj[i] = pr;
     depth[i] = zdepth;
+    if (!RGB) return;
     rgb[i * 3 + 0] = col[0];
     rgb[i * 3 + 1] = col[1];
     rgb[i * 3 + 2] = col[2];
@@ -552,13 +554,16 @@ __global__ void __launch_bounds__(256) expand_place_kernel(FrameCamera cam, Fram
 
 void launch_project(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, int64_t n, const float* particles,
                     const float* sph, int sph_degree, uint32_t* tiles_count, ProjRecord* proj, float* depth, float* rgb,
-                    float* visibility, uint32_t* tile_hist) {
+                    float* visibility, uint32_t* tile_hist, bool radiance) {
     if (n <= 0) return;
     const unsigned blocks = static_cast<unsigned>((n + kProjThreads - 1) / kProjThreads);
-    if (cam.rolling_shutter != 0)
-        project_kernel<true><<<blocks, kProjThreads, 0, s>>>(cam, cfg, n, particles, sph, sph_degree, tiles_count, proj, depth, rgb, visibility, tile_hist);
-    else
-        project_kernel<false><<<blocks, kProjThreads, 0, s>>>(cam, cfg, n, particles, sph, sph_degree, tiles_count, proj, depth, rgb, visibility, tile_hist);
+#define GUT_PROJ(ROLLING_, RGB_) project_kernel<ROLLING_, RGB_><<<blocks, kProjThreads, 0, s>>>(cam, cfg, n, particles, sph, sph_degree, tiles_count, proj, depth, rgb, visibility, tile_hist)
+    if (cam.rolling_shutter != 0) {
+        if (radiance) GUT_PROJ(true, true); else GUT_PROJ(true, false);
+    } else {
+        if (radiance) GUT_PROJ(false, true); else GUT_PROJ(false, false);
+    }
+#undef GUT_PROJ
 }
 
 void launch_expand_place(cudaStream_t s, const FrameCamera& cam, const FrameConfig& cfg, int64_t n, const ProjRecord* proj, const float* depth,

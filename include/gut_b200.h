@@ -94,6 +94,20 @@ int gutb200_backward(gutb200_ctx* ctx, void* stream, const gutb200_camera* cam, 
                      const float* out_rgba, const float* d_rgba, const float* out_dist, const float* d_dist,
                      float* d_particles, float* d_sph);
 
+/* Neural Harmonic Texture (NHT) features instead of SH radiance (model.feature_type: nht; neuralHarmonicFeaturesParticle.slang).
+ * features [N,feature_dim] per particle: 4 tetrahedron vertices x 12 features, fp32 (features_half = 0) or fp16 (features_half = 1,
+ * render.particle_feature_half), 16-byte aligned.  Built: feature_dim 48, barycentric interpolation, sincos activation with 1 frequency
+ * -> 24 ray features.  out_features_alpha [H,W,25] = 24 features then the opacity, fp32; out_dist / out_hits / visibility as
+ * gutb200_forward.  The backward replays the forward of the same camera and stream, which must be gutb200_forward_nht (and SH forwards
+ * only take gutb200_backward); d_particles [N,12] as gutb200_backward, d_features [N,48] fp32 whatever the feature precision.  Every row of
+ * both is written.  k_buffer_size > 0 is refused. */
+int gutb200_forward_nht(gutb200_ctx* ctx, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const void* features,
+                        int32_t feature_dim, int32_t features_half, const float* rays_o, const float* rays_d, float* out_features_alpha,
+                        float* out_dist, float* out_hits, float* visibility);
+int gutb200_backward_nht(gutb200_ctx* ctx, void* stream, const gutb200_camera* cam, int64_t n, const float* particles, const void* features,
+                         int32_t feature_dim, int32_t features_half, const float* rays_o, const float* rays_d, const float* out_features_alpha,
+                         const float* d_features_alpha, const float* out_dist, const float* d_dist, float* d_particles, float* d_features);
+
 /* Host-buffer variants: pinned or pageable host pointers; H2D/D2H copies happen inside on the context's stream. */
 /* View-parallel training (ours, no reference twin -- the reference is single-GPU): the [N,48] SH gradient row of a view is the outer
  * product basis16(direction particle <- sensor) x g, g = masked dL/d(radiance) of the particle in that view.  gutb200_backward_compact
