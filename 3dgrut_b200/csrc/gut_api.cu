@@ -151,8 +151,9 @@ struct gutb200_ctx {
     DeviceBuffer tiles_count, proj, depth, rgb, grad_acc;
     // per intersection: 64-bit (depth bits << 32 | particle) keys in per-tile slices, sorted particle indices, hit words
     DeviceBuffer keys64, keys64_alt, vals_out, hit_words;
-    // per tile: list-length histogram, slot counters, ranges, heaviest-first order, hit-word slice offsets; {I, overflow} on the device
-    DeviceBuffer tile_hist, tile_fill, sub_base, ranges, tile_order, chunk_base, totals;
+    // per tile: list-length histogram, slot counters, ranges, heaviest-first order, hit-word slice offsets; {I, overflow} on the device;
+    // per-CTA partial sums of the tile scan
+    DeviceBuffer tile_hist, tile_fill, sub_base, ranges, tile_order, chunk_base, totals, scan_parts;
     cudaEvent_t ev_total = nullptr;
     gutb200_camera fwd_camera{};   // the camera of the forward whose context the backward replays
     // host staging for the *_host entry points
@@ -373,7 +374,7 @@ void gutb200_destroy(gutb200_ctx* c) {
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
     DeviceBuffer* bufs[] = {&c->tiles_count, &c->proj, &c->depth, &c->rgb, &c->grad_acc, &c->keys64, &c->keys64_alt, &c->vals_out, &c->hit_words, &c->tile_hist,
-                            &c->tile_fill, &c->sub_base, &c->ranges, &c->tile_order, &c->chunk_base, &c->totals, &c->h_particles, &c->h_sph,
+                            &c->tile_fill, &c->scan_parts, &c->sub_base, &c->ranges, &c->tile_order, &c->chunk_base, &c->totals, &c->h_particles, &c->h_sph,
                             &c->h_rays_o, &c->h_rays_d, &c->h_rgba, &c->h_dist, &c->h_hits, &c->h_vis, &c->h_drgba, &c->h_ddist,
                             &c->h_dpart, &c->h_dsph};
     for (DeviceBuffer* b : bufs) b->release();
@@ -433,6 +434,7 @@ int forward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_
     GUT_CUDA(c, c->tile_order.reserve(tt * 4, s));
     GUT_CUDA(c, c->chunk_base.reserve(tt * 4, s));
     GUT_CUDA(c, c->totals.reserve(16, s));
+    GUT_CUDA(c, c->scan_parts.reserve(tile_scan_parts_words(static_cast<int>(tiles)) * 4, s));
 
     // The frame is enqueued in one go.  The list total I is needed on the host only to SIZE the key / value / hit-word buffers, so the
     // kernels that depend on it are launched speculatively against the capacity those (grow-only) buffers already have, and the host
@@ -443,11 +445,12 @@ int forward_impl(gutb200_ctx* c, void* stream, const gutb200_camera* cam, int64_
         {
             StageTimer t(c, 1, s);
             launch_tile_scan(s, static_cast<int>(tiles), c->tile_hist.as<uint32_t>(), capacity, c->ranges.as<uint32_t>(), c->sub_base.as<uint32_t>(),
-                             c->chunk_base.as<uint32_t>(), c->tile_order.as<uint32_t>(), c->tile_fill.as<uint32_t>(), c->totals.as<uint32_t>());
+                             c->chunk_base.as<uint32_t>(), c->tile_order.as<uint32_t>(), c->tile_fill.as<uint32_t>(), c->totals.as<uint32_t>(),
+                             c->scan_parts.as<uint32_t>());
         }
         GUT_CUDA(c, cudaMemcpyAsync(c->pinned_total, c->totals.ptr, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         GUT_CUDA(c, cudaEventRecord(c->ev_total, s));
-        c->launches++;
+        c->launches += 2;
         if (capacity > 0 && n > 0) {
             {
                 StageTimer t(c, 2, s);

@@ -63,8 +63,9 @@ void launch_expand_place(cudaStream_t s, const FrameCamera& cam, const FrameConf
                          unsigned long long* keys);
 // gut_binning.cu: tile ranges / order / hit-word slices from the per-tile histogram, per-tile on-chip sort of the 64-bit keys
 constexpr int kTileSubs = 16;  // sub-counters per tile (a particle uses sub-counter `particle & 15`): spreads the atomics of hot tiles
+size_t tile_scan_parts_words(int num_tiles);  // size of the scan's per-CTA partials (`parts`) in 32-bit words
 void launch_tile_scan(cudaStream_t s, int num_tiles, const uint32_t* counts, uint32_t capacity, uint32_t* ranges, uint32_t* sub_base,
-                      uint32_t* chunk_base, uint32_t* order, uint32_t* fill, uint32_t* totals);
+                      uint32_t* chunk_base, uint32_t* order, uint32_t* fill, uint32_t* totals, uint32_t* parts);
 cudaError_t launch_tile_sort(cudaStream_t s, int num_tiles, const uint32_t* order, const uint32_t* ranges, const uint32_t* totals,
                              unsigned long long* keys, unsigned long long* keys_alt, uint32_t* sorted_values);
 void launch_synth_tile_keys(cudaStream_t s, int num_tiles, const uint32_t* ranges, const uint32_t* vals, const float* depth, uint64_t* out);
