@@ -64,6 +64,7 @@ _vp, _i32, _i64, _f32, _int, _sz, _str = C.c_void_p, C.c_int32, C.c_int64, C.c_f
 _cam, _vpp, _i64p, _f32p = C.POINTER(Camera), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_float)
 _adam = [_vp, _i64, _vpp, _vpp, _vpp, _f32p, _f32, _f32, _f32, _i64, _i32, _vp, _vp, _vp]
 _grt_trace = [_vp, _vp, _i64, _vp, _vp, _i32, _f32, _i32, _i32, _i32, _vp, _vp, _vp]  # ctx ... ray_to_world_host
+_grt_trace_nht = [_vp, _vp, _i64, _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, _vp, _vp, _vp]  # ctx ... ray_to_world_host (NHT features)
 _nht = C.POINTER(NhtConfig)
 
 # C function -> (restype, argtypes) for every function the three headers declare; load() applies it once.  None = void.
@@ -108,6 +109,8 @@ SIGNATURES = {
     "grtb200_build_bvh_packed": (_int, [_vp, _vp, _i64, _vp]),
     "grtb200_trace": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_bwd": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "grtb200_trace_nht": (_int, _grt_trace_nht + [_vp, _vp, _vp, _vp, _vp]),
+    "grtb200_trace_bwd_nht": (_int, _grt_trace_nht + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "grtb200_scene_aabb": (_int, [_vp, _vp]),
     "grtb200_launch_count": (_i64, [_vp]),
     "grtb200_set_replay": (_int, [_vp, _i32]),
@@ -316,6 +319,27 @@ class Context(_Handle):
 # ---------------------------------------------------------------------------------------------------------------
 # include/grt_b200.h (3DGRT: LBVH build + ordered ray tracing), same shared library
 
+NHT_FEATURE_DIM = 48  # model.nht_features.dim of the shipped NHT configs (configs/base_gs.yaml): 4 tetrahedron vertices x 12
+_NHT_BUILT = (("model.nht_features.dim", NHT_FEATURE_DIM), ("model.nht_features.activation.type", "sincos"),
+              ("model.nht_features.activation.num_frequencies", 1), ("model.nht_features.interpolation_type", "barycentric"))
+
+
+def nht_feature_config(conf, tracer: str):
+    """model.feature_type -> None (SH radiance) or the NHT settings both tracers take: {"half": render.particle_feature_half}.
+    Only the reference's shipped NHT configuration is built (configs/base_gs.yaml: dim 48, barycentric, sincos with 1 frequency);
+    anything else raises NotImplementedError naming the key.  Pure config logic: needs no GPU.  `tracer` names the caller in messages."""
+    kind = str(cfg_get(conf, "model.feature_type", "sh")).lower()
+    if kind == "sh":
+        return None
+    if kind != "nht":
+        raise NotImplementedError(f"model.feature_type={kind!r}: the {tracer} tracer renders 'sh' or 'nht'")
+    for key, want in _NHT_BUILT:
+        got = cfg_get(conf, key, want)
+        if (str(got).lower() if isinstance(want, str) else int(got)) != want:
+            raise NotImplementedError(f"{key}={got!r}: NHT features are built for {key}={want!r} only")
+    return {"half": bool(cfg_get(conf, "render.particle_feature_half", False))}
+
+
 def grt_default_config() -> GrtConfig:
     cfg = GrtConfig()
     load().grtb200_default_config(C.byref(cfg))
@@ -349,6 +373,20 @@ class GrtContext(_Handle):
         self._check(self._lib.grtb200_trace_bwd(self._h, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d,
                                                 r2w_host, out_rgb, out_alpha, out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph),
                     "grtb200_trace_bwd")
+
+    def trace_nht(self, stream, n, particles, features, feature_dim, features_half, min_t, batch, height, width, rays_o, rays_d, r2w_host,
+                  out_features, out_alpha, out_dist, out_hits, visibility):
+        """NHT features instead of SH radiance: out_features [R,feature_dim/2] (grtb200_trace_nht)."""
+        self._check(self._lib.grtb200_trace_nht(self._h, stream, n, particles, features, feature_dim, features_half, min_t, batch, height, width,
+                                                rays_o, rays_d, r2w_host, out_features, out_alpha, out_dist, out_hits, visibility),
+                    "grtb200_trace_nht")
+
+    def trace_bwd_nht(self, stream, n, particles, features, feature_dim, features_half, min_t, batch, height, width, rays_o, rays_d, r2w_host,
+                      out_features, out_alpha, out_dist, d_features_out, d_alpha, d_dist, d_particles, d_features):
+        """Adjoint of trace_nht: d_particles [N,12], d_features [N,feature_dim] fp32 (grtb200_trace_bwd_nht)."""
+        self._check(self._lib.grtb200_trace_bwd_nht(self._h, stream, n, particles, features, feature_dim, features_half, min_t, batch, height,
+                                                    width, rays_o, rays_d, r2w_host, out_features, out_alpha, out_dist, d_features_out, d_alpha,
+                                                    d_dist, d_particles, d_features), "grtb200_trace_bwd_nht")
 
     def scene_aabb(self):
         import numpy as np

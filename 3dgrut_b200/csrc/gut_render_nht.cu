@@ -19,6 +19,7 @@
 #include <cuda_fp16.h>
 
 #include "gut_common.cuh"
+#include "nht_features.cuh"
 #include "render_tile.cuh"
 #include "subtile_cull.cuh"
 
@@ -27,37 +28,7 @@ namespace gutb200 {
 namespace {
 
 constexpr int kNhtBatch = 128;
-constexpr int kNhtBase = 12;                    // features per tetrahedron vertex
-constexpr int kNhtOut = 2 * kNhtBase;           // ray features (sin, cos of every blended feature)
-constexpr int kNhtRow = 4 * kNhtBase;           // particle feature row
 constexpr int kNhtChannels = kNhtOut + 1;       // output channels: features, then opacity
-
-// tetrahedron vertices / 12: w_k = 1/4 + vk12[k] . P
-__constant__ float kVk12[4][3] = {{0.2041241452319315f, -0.11785113019775793f, -0.08333333333333333f},
-                                   {-0.2041241452319315f, -0.11785113019775793f, -0.08333333333333333f},
-                                   {0.0f, 0.23570226039551587f, -0.08333333333333333f},
-                                   {0.0f, 0.0f, 0.25f}};
-
-__device__ __forceinline__ void bary_weights(float px, float py, float pz, float (&w)[4]) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) w[k] = 0.25f + (kVk12[k][0] * px + kVk12[k][1] * py + kVk12[k][2] * pz);
-}
-
-// blended base features of staged row `f` (12 float4 = [vertex][12])
-__device__ __forceinline__ void blend(const float4* __restrict__ f, const float (&w)[4], float (&b)[kNhtBase]) {
-#pragma unroll
-    for (int q = 0; q < 3; ++q) {
-        float4 a = f[q];
-        b[q * 4 + 0] = w[0] * a.x; b[q * 4 + 1] = w[0] * a.y; b[q * 4 + 2] = w[0] * a.z; b[q * 4 + 3] = w[0] * a.w;
-    }
-#pragma unroll
-    for (int k = 1; k < 4; ++k)
-#pragma unroll
-        for (int q = 0; q < 3; ++q) {
-            const float4 a = f[k * 3 + q];
-            b[q * 4 + 0] += w[k] * a.x; b[q * 4 + 1] += w[k] * a.y; b[q * 4 + 2] += w[k] * a.z; b[q * 4 + 3] += w[k] * a.w;
-        }
-}
 
 // stage the feature rows of entries [base, base + count) into feat[entry][12 float4]; all threads of the CTA take part
 template <bool HALF>

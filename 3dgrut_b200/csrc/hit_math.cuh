@@ -149,6 +149,75 @@ __device__ __forceinline__ void hit_adjoint(const ParticleFrame& f, const Canoni
     T = nextT;
 }
 
+// Adjoint of one accepted hit in the form of the reference's Slang pipelines (gaussianParticles.slang hit() / processHitFromBuffer
+// under bwd_diff), used for NHT features.  Differences from hit_adjoint:
+//   * alpha = min(max_alpha, response density) is differentiated: a clamped hit passes no gradient through response or density;
+//   * the radiance residual is replaced by the features': fg = sum_c f_c g_c of this hit, FiG = sum_c F_out,c g_c of the ray and the
+//     running FG = sum_c F_acc,c g_c (in/out), so res = (FiG - FG) / T_next is peeled without a clamp;
+//   * pg = dL/dP of the canonical hit point P = gro + grd pd (the features depend on it) flows into gro and grd:
+//     groGrd += pg - grd s, grdGrd += pd pg - s gro with s = grd . pg; the normalize adjoint below is the general one.
+// g[0..10] = d(pos3, density, quat4, scale3).
+template <int DEG>
+__device__ __forceinline__ void hit_adjoint_nht(const ParticleFrame& f, const CanonicalHit& h, float dx, float dy, float dz, float fg, float pgx,
+                                                float pgy, float pgz, float min_transmittance, float Tint, float Tgrad, float FiG, float Dint,
+                                                float Dgrad, float& T, float& FG, float& D, float g[11]) {
+    const float pd = -(h.gdx * h.gox + h.gdy * h.goy + h.gdz * h.goz);
+    const float ddx = h.gdx * pd, ddy = h.gdy * pd, ddz = h.gdz * pd;
+    const float hx = f.sx * ddx, hy = f.sy * ddy, hz = f.sz * ddz;
+    const float gsq = hx * hx + hy * hy + hz * hz;
+    const float gdist = sqrtf(gsq);
+    const float weight = h.alpha * T;
+    const float nextT = (1.f - h.alpha) * T;
+    const float inv_next = nextT <= min_transmittance ? 0.f : 1.0f / nextT;
+    D += weight * gdist;
+    const float resD = fmaxf((Dint - D) * inv_next, 0.f);
+    const float a_hit = (gdist - resD) * T * Dgrad;
+    const float hs = gsq > 0.f ? (weight / gdist) * Dgrad : 0.f;
+    const float hgx = hx * hs, hgy = hy * hs, hgz = hz * hs;
+    const float sd = hgx * f.sx * h.gdx + hgy * f.sy * h.gdy + hgz * f.sz * h.gdz;
+    const float resT = h.alpha < 0.999999f ? Tint / (1.f - h.alpha) : T;
+    const float a_dns = resT * -Tgrad;
+    FG += weight * fg;
+    const float res_g = (FiG - FG) * inv_next;
+    float common = a_hit + a_dns + T * (fg - res_g);
+    if (h.gres * f.dns > h.alpha) common = 0.f;  // clamped at max_alpha: d min(max_alpha, x) / dx = 0
+    g[3] = h.gres * common;
+    const float gray_g = response_grad<DEG>(h.gray, h.gres, f.dns * common);
+    const float kx = 2.f * h.ccx * gray_g, ky = 2.f * h.ccy * gray_g, kz = 2.f * h.ccz * gray_g;
+    const float ps = h.gdx * pgx + h.gdy * pgy + h.gdz * pgz;
+    const float gd_gx = kz * h.goy - ky * h.goz + (f.sx * hgx * pd - h.gox * sd) + (pd * pgx - ps * h.gox);
+    const float gd_gy = kx * h.goz - kz * h.gox + (f.sy * hgy * pd - h.goy * sd) + (pd * pgy - ps * h.goy);
+    const float gd_gz = ky * h.gox - kx * h.goy + (f.sz * hgz * pd - h.goz * sd) + (pd * pgz - ps * h.goz);
+    const float go_gx = ky * h.gdz - kz * h.gdy - h.gdx * sd + (pgx - h.gdx * ps);
+    const float go_gy = kz * h.gdx - kx * h.gdz - h.gdy * sd + (pgy - h.gdy * ps);
+    const float go_gz = kx * h.gdy - ky * h.gdx - h.gdz * sd + (pgz - h.gdz * ps);
+    const float prg_x = f.isx * go_gx, prg_y = f.isy * go_gy, prg_z = f.isz * go_gz;
+    float sgx = ddx * hgx - h.gox * prg_x;
+    float sgy = ddy * hgy - h.goy * prg_y;
+    float sgz = ddz * hgz - h.goz * prg_z;
+    g[0] = -(prg_x * f.r0x + prg_y * f.r1x + prg_z * f.r2x);
+    g[1] = -(prg_x * f.r0y + prg_y * f.r1y + prg_z * f.r2y);
+    g[2] = -(prg_x * f.r0z + prg_y * f.r1z + prg_z * f.r2z);
+    const float il3 = h.il * h.il * h.il;
+    const float du = gd_gx * h.ux + gd_gy * h.uy + gd_gz * h.uz;
+    const float ug_x = h.l > 0.f ? h.il * gd_gx - il3 * h.ux * du : 0.f;
+    const float ug_y = h.l > 0.f ? h.il * gd_gy - il3 * h.uy * du : 0.f;
+    const float ug_z = h.l > 0.f ? h.il * gd_gz - il3 * h.uz * du : 0.f;
+    const float rdg_x = f.isx * ug_x, rdg_y = f.isy * ug_y, rdg_z = f.isz * ug_z;
+    sgx -= h.ux * rdg_x;
+    sgy -= h.uy * rdg_y;
+    sgz -= h.uz * rdg_z;
+    g[8] = sgx; g[9] = sgy; g[10] = sgz;
+    const float m00 = prg_x * h.pcx + rdg_x * dx, m01 = prg_x * h.pcy + rdg_x * dy, m02 = prg_x * h.pcz + rdg_x * dz;
+    const float m10 = prg_y * h.pcx + rdg_y * dx, m11 = prg_y * h.pcy + rdg_y * dy, m12 = prg_y * h.pcz + rdg_y * dz;
+    const float m20 = prg_z * h.pcx + rdg_z * dx, m21 = prg_z * h.pcy + rdg_z * dy, m22 = prg_z * h.pcz + rdg_z * dz;
+    g[4] = 2.f * (f.qz * (m01 - m10) + f.qy * (m20 - m02) + f.qx * (m12 - m21));
+    g[5] = 2.f * (f.qy * (m01 + m10) + f.qz * (m02 + m20) + f.qr * (m12 - m21)) - 4.f * f.qx * (m11 + m22);
+    g[6] = 2.f * (f.qx * (m01 + m10) + f.qr * (m20 - m02) + f.qz * (m12 + m21)) - 4.f * f.qy * (m00 + m22);
+    g[7] = 2.f * (f.qr * (m01 - m10) + f.qx * (m02 + m20) + f.qy * (m12 + m21)) - 4.f * f.qz * (m00 + m11);
+    T = nextT;
+}
+
 // 16 real SH basis values of a direction (radianceFromSpH, gaussianParticles.cuh:61-93)
 __device__ __forceinline__ void sh_basis16(int deg, float x, float y, float z, float b[16]) {
 #pragma unroll

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 import b200_native as native
-from b200_native import cfg_get, ptr
+from b200_native import NHT_FEATURE_DIM, cfg_get, ptr
 
 
 class ShutterType(enum.IntEnum):  # bindings.cpp:36-42
@@ -130,27 +130,14 @@ def _native_config(conf) -> native.Config:
     return cfg
 
 
-NHT_FEATURE_DIM = 48  # model.nht_features.dim of the shipped NHT configs (configs/base_gs.yaml): 4 tetrahedron vertices x 12
-
-
 def _nht_config(conf):
     """model.feature_type -> None (SH radiance) or the NHT settings the kernels take: {"half": render.particle_feature_half}.
-    Only the reference's shipped NHT configuration is built (configs/base_gs.yaml: dim 48, barycentric, sincos with 1 frequency);
+    The shipped NHT configuration only (b200_native.nht_feature_config, shared with the 3DGRT tracer), and not with the k-buffer;
     anything else raises NotImplementedError naming the key.  Pure config logic: needs no GPU."""
-    kind = str(cfg_get(conf, "model.feature_type", "sh")).lower()
-    if kind == "sh":
-        return None
-    if kind != "nht":
-        raise NotImplementedError(f"model.feature_type={kind!r}: the 3DGUT tracer renders 'sh' or 'nht'")
-    built = (("model.nht_features.dim", NHT_FEATURE_DIM), ("model.nht_features.activation.type", "sincos"),
-             ("model.nht_features.activation.num_frequencies", 1), ("model.nht_features.interpolation_type", "barycentric"))
-    for key, want in built:
-        got = cfg_get(conf, key, want)
-        if (str(got).lower() if isinstance(want, str) else int(got)) != want:
-            raise NotImplementedError(f"{key}={got!r}: NHT features are built for {key}={want!r} only")
-    if int(cfg_get(conf, "render.splat.k_buffer_size", 0)) > 0:
+    nht = native.nht_feature_config(conf, "3DGUT")
+    if nht is not None and int(cfg_get(conf, "render.splat.k_buffer_size", 0)) > 0:
         raise NotImplementedError("render.splat.k_buffer_size > 0: NHT features are not built with the k-buffer")
-    return {"half": bool(cfg_get(conf, "render.particle_feature_half", False))}
+    return nht
 
 
 def _c(t: torch.Tensor) -> torch.Tensor:

@@ -10,6 +10,7 @@
  *   grtb200_build_bvh_packed   the same build from the [N,12] particle record (ours: the no-autograd training step)
  *   grtb200_trace              <- OptixTracer::trace   -> __raygen__rg            (src/optixTracer.cpp:893-960, src/kernels/cuda/referenceOptix.cu:103-186)
  *   grtb200_trace_bwd          <- OptixTracer::traceBwd -> bwd __raygen__rg        (src/optixTracer.cpp:962-1031, src/kernels/cuda/referenceBwdOptix.cu:103-170)
+ *   grtb200_trace_nht / grtb200_trace_bwd_nht  the same with NHT features         (src/kernels/cuda/referenceSlangOptix.cu, referenceSlangBwdOptix.cu)
  *
  * Layouts (fp32): particles [N,12] = pos3, density, quat(wxyz), scale3, pad; sph [N,48]; rays_o/rays_d [B,H,W,3]
  * (R = B*H*W rays, ray space); ray_to_world = first three rows of T_to_world, row major [3,4], HOST pointer
@@ -75,6 +76,23 @@ int grtb200_trace_bwd(grtb200_ctx* ctx, void* stream, int64_t n, const float* pa
                       const float* rays_d, const float* ray_to_world_host, const float* out_rgb, const float* out_alpha,
                       const float* out_dist, const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles,
                       float* d_sph);
+
+/* Neural Harmonic Texture (NHT) features instead of SH radiance (model.feature_type: nht; <- the referenceSlang / referenceSlangBwd
+ * pipelines, src/kernels/cuda/referenceSlangOptix.cu:103-200, referenceSlangBwdOptix.cu:103-230).  features: [N,feature_dim] rows,
+ * fp32, or fp16 when features_half != 0; only feature_dim = 48 (4 tetrahedron vertices x 12, barycentric, sincos x 1) is built, other
+ * dims are refused.  out_features [R,24] fp32 (sin / cos of the 12 blended features), d_features_out its gradient, d_features [N,48]
+ * fp32 (zeroed by the call).  Every other argument, output and the hit-list replay are as in grtb200_trace / grtb200_trace_bwd; the
+ * backward replays only the lists of an NHT forward with the same feature row layout and otherwise re-traces. */
+int grtb200_trace_nht(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles, const void* features, int32_t feature_dim,
+                      int32_t features_half, float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                      const float* rays_d, const float* ray_to_world_host, float* out_features, float* out_alpha, float* out_dist,
+                      float* out_hits, float* visibility);
+
+int grtb200_trace_bwd_nht(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles, const void* features, int32_t feature_dim,
+                          int32_t features_half, float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                          const float* rays_d, const float* ray_to_world_host, const float* out_features, const float* out_alpha,
+                          const float* out_dist, const float* d_features_out, const float* d_alpha, const float* d_dist, float* d_particles,
+                          float* d_features);
 
 /* Scene bounding box of the last build: min xyz, max xyz (host array of 6 floats; synchronises). */
 int grtb200_scene_aabb(grtb200_ctx* ctx, float* aabb6);
