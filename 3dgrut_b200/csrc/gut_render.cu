@@ -41,209 +41,28 @@ constexpr int kBatch = 256;
 // the switch on and off (tests/test_gut_parity_gpu.py::test_subtile_culling_is_bit_identical).
 
 // ----------------------------------------------------------------------------------------------------------
-// G6 forward
-// staged record, 5 x float4: rows of M = diag(1/s) R^T with the particle position in .w, then (s, density), (rgb)
+// G6 forward: the shared walk (render_tile.cuh) with the radiance payload.
+// staged record, 5 x float4: FwdRecords (rows of M = diag(1/s) R^T with the particle position in .w, then (s, density)), then (rgb)
 
-struct FwdSmem {
-    float4 m0[kBatch], m1[kBatch], m2[kBatch], sd[kBatch], col[kBatch];
+struct FwdSmem : FwdRecords<kBatch> {
+    float4 col[kBatch];
 };
 
-// exact test + compositing of one (pixel, staged entry j) pair; returns whether the accept test passed (before the t-range test:
-// the reference's backward does not re-apply the range test, DESIGN.md section 5)
-template <int DEG, bool UNIFORM>
-__device__ __forceinline__ bool forward_pair(const FrameConfig& cfg, const FwdSmem& sm, int j, const Ray& ray, bool& alive, float& T, float& cr,
-                                             float& cg, float& cb, float& dist, uint32_t& hits) {
-    const float4 m0 = sm.m0[j], m1 = sm.m1[j], m2 = sm.m2[j];
-    float gox, goy, goz;
-    if (UNIFORM) {
-        gox = m0.w; goy = m1.w; goz = m2.w;
-    } else {
-        const float vx = ray.ox - m0.w, vy = ray.oy - m1.w, vz = ray.oz - m2.w;
-        gox = m0.x * vx + m0.y * vy + m0.z * vz;
-        goy = m1.x * vx + m1.y * vy + m1.z * vz;
-        goz = m2.x * vx + m2.y * vy + m2.z * vz;
+struct RadiancePayload {
+    float4* col;
+    const float* __restrict__ rgb;
+    float cr = 0.f, cg = 0.f, cb = 0.f;
+    __device__ __forceinline__ void entry(int slot, uint32_t idx) {
+        col[slot] = make_float4(fmaxf(rgb[idx * 3 + 0], 0.f), fmaxf(rgb[idx * 3 + 1], 0.f), fmaxf(rgb[idx * 3 + 2], 0.f), 0.f);
     }
-    const float ax = m0.x * ray.dx + m0.y * ray.dy + m0.z * ray.dz;
-    const float ay = m1.x * ray.dx + m1.y * ray.dy + m1.z * ray.dz;
-    const float az = m2.x * ray.dx + m2.y * ray.dy + m2.z * ray.dz;
-    const float l = ax * ax + ay * ay + az * az;
-    const float il = l > 0.f ? rsqrtf(l) : 1.f;
-    const float gdx = ax * il, gdy = ay * il, gdz = az * il;
-    const float ccx = gdy * goz - gdz * goy, ccy = gdz * gox - gdx * goz, ccz = gdx * goy - gdy * gox;
-    const float gray = ccx * ccx + ccy * ccy + ccz * ccz;
-    const float gres = kernel_response<DEG>(gray);
-    const float4 sd = sm.sd[j];
-    const float alpha = fminf(cfg.max_alpha, gres * sd.w);
-    const bool accept = (gres > cfg.min_kernel_density) && (alpha > cfg.min_alpha);
-    if (accept) {
-        const float pd = -(gdx * gox + gdy * goy + gdz * goz);
-        const float hx = sd.x * gdx * pd, hy = sd.y * gdy * pd, hz = sd.z * gdz * pd;
-        const float t = sqrtf(hx * hx + hy * hy + hz * hz);
-        if ((t > ray.tmin) && (t < ray.tmax)) {
-            const float w = alpha * T;
-            dist += t * w;
-            T *= (1.f - alpha);
-            if (w > 0.f) {
-                const float4 c = sm.col[j];
-                cr += c.x * w;
-                cg += c.y * w;
-                cb += c.z * w;
-                hits++;
-            }
-            if (T < cfg.min_transmittance) alive = false;
-        }
+    __device__ __forceinline__ void batch(const uint32_t* __restrict__, uint32_t, int, int) {}
+    __device__ __forceinline__ void add(int j, float w, float, float, float) {
+        const float4 c = col[j];
+        cr += c.x * w;
+        cg += c.y * w;
+        cb += c.z * w;
     }
-    return accept;
-}
-
-// Work counters (debug entry point gutb200_debug_work_counters; COUNT instantiations never run on the product path).
-//   0 tests_ref   (pixel, entry) pairs the reference's loop evaluates: every live pixel tests every entry of its tile list
-//   1 tests_exec  lane-level exact tests our forward executes after sub-tile culling
-//   2 hits        accepted pairs (the set the backward's adjoint runs on)
-//   3 fwd_iters   warp iterations of the forward's exact test     4 hit_iters  warp iterations with >= 1 accepting lane (= backward's iterations)
-//   5 screens     lane-level sub-tile culling screens             6 bwd_lanes  live lanes summed over hit_iters (lane-level tests of the backward)
-//   7 iters16 / 8 iters8   backward iterations when half-warps (4x4 pixels) / quarter-warps (4x2) walk their own entries in lockstep
-//   9 sub16_hits / 10 sub8_hits   (half-warp, entry) / (quarter-warp, entry) pairs with >= 1 accepting lane (= gradient rows flushed)
-struct WorkCounters {
-    unsigned long long v[16];
 };
-
-
-template <int DEG, bool UNIFORM, bool COUNT>
-__device__ __forceinline__ void forward_tile(const FrameConfig& cfg, FwdSmem& sm, const WarpFrame& wf, const Ray& ray, float o0x, float o0y,
-                                             float o0z, int tid, uint32_t begin, uint32_t end, const float* __restrict__ particles,
-                                             const float* __restrict__ rgb, const uint32_t* __restrict__ sorted_values,
-                                             uint32_t* __restrict__ hit_words, bool& alive, float& T, float& cr, float& cg, float& cb,
-                                             float& dist, uint32_t& hits, WorkCounters* __restrict__ ctr) {
-    const int lane = tid & 31;
-    unsigned long long c_ref = 0, c_exec = 0, c_hits = 0, c_iters = 0, c_hit_iters = 0, c_screens = 0, c_bwd_lanes = 0;
-    unsigned long long c_iters16 = 0, c_iters8 = 0, c_sub16 = 0, c_sub8 = 0;
-    for (uint32_t base = begin; base < end; base += kBatch) {
-        if (__syncthreads_and(!alive)) break;
-        const uint32_t k = base + tid;
-        if (k < end) {
-            const uint32_t idx = sorted_values[k];
-            const float4* p4 = reinterpret_cast<const float4*>(particles) + static_cast<size_t>(idx) * 3;
-            const float4 a = __ldg(p4), q = __ldg(p4 + 1), s = __ldg(p4 + 2);
-            const float r = q.x, x = q.y, y = q.z, z = q.w;
-            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, xz = x * z, yz = y * z;
-            const float rx = r * x, ry = r * y, rz = r * z;
-            const float isx = 1.0f / s.x, isy = 1.0f / s.y, isz = 1.0f / s.z;
-            float4 m0 = make_float4(isx * (1.f - 2.f * (yy + zz)), isx * (2.f * (xy + rz)), isx * (2.f * (xz - ry)), a.x);
-            float4 m1 = make_float4(isy * (2.f * (xy - rz)), isy * (1.f - 2.f * (xx + zz)), isy * (2.f * (yz + rx)), a.y);
-            float4 m2 = make_float4(isz * (2.f * (xz + ry)), isz * (2.f * (yz - rx)), isz * (1.f - 2.f * (xx + yy)), a.z);
-            if (UNIFORM) {  // .w carries the canonical origin instead of the particle position
-                const float vx = o0x - a.x, vy = o0y - a.y, vz = o0z - a.z;
-                m0.w = m0.x * vx + m0.y * vy + m0.z * vz;
-                m1.w = m1.x * vx + m1.y * vy + m1.z * vz;
-                m2.w = m2.x * vx + m2.y * vy + m2.z * vz;
-            }
-            sm.m0[tid] = m0;
-            sm.m1[tid] = m1;
-            sm.m2[tid] = m2;
-            sm.sd[tid] = make_float4(s.x, s.y, s.z, a.w);
-            sm.col[tid] = make_float4(fmaxf(rgb[idx * 3 + 0], 0.f), fmaxf(rgb[idx * 3 + 1], 0.f), fmaxf(rgb[idx * 3 + 2], 0.f), 0.f);
-        }
-        __syncthreads();
-        const int count = min(kBatch, static_cast<int>(end - base));
-        // this warp's hit words of the batch: bit e of word c/32 = "some pixel of the warp's 8x4 block accepted entry c + e" -- the backward
-        // walks only those entries (a necessary condition of its own exact test, so it drops nothing it would have accepted)
-        uint32_t* words = hit_words + (static_cast<size_t>(base - begin) >> 5) * kWordsPerChunk + (tid >> 5) * 4;
-        const int quarter = lane_quarter(lane);
-        const unsigned my_quarter = quarter_lanes(quarter);
-        const bool writer = (lane & 0x0B) == 0;  // lanes 0, 4, 16, 20: one per quarter
-        if (UNIFORM) {
-            // chunks of 32 entries: lane k screens entry k against the warp's pixel block, the warp walks the survivors
-            for (int c = 0; c < count; c += 32) {
-                if (!__any_sync(kFull, alive)) break;
-                const int e = c + lane;
-                bool cand = e < count;
-                if (wf.on && cand) {
-                    const float4 m0 = sm.m0[e], m1 = sm.m1[e], m2 = sm.m2[e];
-                    cand = block_candidate<DEG>(cfg, wf, m0.x, m0.y, m0.z, m1.x, m1.y, m1.z, m2.x, m2.y, m2.z, m0.w, m1.w, m2.w, sm.sd[e].w);
-                    if (COUNT) c_screens++;
-                }
-                unsigned todo = __ballot_sync(kFull, cand);
-                uint32_t word = 0;
-                int prev = c;
-                while (todo) {
-                    const int b = __ffs(todo) - 1;
-                    const int j = c + b;
-                    todo &= todo - 1;
-                    int live_n = 0;
-                    if (COUNT) {
-                        live_n = __popc(__ballot_sync(kFull, alive));
-                        c_ref += static_cast<unsigned long long>(live_n) * (j - prev + 1);
-                        prev = j + 1;
-                        c_iters++;
-                        if (alive) c_exec++;
-                    }
-                    bool acc = false;
-                    if (alive) acc = forward_pair<DEG, true>(cfg, sm, j, ray, alive, T, cr, cg, cb, dist, hits);
-                    const unsigned accs = __ballot_sync(kFull, acc);
-                    if (accs & my_quarter) word |= 1u << b;  // this lane's quarter (4x2 pixels) accepted entry j
-                    if (COUNT && accs) {
-                        c_hit_iters++;
-                        c_bwd_lanes += live_n;
-                        c_hits += acc ? 1 : 0;
-                    }
-                }
-                if (COUNT) {
-                    const unsigned live = __ballot_sync(kFull, alive);
-                    c_ref += static_cast<unsigned long long>(__popc(live)) * (min(c + 32, count) - prev);
-                    // lockstep iteration counts of the sub-block walks: halves split by b2, quarters by (b2, b4)
-                    const uint32_t wq = word, wh = word | __shfl_xor_sync(kFull, word, 16);
-                    const int p16 = __popc(wh), p8 = __popc(wq);
-                    const int m16 = max(p16, __shfl_xor_sync(kFull, p16, 4));
-                    int m8 = max(p8, __shfl_xor_sync(kFull, p8, 4));
-                    m8 = max(m8, __shfl_xor_sync(kFull, m8, 16));
-                    c_iters16 += m16;
-                    c_iters8 += m8;
-                    c_sub16 += p16 + __shfl_xor_sync(kFull, p16, 4);
-                    int s8 = p8 + __shfl_xor_sync(kFull, p8, 4);
-                    s8 += __shfl_xor_sync(kFull, s8, 16);
-                    c_sub8 += s8;
-                }
-                if (writer) words[(c >> 5) * kWordsPerChunk + quarter] = word;
-            }
-        } else {
-            // per-pixel origins: no warp-level screening; the backward gets all-ones words for these tiles
-            if (writer)
-                for (int c = 0; c < count; c += 32) words[(c >> 5) * kWordsPerChunk + quarter] = 0xFFFFFFFFu;
-            for (int j = 0; alive && j < count; ++j) {
-                const bool acc = forward_pair<DEG, false>(cfg, sm, j, ray, alive, T, cr, cg, cb, dist, hits);
-                if (COUNT) {
-                    c_exec++;
-                    c_hits += acc ? 1 : 0;
-                }
-            }
-        }
-    }
-    if (COUNT) {
-        // c_ref, c_iters, c_hit_iters are warp-uniform (lane 0 reports); the others are per lane
-        if (!UNIFORM) c_ref = 0;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            c_exec += __shfl_xor_sync(kFull, c_exec, o);
-            c_hits += __shfl_xor_sync(kFull, c_hits, o);
-            c_screens += __shfl_xor_sync(kFull, c_screens, o);
-        }
-        if (lane == 0) {
-            if (!UNIFORM) c_ref = c_exec;
-            atomicAdd(&ctr->v[0], c_ref);
-            atomicAdd(&ctr->v[1], c_exec);
-            atomicAdd(&ctr->v[2], c_hits);
-            atomicAdd(&ctr->v[3], c_iters);
-            atomicAdd(&ctr->v[4], c_hit_iters);
-            atomicAdd(&ctr->v[5], c_screens);
-            atomicAdd(&ctr->v[6], c_bwd_lanes);
-            atomicAdd(&ctr->v[7], c_iters16);
-            atomicAdd(&ctr->v[8], c_iters8);
-            atomicAdd(&ctr->v[9], c_sub16);
-            atomicAdd(&ctr->v[10], c_sub8);
-        }
-    }
-}
 
 template <int DEG, bool COUNT>
 __global__ void __launch_bounds__(kTilePixels) render_forward_kernel(FrameCamera cam, FrameConfig cfg,
@@ -258,37 +77,20 @@ __global__ void __launch_bounds__(kTilePixels) render_forward_kernel(FrameCamera
                                                                      float* __restrict__ out_rgba, float* __restrict__ out_dist,
                                                                      float* __restrict__ out_hits, WorkCounters* __restrict__ ctr) {
     __shared__ FwdSmem sm;
-    const int tile = tile_order[blockIdx.x];  // heaviest tiles first (tile_scan_kernel's order): shortens the tail of the grid
     const int tid = threadIdx.x;
-    int px, py;
-    tile_pixel(tile, cam.grid_x, tid, px, py);
-    const bool inside = (px < cam.width) && (py < cam.height);
-    const int64_t pix = static_cast<int64_t>(py) * cam.width + px;
-
-    Ray ray;
-    ray.alive = false;
-    if (inside) ray = make_ray(cam, rays_o, rays_d, pix);
-    const bool valid = inside && ray.alive;
-    float o0x, o0y, o0z;
-    const bool uniform = tile_common_origin(cam, rays_o, tile, inside, pix, o0x, o0y, o0z);
-    const WarpFrame wf = make_warp_frame(cam, ray, valid, uniform && (cfg.subtile_culling & 2), tid & 31);
-
-    float T = 1.f, cr = 0.f, cg = 0.f, cb = 0.f, dist = 0.f;
+    const TileRay tr = tile_ray(cam, rays_o, rays_d, tile_order, tid);
+    RadiancePayload pay{sm.col, rgb};
+    float T = 1.f, dist = 0.f;
     uint32_t hits = 0;
-    bool alive = valid;
-    const uint32_t begin = ranges[tile * 2], end = ranges[tile * 2 + 1];
-    uint32_t* words = hit_words + static_cast<size_t>(chunk_base[tile]) * kWordsPerChunk;
-    if (uniform)
-        forward_tile<DEG, true, COUNT>(cfg, sm, wf, ray, o0x, o0y, o0z, tid, begin, end, particles, rgb, sorted_values, words, alive, T, cr, cg, cb, dist, hits, ctr);
-    else
-        forward_tile<DEG, false, COUNT>(cfg, sm, wf, ray, o0x, o0y, o0z, tid, begin, end, particles, rgb, sorted_values, words, alive, T, cr, cg, cb, dist, hits, ctr);
+    forward_list<DEG, COUNT>(cam, cfg, sm, pay, tr, tid, rays_o, particles, sorted_values, ranges, chunk_base, hit_words, T, dist, hits, ctr);
     if (COUNT) return;  // the counting pass leaves the frame's outputs alone
 
-    if (valid) {  // finalizeRay (rayPayload.cuh:160-193); invalid rays keep the initial buffer values
-        reinterpret_cast<float4*>(out_rgba)[pix] = make_float4(cr, cg, cb, 1.0f - T);
+    const int64_t pix = tr.pix;
+    if (tr.valid) {  // finalizeRay (rayPayload.cuh:160-193); invalid rays keep the initial buffer values
+        reinterpret_cast<float4*>(out_rgba)[pix] = make_float4(pay.cr, pay.cg, pay.cb, 1.0f - T);
         out_dist[pix] = dist;
         out_hits[pix] = static_cast<float>(hits);
-    } else if (inside) {
+    } else if (tr.inside) {
         reinterpret_cast<float4*>(out_rgba)[pix] = make_float4(0.f, 0.f, 0.f, 0.f);
         out_dist[pix] = 1e06f;  // torch::ones(...)*1e6 (splatRaster.cpp:213)
         out_hits[pix] = 0.f;
@@ -315,12 +117,7 @@ __global__ void __launch_bounds__(kTilePixels) render_forward_kernel(FrameCamera
 // give  grduGrd = (-(grd . gro) / |grdu|) groGrd  exactly, so the cross product, the dot product and the three-term normalisation
 // adjoint of (:684-731) are one multiply; the terms that cancel analytically there (grd |gro|^2) are never formed.
 //
-// staged record, 6 x float4:
-//   r0, r1, r2 = rows of quaternionWXYZToMatrix (columns of R); .w = canonical frame origin S^-1 R (o_f - mu) (FAST) | position (GENERAL)
-//   sc = scale.xyz, density     is = 1/scale.xyz, _     cl = clamped rgb, particle index bits
-// The rotation rows are kept apart from 1/scale (the forward stages M = S^-1 R^T): the backward's accept test applies 1/s after the
-// rotation, as the reference's adjoint does.  With the forward's record the test moves by the last bits, borderline pairs flip, and
-// on a 500-Gaussian scene the gradients drifted from 4.7e-4 to 1.8e-3 relative to the CPU restatement of the reference.
+// staged record, 6 x float4: BwdRecords (r0, r1, r2, sc, is; render_tile.cuh), then cl = clamped rgb, particle index bits.
 //
 // The gradient rows of one lockstep iteration are summed through a per-warp scratch:
 //   every lane stores its row (g[0..15], the depth slots 16..18 when the warp carries a distance gradient; zeros without a hit) as
@@ -333,8 +130,8 @@ __global__ void __launch_bounds__(kTilePixels) render_forward_kernel(FrameCamera
 // the depth slots).  render_backward on C2 (H100 80GB HBM3, 700 W, 1980 MHz, three runs each): 0.454-0.460 -> 0.417-0.422 ms; with the rgb / opacity
 // loss (no depth slots) unchanged at 0.354-0.358 ms.
 
-struct BwdSmem {
-    float4 r0[kBatch], r1[kBatch], r2[kBatch], sc[kBatch], is[kBatch], cl[kBatch];
+struct BwdSmem : BwdRecords<kBatch> {
+    float4 cl[kBatch];
     uint32_t hw[(kBatch / 32) * kWordsPerChunk];        // the forward's hit words of this batch, [chunk][warp][quarter]
     float4 rows[kTilePixels / 32][32 * kGradRow / 4];  // gradient rows of one lockstep iteration, [warp][lane * 5 + column]
 };
@@ -359,101 +156,29 @@ __device__ __forceinline__ int sub_rank(int lane) {
 }
 
 
-// exact test + adjoint of one (pixel, staged entry j) pair (processHitBwd, gaussianParticles.cuh:484-751); fills g[] and returns true on a hit
-template <int DEG, bool FAST>
-__device__ __forceinline__ bool backward_pair(const FrameConfig& cfg, const BwdSmem& sm, int j, const Ray& ray, float dox, float doy, float doz,
-                                              bool depth_grads, BwdRay& st, bool& alive, float (&g)[16], float (&ex)[3]) {
-    const float4 r0 = sm.r0[j], r1 = sm.r1[j], r2 = sm.r2[j], sc = sm.sc[j], is = sm.is[j];
-    float gox, goy, goz;                                                                          // gro
-    float pcx = 0.f, pcy = 0.f, pcz = 0.f;
-    if (FAST) {
-        gox = r0.w; goy = r1.w; goz = r2.w;
-    } else {
-        pcx = ray.ox - r0.w; pcy = ray.oy - r1.w; pcz = ray.oz - r2.w;                              // gposc
-        gox = is.x * (r0.x * pcx + r0.y * pcy + r0.z * pcz);
-        goy = is.y * (r1.x * pcx + r1.y * pcy + r1.z * pcz);
-        goz = is.z * (r2.x * pcx + r2.y * pcy + r2.z * pcz);
-    }
-    const float drx = r0.x * ray.dx + r0.y * ray.dy + r0.z * ray.dz;                                // rayDirR
-    const float dry = r1.x * ray.dx + r1.y * ray.dy + r1.z * ray.dz;
-    const float drz = r2.x * ray.dx + r2.y * ray.dy + r2.z * ray.dz;
-    const float ux = is.x * drx, uy = is.y * dry, uz = is.z * drz;                                  // grdu
-    const float l = ux * ux + uy * uy + uz * uz;
-    const float il = l > 0.f ? rsqrtf(l) : 1.f;
-    const float gdx = ux * il, gdy = uy * il, gdz = uz * il;                                        // grd
-    const float ccx = gdy * goz - gdz * goy, ccy = gdz * gox - gdx * goz, ccz = gdx * goy - gdy * gox;  // gcrod
-    const float gray = ccx * ccx + ccy * ccy + ccz * ccz;
-    const float gres = kernel_response<DEG>(gray);
-    const float dns = sc.w;
-    const float alpha = fminf(cfg.max_alpha, gres * dns);
-    if (!((gres > cfg.min_kernel_density) && (alpha > cfg.min_alpha))) return false;
+// per-pixel backward state (initializeBackwardRay, kernels/cuda/common/rayPayloadBackward.cuh:31-73)
+struct BwdRay {
+    float Cix, Ciy, Ciz, Cgx, Cgy, Cgz, Tint, Tgrad, Dint, Dgrad;
+    float T, Cx, Cy, Cz, D;
+};
 
-    const float4 cl = sm.cl[j];
-    const float T = st.T;
-    const float weight = alpha * T;
-    const float nextT = (1.f - alpha) * T;
-    const bool last = nextT <= cfg.min_transmittance;
-    const float inv_next = last ? 0.f : 1.0f / nextT;
-    const float pd = -(gdx * gox + gdy * goy + gdz * goz);
-
-    // depth branch (:545-580); skipped by warps whose pixels carry no distance gradient (an RGB-only loss)
-    float a_hit = 0.f, sd = 0.f, hgx = 0.f, hgy = 0.f, hgz = 0.f, ddx = 0.f, ddy = 0.f, ddz = 0.f;
-    if (depth_grads) {
-        ddx = gdx * pd; ddy = gdy * pd; ddz = gdz * pd;                                             // grdd
-        const float hx = sc.x * ddx, hy = sc.y * ddy, hz = sc.z * ddz;                              // grds
-        const float gsq = hx * hx + hy * hy + hz * hz;
-        const float gdist = sqrtf(gsq);
-        st.D += weight * gdist;
-        const float resD = fmaxf((st.Dint - st.D) * inv_next, 0.f);
-        a_hit = (gdist - resD) * T * st.Dgrad;
-        const float hs = gsq > 0.f ? (weight / gdist) * st.Dgrad : 0.f;
-        hgx = hx * hs; hgy = hy * hs; hgz = hz * hs;                                                // grdsRayHitGrd
-        sd = hgx * sc.x * gdx + hgy * sc.y * gdy + hgz * sc.z * gdz;                                // grdScaledDot
-    }
-    // opacity branch (:586-587)
-    const float resT = alpha < 0.999999f ? st.Tint / (1.f - alpha) : T;
-    const float a_dns = resT * -st.Tgrad;
+// the radiance terms of backward_pair (render_tile.cuh): g[13..15] = d rgb, depth slots 16..18
+struct RadianceHit {
+    static constexpr int kDepthSlot = 16;
+    static constexpr bool kHitPoint = false;
+    float4 cl;
+    __device__ __forceinline__ void at_hit(const BwdSmem& sm, int j, const BwdRay&, float, float, float, float, float (&)[19]) { cl = sm.cl[j]; }
     // radiance branch (:602-612)
-    g[13] = st.Cgx * weight; g[14] = st.Cgy * weight; g[15] = st.Cgz * weight;
-    st.Cx += weight * cl.x; st.Cy += weight * cl.y; st.Cz += weight * cl.z;
-    const float rcx = fmaxf((st.Cix - st.Cx) * inv_next, 0.f);
-    const float rcy = fmaxf((st.Ciy - st.Cy) * inv_next, 0.f);
-    const float rcz = fmaxf((st.Ciz - st.Cz) * inv_next, 0.f);
-    const float common = a_hit + a_dns + T * ((cl.x - rcx) * st.Cgx + (cl.y - rcy) * st.Cgy + (cl.z - rcz) * st.Cgz);
-    g[3] = gres * common;                                                                           // d density (:624-627)
-    const float gray_g = kernel_response_grad<DEG>(gray, gres, dns * common);                       // (:639-648)
-    // gray = |grd x gro|^2  (:684-702)
-    const float kx = 2.f * ccx * gray_g, ky = 2.f * ccy * gray_g, kz = 2.f * ccz * gray_g;          // gcrodGrd
-    float go_gx = ky * gdz - kz * gdy, go_gy = kz * gdx - kx * gdz, go_gz = kx * gdy - ky * gdx;    // groGrd
-    float ug_x, ug_y, ug_z;                                                                         // grduGrd
-    if (depth_grads) {
-        // + grdRayHitGrd = S grdsRayHitGrd pd - gro sd, groRayHitGrd = -grd sd (:560-580), then grd = normalize(grdu) (:729-731): with
-        // P = k x grd (the groGrd above) the projection (I - grd grd^T) of grdGrd = gro x k + S hg pd - gro sd is, term by term,
-        // pd P,  pd (S hg - grd sd)  and  -sd (gro + pd grd), i.e.  grduGrd = (pd (P + S hg - 2 sd grd) - sd gro) / |grdu|
-        const float sd2 = 2.f * sd;
-        const float vx = (go_gx + sc.x * hgx) - sd2 * gdx, vy = (go_gy + sc.y * hgy) - sd2 * gdy, vz = (go_gz + sc.z * hgz) - sd2 * gdz;
-        ug_x = il * (pd * vx - sd * gox); ug_y = il * (pd * vy - sd * goy); ug_z = il * (pd * vz - sd * goz);
-        go_gx -= gdx * sd; go_gy -= gdy * sd; go_gz -= gdz * sd;
-        ex[0] = ddx * hgx; ex[1] = ddy * hgy; ex[2] = ddz * hgz;                                     // gsclRayHitGrd (:705-713)
-    } else {  // the same chain in closed form (section comment): grduGrd = (pd / |grdu|) groGrd
-        const float tq = pd * il;
-        ug_x = tq * go_gx; ug_y = tq * go_gy; ug_z = tq * go_gz;
+    __device__ __forceinline__ float common(const FrameConfig&, BwdRay& st, float T, float weight, float inv_next, float, float partial,
+                                            float (&g)[19]) {
+        g[13] = st.Cgx * weight; g[14] = st.Cgy * weight; g[15] = st.Cgz * weight;
+        st.Cx += weight * cl.x; st.Cy += weight * cl.y; st.Cz += weight * cl.z;
+        const float rcx = fmaxf((st.Cix - st.Cx) * inv_next, 0.f);
+        const float rcy = fmaxf((st.Ciy - st.Cy) * inv_next, 0.f);
+        const float rcz = fmaxf((st.Ciz - st.Cz) * inv_next, 0.f);
+        return partial + T * ((cl.x - rcx) * st.Cgx + (cl.y - rcy) * st.Cgy + (cl.z - rcz) * st.Cgz);
     }
-    g[0] = go_gx; g[1] = go_gy; g[2] = go_gz;          // canonical: G8 turns the sums into d pos, the gro part of d scale and of d quat
-    // W rows: grduGrd_i * d  (+ groGrd_i * (o - o_f) for pixels off the frame origin); G8 scales row i by 1/s_i (rayDirRGrd, gposcrGrd)
-    // and contracts it with R for d scale (:733-738) and with the quaternion Jacobian for d quat (matmul_bw_quat, :719-747)
-    g[4] = ug_x * ray.dx; g[5] = ug_x * ray.dy; g[6] = ug_x * ray.dz;
-    g[7] = ug_y * ray.dx; g[8] = ug_y * ray.dy; g[9] = ug_y * ray.dz;
-    g[10] = ug_z * ray.dx; g[11] = ug_z * ray.dy; g[12] = ug_z * ray.dz;
-    if (!FAST) {
-        g[4] += go_gx * dox; g[5] += go_gx * doy; g[6] += go_gx * doz;
-        g[7] += go_gy * dox; g[8] += go_gy * doy; g[9] += go_gy * doz;
-        g[10] += go_gz * dox; g[11] += go_gz * doy; g[12] += go_gz * doz;
-    }
-    st.T = nextT;
-    if (nextT < cfg.min_transmittance) alive = false;
-    return true;
-}
+};
 
 template <int DEG, bool FAST, int SUBL>
 __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& sm, const Ray& ray, float ofx, float ofy, float ofz, int tid,
@@ -470,40 +195,12 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
     const int col = sub_rank<SUBL>(lane);
     const int cols = depth_grads ? 5 : 4;
     float4* rows = sm.rows[tid >> 5];
-    for (uint32_t base = begin; base < end; base += kBatch) {
-        if (__syncthreads_and(!alive)) break;
-        const uint32_t k = base + tid;
-        {   // 8 chunks x 8 warps x 4 quarters = one word per thread
-            const uint32_t chunk = (base - begin) / 32 + (tid >> 5);
-            const bool in_list = base + (tid >> 5) * 32 < end;
-            sm.hw[tid] = (use_words && in_list) ? hit_words[static_cast<size_t>(chunk) * kWordsPerChunk + (tid & 31)] : 0xFFFFFFFFu;
-        }
-        if (k < end) {
-            const uint32_t idx = sorted_values[k];
-            const float4* p4 = reinterpret_cast<const float4*>(particles) + static_cast<size_t>(idx) * 3;
-            const float4 a = __ldg(p4), q = __ldg(p4 + 1), s = __ldg(p4 + 2);
-            const float r = q.x, x = q.y, y = q.z, z = q.w;
-            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, xz = x * z, yz = y * z;
-            const float rx = r * x, ry = r * y, rz = r * z;
-            float4 t0 = make_float4(1.f - 2.f * (yy + zz), 2.f * (xy + rz), 2.f * (xz - ry), a.x);
-            float4 t1 = make_float4(2.f * (xy - rz), 1.f - 2.f * (xx + zz), 2.f * (yz + rx), a.y);
-            float4 t2 = make_float4(2.f * (xz + ry), 2.f * (yz - rx), 1.f - 2.f * (xx + yy), a.z);
-            if (FAST) {  // .w carries the canonical frame origin instead of the particle position
-                const float vx = ofx - a.x, vy = ofy - a.y, vz = ofz - a.z;
-                t0.w = (t0.x * vx + t0.y * vy + t0.z * vz) / s.x;
-                t1.w = (t1.x * vx + t1.y * vy + t1.z * vz) / s.y;
-                t2.w = (t2.x * vx + t2.y * vy + t2.z * vz) / s.z;
-            }
-            sm.r0[tid] = t0;
-            sm.r1[tid] = t1;
-            sm.r2[tid] = t2;
-            sm.sc[tid] = make_float4(s.x, s.y, s.z, a.w);
-            sm.is[tid] = make_float4(1.0f / s.x, 1.0f / s.y, 1.0f / s.z, 0.f);
-            sm.cl[tid] = make_float4(fmaxf(rgb[idx * 3 + 0], 0.f), fmaxf(rgb[idx * 3 + 1], 0.f), fmaxf(rgb[idx * 3 + 2], 0.f),
-                                     __uint_as_float(idx));
-        }
-        __syncthreads();
-        const int count = min(kBatch, static_cast<int>(end - base));
+    backward_batches<FAST>(sm, sm.hw, ofx, ofy, ofz, tid, begin, end, particles, sorted_values, hit_words, use_words, alive,
+        [&](uint32_t idx) {
+            sm.cl[tid] = make_float4(fmaxf(rgb[idx * 3 + 0], 0.f), fmaxf(rgb[idx * 3 + 1], 0.f), fmaxf(rgb[idx * 3 + 2], 0.f), __uint_as_float(idx));
+        },
+        [](uint32_t, int) {},
+        [&](int count) {
         // chunks of 32 entries.  Every sub-block of the warp walks ITS OWN entries -- those some pixel of the sub-block accepted in the
         // forward (hit words) -- in lockstep with the other sub-blocks: one pass of the adjoint serves up to 32 / SUBL particles, and
         // the reduction tree is log2(SUBL) levels deep.
@@ -519,12 +216,11 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
                 const bool act = todo != 0u;
                 const int j = act ? c + __ffs(todo) - 1 : c;
                 todo &= todo - 1;
-                float g[16], ex[3];
+                float g[19];
 #pragma unroll
-                for (int i = 0; i < 16; ++i) g[i] = 0.f;
-                ex[0] = ex[1] = ex[2] = 0.f;
+                for (int i = 0; i < 19; ++i) g[i] = 0.f;
                 bool hit = false;
-                if (act && alive) hit = backward_pair<DEG, FAST>(cfg, sm, j, ray, dox, doy, doz, depth_grads, st, alive, g, ex);
+                if (act && alive) hit = backward_pair<DEG, FAST, RadianceHit>(cfg, sm, j, ray, dox, doy, doz, depth_grads, st, alive, g);
                 const unsigned hits = __ballot_sync(kFull, hit);
                 if (hits) {
                     float4* mine = rows + lane * (kGradRow / 4);
@@ -532,7 +228,7 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
                     mine[1] = make_float4(g[4], g[5], g[6], g[7]);
                     mine[2] = make_float4(g[8], g[9], g[10], g[11]);
                     mine[3] = make_float4(g[12], g[13], g[14], g[15]);
-                    if (depth_grads) mine[4] = make_float4(ex[0], ex[1], ex[2], 0.f);  // warp-uniform
+                    if (depth_grads) mine[4] = make_float4(g[16], g[17], g[18], 0.f);  // warp-uniform
                     __syncwarp();
                     if ((hits & sub_lanes) && col < cols) {  // this sub-block's particle received something
                         float4 s = rows[sub_lane<SUBL>(first, 0) * (kGradRow / 4) + col];
@@ -548,7 +244,7 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
                 }
             }
         }
-    }
+    });
 }
 
 // 3 CTAs per SM (72-80 registers, 45 KB of shared memory per CTA; 24 warps per SM).  4 CTAs would fit in shared memory but cap the
@@ -569,24 +265,15 @@ __global__ void __launch_bounds__(kTilePixels, 3) render_backward_kernel(FrameCa
                                                                       const float* __restrict__ out_dist, const float* __restrict__ d_dist,
                                                                       float* __restrict__ grad_acc) {
     __shared__ BwdSmem sm;
-    const int tile = tile_order[blockIdx.x];
     const int tid = threadIdx.x;
-    const int lane = tid & 31;
-    int px, py;
-    tile_pixel(tile, cam.grid_x, tid, px, py);
-    const bool inside = (px < cam.width) && (py < cam.height);
-    const int64_t pix = static_cast<int64_t>(py) * cam.width + px;
-
-    Ray ray;
-    ray.alive = false;
-    if (inside) ray = make_ray(cam, rays_o, rays_d, pix);
-    const bool alive = inside && ray.alive;
+    const TileRay tr = tile_ray(cam, rays_o, rays_d, tile_order, tid);
+    const int64_t pix = tr.pix;
 
     BwdRay st;
     st.Cix = st.Ciy = st.Ciz = st.Cgx = st.Cgy = st.Cgz = 0.f;
     st.Tint = 1.f; st.Tgrad = 0.f; st.Dint = 0.f; st.Dgrad = 0.f;
     st.T = 1.f; st.Cx = st.Cy = st.Cz = st.D = 0.f;
-    if (alive) {
+    if (tr.valid) {
         const float4 o = reinterpret_cast<const float4*>(out_rgba)[pix];
         const float4 g = reinterpret_cast<const float4*>(d_rgba)[pix];
         st.Cix = o.x; st.Ciy = o.y; st.Ciz = o.z;
@@ -598,20 +285,19 @@ __global__ void __launch_bounds__(kTilePixels, 3) render_backward_kernel(FrameCa
     }
 
     float ofx, ofy, ofz;
-    const bool fast = frame_common_origin(cam, rays_o, inside, pix, ofx, ofy, ofz);
-    const uint32_t begin = ranges[tile * 2], end = ranges[tile * 2 + 1];
-    const uint32_t* words = hit_words + static_cast<size_t>(chunk_base[tile]) * kWordsPerChunk;
+    const bool fast = frame_common_origin(cam, rays_o, tr.inside, pix, ofx, ofy, ofz);
+    const uint32_t begin = ranges[tr.tile * 2], end = ranges[tr.tile * 2 + 1];
+    const uint32_t* words = hit_words + static_cast<size_t>(chunk_base[tr.tile]) * kWordsPerChunk;
     const bool use_words = (cfg.subtile_culling & 4) != 0;
     if (fast)
-        backward_tile<DEG, true, SUBL>(cfg, sm, ray, ofx, ofy, ofz, tid, lane, begin, end, particles, rgb, sorted_values, words, use_words, alive, st, grad_acc);
+        backward_tile<DEG, true, SUBL>(cfg, sm, tr.ray, ofx, ofy, ofz, tid, tid & 31, begin, end, particles, rgb, sorted_values, words, use_words, tr.valid, st, grad_acc);
     else
-        backward_tile<DEG, false, SUBL>(cfg, sm, ray, ofx, ofy, ofz, tid, lane, begin, end, particles, rgb, sorted_values, words, use_words, alive, st, grad_acc);
+        backward_tile<DEG, false, SUBL>(cfg, sm, tr.ray, ofx, ofy, ofz, tid, tid & 31, begin, end, particles, rgb, sorted_values, words, use_words, tr.valid, st, grad_acc);
 }
 
 // ----------------------------------------------------------------------------------------------------------
 // G8 per-particle SH adjoint + emission of the final gradient rows; re-zeroes the accumulator for the next frame.
 
-constexpr float kC0 = 0.28209479177387814f;
 constexpr float kC1 = 0.4886025119029199f;
 __constant__ float kC2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f, -1.0925484305920792f,
                              0.5462742152960396f};
@@ -695,6 +381,7 @@ __global__ void __launch_bounds__(kPbThreads) project_backward_kernel(FrameCamer
                 const float r = pq.x, x = pq.y, y = pq.z, z = pq.w;
                 const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, xz = x * z, yz = y * z;
                 const float rx = r * x, ry = r * y, rz = r * z;
+                // rotation_rows (render_tile.cuh) written out: routed through the helper this kernel compiles to different SASS
                 const float r0x = 1.f - 2.f * (yy + zz), r0y = 2.f * (xy + rz), r0z = 2.f * (xz - ry);
                 const float r1x = 2.f * (xy - rz), r1y = 1.f - 2.f * (xx + zz), r1z = 2.f * (yz + rx);
                 const float r2x = 2.f * (xz + ry), r2y = 2.f * (yz - rx), r2z = 1.f - 2.f * (xx + yy);

@@ -158,6 +158,12 @@ class SplatRaster:
             raise RuntimeError("threedgut_tracer: CUDA device required; there is no CPU path")
         self._cfg = _native_config(conf)
         self._nht = _nht_config(conf)  # None: SH radiance
+        # kind-dependent parts of trace / trace_bwd, resolved once: ray-feature channels (rgb | 24 NHT features, then alpha) and how the
+        # per-particle radiance is handed to the kernels
+        if self._nht is None:
+            self._out_channels, self._radiance = 4, _c
+        else:
+            self._out_channels, self._radiance = NHT_FEATURE_DIM // 2 + 1, self._nht_features
         self._ctx = {}  # one native context per device, like one SplatRaster per process/GPU in the reference
         self._last_camera = None  # (sensor, pose_start, pose_end, w, h, native.Camera) of the latest call: trace_bwd re-uses trace's struct
 
@@ -209,25 +215,29 @@ class SplatRaster:
               timestamp_start, timestamp_end, pose_start, pose_end):
         """splatRaster.cpp:184-262 -> (feat+alpha [H,W,4], dist [H,W,1], hits [H,W,1], visibility [N,1]); with NHT features
         (model.feature_type: nht) feat+alpha is [H,W,25] and particle_radiance the [N,48] features."""
-        if self._nht is not None:
-            return self._trace_nht(particle_density, particle_radiance, ray_ori, ray_dir, sensor_params, pose_start, pose_end)
+        nht = self._nht
         dev = ray_ori.device
         h, w = int(ray_ori.shape[1]), int(ray_ori.shape[2])
         n = int(particle_density.shape[0])
-        particle_density, particle_radiance = _c(particle_density), _c(particle_radiance)
+        particle_density, particle_radiance = _c(particle_density), self._radiance(particle_radiance)
         ray_ori, ray_dir = _c(ray_ori), _c(ray_dir)
-        for t in (particle_density, particle_radiance, ray_ori, ray_dir):
+        # NHT features are checked (and rounded) by _nht_features; they may be fp16 here
+        for t in ((particle_density, particle_radiance, ray_ori, ray_dir) if nht is None else (particle_density, ray_ori, ray_dir)):
             if t.dtype != torch.float32 or not t.is_cuda:
                 raise RuntimeError("trace: tensors must be float32 CUDA tensors")
-        rgba = torch.empty((h, w, 4), dtype=torch.float32, device=dev)
+        out = torch.empty((h, w, self._out_channels), dtype=torch.float32, device=dev)
         dist = torch.empty((h, w, 1), dtype=torch.float32, device=dev)
         hits = torch.empty((h, w, 1), dtype=torch.float32, device=dev)
         vis = torch.empty((n, 1), dtype=torch.float32, device=dev)
         cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
-        stream = _raw_stream(dev)
-        self._context(dev).forward(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features),
-                                   ptr(ray_ori), ptr(ray_dir), ptr(rgba), ptr(dist), ptr(hits), ptr(vis))
-        return rgba, dist, hits, vis
+        stream, ctx = _raw_stream(dev), self._context(dev)
+        if nht is None:
+            ctx.forward(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features), ptr(ray_ori), ptr(ray_dir),
+                        ptr(out), ptr(dist), ptr(hits), ptr(vis))
+        else:
+            ctx.forward_nht(stream, cam, n, ptr(particle_density), ptr(particle_radiance), NHT_FEATURE_DIM, int(nht["half"]), ptr(ray_ori),
+                            ptr(ray_dir), ptr(out), ptr(dist), ptr(hits), ptr(vis))
+        return out, dist, hits, vis
 
     def trace_bwd(self, frame_id, n_active_features, particle_density, particle_radiance, ray_ori, ray_dir, ray_time, sensor_params,
                   timestamp_start, timestamp_end, pose_start, pose_end, ray_radiance_density, ray_radiance_density_grd,
@@ -235,30 +245,10 @@ class SplatRaster:
         """splatRaster.cpp:264-350 -> (dDensity [N,12], dRadiance [N,48]).  `out` (extension): a pair of preallocated
         tensors to write into, e.g. two views of one flat buffer so that a single all-reduce covers both.  With NHT features dRadiance
         is the fp32 [N,48] feature gradient."""
-        if self._nht is not None:
-            if out is not None:
-                raise NotImplementedError("trace_bwd(out=...) is not built for NHT features")
-            return self._trace_bwd_nht(particle_density, particle_radiance, ray_ori, ray_dir, sensor_params, pose_start, pose_end,
-                                       ray_radiance_density, ray_radiance_density_grd, ray_hit_distance, ray_hit_distance_grd)
-        dev = ray_ori.device
-        h, w = int(ray_ori.shape[1]), int(ray_ori.shape[2])
-        n = int(particle_density.shape[0])
-        particle_density, particle_radiance = _c(particle_density), _c(particle_radiance)
-        ray_ori, ray_dir = _c(ray_ori), _c(ray_dir)
-        rgba, d_rgba = _c(ray_radiance_density), _c(ray_radiance_density_grd).float()
-        dist, d_dist = _c(ray_hit_distance), _c(ray_hit_distance_grd).float()
-        if out is not None:
-            d_density, d_radiance = out
-            assert d_density.shape == (n, 12) and d_radiance.shape == (n, 48) and d_density.is_contiguous() and d_radiance.is_contiguous()
-        else:
-            d_density = torch.empty((n, 12), dtype=torch.float32, device=dev)
-            d_radiance = torch.empty((n, 48), dtype=torch.float32, device=dev)
-        cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
-        stream = _raw_stream(dev)
-        self._context(dev).backward(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features),
-                                    ptr(ray_ori), ptr(ray_dir), ptr(rgba), ptr(d_rgba), ptr(dist), ptr(d_dist),
-                                    ptr(d_density), ptr(d_radiance))
-        return d_density, d_radiance
+        if self._nht is not None and out is not None:
+            raise NotImplementedError("trace_bwd(out=...) is not built for NHT features")
+        return self._backward("backward", n_active_features, particle_density, particle_radiance, ray_ori, ray_dir, sensor_params, pose_start,
+                              pose_end, ray_radiance_density, ray_radiance_density_grd, ray_hit_distance, ray_hit_distance_grd, out)
 
     def _nht_features(self, features: torch.Tensor) -> torch.Tensor:
         """[N,48] features as the kernels read them: rounded to fp16 under render.particle_feature_half (splatRaster.cpp:90-98)"""
@@ -266,39 +256,35 @@ class SplatRaster:
             raise RuntimeError(f"trace: NHT features must be a [N,{NHT_FEATURE_DIM}] CUDA tensor, got {tuple(features.shape)}")
         return _c(features.to(torch.float16 if self._nht["half"] else torch.float32))
 
-    def _trace_nht(self, particle_density, features, ray_ori, ray_dir, sensor_params, pose_start, pose_end):
+    def _backward(self, sh_call, n_active_features, particle_density, particle_radiance, ray_ori, ray_dir, sensor_params, pose_start, pose_end,
+                  rgba, d_rgba, dist, d_dist, out):
+        """trace_bwd (sh_call "backward") and trace_bwd_compact ("backward_compact", the SH compact backward whatever the feature type):
+        the second output is the [N,48] SH or NHT feature gradient, or, compact, the [N,4] masked radiance gradient."""
+        compact = sh_call == "backward_compact"
+        nht = None if compact else self._nht
         dev = ray_ori.device
         h, w = int(ray_ori.shape[1]), int(ray_ori.shape[2])
         n = int(particle_density.shape[0])
         particle_density, ray_ori, ray_dir = _c(particle_density), _c(ray_ori), _c(ray_dir)
-        for t in (particle_density, ray_ori, ray_dir):
-            if t.dtype != torch.float32 or not t.is_cuda:
-                raise RuntimeError("trace: tensors must be float32 CUDA tensors")
-        feats = self._nht_features(features)
-        out = torch.empty((h, w, NHT_FEATURE_DIM // 2 + 1), dtype=torch.float32, device=dev)
-        dist = torch.empty((h, w, 1), dtype=torch.float32, device=dev)
-        hits = torch.empty((h, w, 1), dtype=torch.float32, device=dev)
-        vis = torch.empty((n, 1), dtype=torch.float32, device=dev)
-        cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
-        self._context(dev).forward_nht(_raw_stream(dev), cam, n, ptr(particle_density), ptr(feats), NHT_FEATURE_DIM, int(self._nht["half"]),
-                                       ptr(ray_ori), ptr(ray_dir), ptr(out), ptr(dist), ptr(hits), ptr(vis))
-        return out, dist, hits, vis
-
-    def _trace_bwd_nht(self, particle_density, features, ray_ori, ray_dir, sensor_params, pose_start, pose_end, out, d_out, dist, d_dist):
-        dev = ray_ori.device
-        h, w = int(ray_ori.shape[1]), int(ray_ori.shape[2])
-        n = int(particle_density.shape[0])
-        particle_density, ray_ori, ray_dir = _c(particle_density), _c(ray_ori), _c(ray_dir)
-        feats = self._nht_features(features)
-        out, d_out = _c(out), _c(d_out).float()
+        particle_radiance = _c(particle_radiance) if nht is None else self._nht_features(particle_radiance)
+        rgba, d_rgba = _c(rgba), _c(d_rgba).float()
         dist, d_dist = _c(dist), _c(d_dist).float()
-        d_density = torch.empty((n, 12), dtype=torch.float32, device=dev)
-        d_features = torch.empty((n, NHT_FEATURE_DIM), dtype=torch.float32, device=dev)
+        width = 4 if compact else 48
+        if out is not None:
+            d_density, d_radiance = out
+            assert d_density.shape == (n, 12) and d_radiance.shape == (n, width) and d_density.is_contiguous() and d_radiance.is_contiguous()
+        else:
+            d_density = torch.empty((n, 12), dtype=torch.float32, device=dev)
+            d_radiance = torch.empty((n, width), dtype=torch.float32, device=dev)
         cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
-        self._context(dev).backward_nht(_raw_stream(dev), cam, n, ptr(particle_density), ptr(feats), NHT_FEATURE_DIM, int(self._nht["half"]),
-                                        ptr(ray_ori), ptr(ray_dir), ptr(out), ptr(d_out), ptr(dist), ptr(d_dist), ptr(d_density),
-                                        ptr(d_features))
-        return d_density, d_features
+        stream, ctx = _raw_stream(dev), self._context(dev)
+        if nht is None:
+            getattr(ctx, sh_call)(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features), ptr(ray_ori),
+                                  ptr(ray_dir), ptr(rgba), ptr(d_rgba), ptr(dist), ptr(d_dist), ptr(d_density), ptr(d_radiance))
+        else:
+            ctx.backward_nht(stream, cam, n, ptr(particle_density), ptr(particle_radiance), NHT_FEATURE_DIM, int(nht["half"]), ptr(ray_ori),
+                             ptr(ray_dir), ptr(rgba), ptr(d_rgba), ptr(dist), ptr(d_dist), ptr(d_density), ptr(d_radiance))
+        return d_density, d_radiance
 
     # ---- view-parallel extensions (no reference twin: the reference trains on one GPU) -----------------------------------------
 
@@ -307,25 +293,8 @@ class SplatRaster:
                           ray_hit_distance, ray_hit_distance_grd, out=None):
         """trace_bwd that returns (dDensity [N,12], g [N,4]): g is the masked dL/d(radiance) of each particle in this view, from
         which sph_grad_from_views rebuilds the [N,48] SH gradient of any set of views (16 instead of 192 bytes per particle to exchange)."""
-        dev = ray_ori.device
-        h, w = int(ray_ori.shape[1]), int(ray_ori.shape[2])
-        n = int(particle_density.shape[0])
-        particle_density, particle_radiance = _c(particle_density), _c(particle_radiance)
-        ray_ori, ray_dir = _c(ray_ori), _c(ray_dir)
-        rgba, d_rgba = _c(ray_radiance_density), _c(ray_radiance_density_grd).float()
-        dist, d_dist = _c(ray_hit_distance), _c(ray_hit_distance_grd).float()
-        if out is not None:
-            d_density, g = out
-            assert d_density.shape == (n, 12) and g.shape == (n, 4) and d_density.is_contiguous() and g.is_contiguous()
-        else:
-            d_density = torch.empty((n, 12), dtype=torch.float32, device=dev)
-            g = torch.empty((n, 4), dtype=torch.float32, device=dev)
-        cam = self._camera_cached(sensor_params, pose_start, pose_end, w, h)
-        stream = _raw_stream(dev)
-        self._context(dev).backward_compact(stream, cam, n, ptr(particle_density), ptr(particle_radiance), int(n_active_features),
-                                            ptr(ray_ori), ptr(ray_dir), ptr(rgba), ptr(d_rgba), ptr(dist), ptr(d_dist),
-                                            ptr(d_density), ptr(g))
-        return d_density, g
+        return self._backward("backward_compact", n_active_features, particle_density, particle_radiance, ray_ori, ray_dir, sensor_params, pose_start,
+                              pose_end, ray_radiance_density, ray_radiance_density_grd, ray_hit_distance, ray_hit_distance_grd, out)
 
     def sensor_position(self, sensor_params, pose_start, pose_end, width, height):
         """World-space sensor position of a view exactly as the kernels compute it: float32 numpy [3]."""
