@@ -86,6 +86,8 @@ SIGNATURES = {
     "gutb200_selective_adam_update": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i64, _i64]),
     "gutb200_gaussian_adam_step": (_int, _adam),
     "gutb200_gaussian_adam_step_reg": (_int, _adam + [_f32, _f32]),
+    "gutb200_nht_adam_step": (_int, [_vp, _i64, _i64, _vpp, _vpp, _vpp, _f32p, _i64p, _f32, _f32, _f32, _i32, _f32, _f32, _f32, _f32, _i32,
+                                     _vp, _vp, _vp, _vp, _f32, _f32]),
     "gutb200_image_loss_scratch_bytes": (_sz, [_i32, _i32]),
     "gutb200_image_loss": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
     "gutb200_image_loss_rgb": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),

@@ -12,7 +12,11 @@
 // gutb200_gaussian_adam_step_reg adds the opacity and scale regularisers of the reference loss (trainer.py:722-736:
 // lambda_opacity mean|sigmoid(raw density)| + lambda_scale mean|exp(raw scale)|) to the activated density / scale gradients before the
 // chain rule: + lambda_opacity / N and + lambda_scale / (3 N).  They are a template flag (REG) of the kernel, so the plain entry is unchanged.
-// Both are streaming kernels: every byte is read and written once, coalesced (element-wise index space; the quaternion rows as
+// nht_adam_kernel is the same step for the NHT model (template variant of the same group code): features [N,48] are used raw, and the
+// feature decoder's flat parameter vector is a sixth group with its own Adam (betas, eps, L2 weight decay, step count; never selective),
+// as the reference trains it with a torch.optim.Adam of its own (trainer.py:573-577).  Groups in frozen_mask launch no block: parameters
+// and moments stay untouched, as torch's Adam skips a parameter whose grad is None (colour refinement, trainer.py:168-195).
+// All are streaming kernels: every byte is read and written once, coalesced (element-wise index space; the quaternion rows as
 // float4).  Algorithmic bytes per Gaussian of the fused step: 59 x (4 param r + 4 param w + 8 moments r + 8 moments w) + 240
 // gradient + 4 visibility = 1660 B.
 #include <cuda_runtime.h>
@@ -66,9 +70,33 @@ struct GaussianAdamArgs {
     float reg_scale;           // lambda_scale / (3 N), added to every d scale (REG only)
 };
 
-// gradient of element (row, col) of group G w.r.t. the RAW parameter value p
-template <int G, bool REG>
-__device__ __forceinline__ float raw_gradient(const GaussianAdamArgs& a, int64_t row, int col, float p) {
+struct NhtAdamArgs {
+    float* param[6];           // positions [N,3], density [N,1], rotation [N,4], scale [N,3], features [N,48] (raw), decoder params [n_decoder]
+    float* m[6];
+    float* v[6];
+    float lr[6];
+    unsigned block_end[6];     // as in GaussianAdamArgs; a frozen group has no blocks
+    const float* d_particles;  // [N,12] w.r.t. the activated values
+    const float* d_features;   // [N,48] (the features are used raw: no chain rule)
+    const float* d_decoder;    // [n_decoder]
+    const float* visibility;   // [N] float bits or nullptr (Gaussian groups only)
+    int64_t n;
+    int64_t n_decoder;
+    AdamHyper h[6];            // per group: its own step count; the decoder its own betas / eps and never selective
+    float weight_decay;        // decoder: L2 on the gradient, g + weight_decay p (torch.optim.Adam weight_decay)
+    float reg_density;
+    float reg_scale;
+};
+
+// the hyper-parameters and the element count of group G (W floats per Gaussian)
+template <int G> __device__ __forceinline__ const AdamHyper& group_hyper(const GaussianAdamArgs& a) { return a.h; }
+template <int G> __device__ __forceinline__ const AdamHyper& group_hyper(const NhtAdamArgs& a) { return a.h[G]; }
+template <int G, int W> __device__ __forceinline__ int64_t group_total(const GaussianAdamArgs& a) { return a.n * W; }
+template <int G, int W> __device__ __forceinline__ int64_t group_total(const NhtAdamArgs& a) { return G == 5 ? a.n_decoder : a.n * W; }
+
+// gradient w.r.t. the RAW value p of the [N,12]-record groups (positions, density, scale), shared by both layouts
+template <int G, bool REG, class A>
+__device__ __forceinline__ float particle_gradient(const A& a, int64_t row, int col, float p) {
     if (G == 0) return a.d_particles[row * 12 + col];
     if (G == 1) {
         const float s = 1.0f / (1.0f + expf(-p));   // density = sigmoid(raw)
@@ -76,25 +104,37 @@ __device__ __forceinline__ float raw_gradient(const GaussianAdamArgs& a, int64_t
         if constexpr (REG) g = g + a.reg_density;
         return g * s * (1.0f - s);
     }
-    if (G == 3) {
-        float g = a.d_particles[row * 12 + 8 + col];
-        if constexpr (REG) g = g + a.reg_scale;
-        return g * expf(p);   // scale = exp(raw)
-    }
+    float g = a.d_particles[row * 12 + 8 + col];
+    if constexpr (REG) g = g + a.reg_scale;
+    return g * expf(p);   // scale = exp(raw)
+}
+
+// gradient of element (row, col) of group G w.r.t. the RAW parameter value p
+template <int G, bool REG>
+__device__ __forceinline__ float raw_gradient(const GaussianAdamArgs& a, int64_t row, int col, float p) {
     if (G == 4) return a.d_sph[row * 48 + col];                        // features = cat(albedo [N,3], specular [N,45])  (model.py:94-96)
-    return a.d_sph[row * 48 + 3 + col];
+    if (G == 5) return a.d_sph[row * 48 + 3 + col];
+    return particle_gradient<G, REG>(a, row, col, p);
+}
+
+template <int G, bool REG>
+__device__ __forceinline__ float raw_gradient(const NhtAdamArgs& a, int64_t row, int col, float p) {
+    if (G == 4) return a.d_features[row * 48 + col];                   // NHT features are raw (model.py:225)
+    if (G == 5) return a.d_decoder[row] + a.weight_decay * p;
+    return particle_gradient<G, REG>(a, row, col, p);
 }
 
 // flat groups: a thread owns 4 consecutive floats of the [N*W] array (16-byte loads and stores of param / moments)
-template <int G, int W, bool REG>
-__device__ __forceinline__ void flat_group(const GaussianAdamArgs& a, int64_t t) {
-    const int64_t total = a.n * W, e0 = t * 4;
+template <int G, int W, bool REG, class A>
+__device__ __forceinline__ void flat_group(const A& a, int64_t t) {
+    const int64_t total = group_total<G, W>(a), e0 = t * 4;
     if (e0 >= total) return;
     float* P = a.param[G] + e0;
     float* M = a.m[G] + e0;
     float* V = a.v[G] + e0;
     const float lr = a.lr[G];
-    const bool masked = a.h.selective && a.visibility;
+    const AdamHyper& h = group_hyper<G>(a);
+    const bool masked = h.selective && a.visibility;
     if (e0 + 3 < total) {
         float4 p = *reinterpret_cast<float4*>(P), m = *reinterpret_cast<float4*>(M), v = *reinterpret_cast<float4*>(V);
         float pe[4] = {p.x, p.y, p.z, p.w}, me[4] = {m.x, m.y, m.z, m.w}, ve[4] = {v.x, v.y, v.z, v.w};
@@ -105,7 +145,7 @@ __device__ __forceinline__ void flat_group(const GaussianAdamArgs& a, int64_t t)
             const int col = static_cast<int>(e - row * W);
             if (masked && (__float_as_uint(a.visibility[row]) == 0u)) continue;
             any = true;
-            pe[k] = adam_update(pe[k], raw_gradient<G, REG>(a, row, col, pe[k]), me[k], ve[k], lr, a.h);
+            pe[k] = adam_update(pe[k], raw_gradient<G, REG>(a, row, col, pe[k]), me[k], ve[k], lr, h);
         }
         if (!any) return;  // nothing visible: leave the 48 bytes alone
         *reinterpret_cast<float4*>(P) = make_float4(pe[0], pe[1], pe[2], pe[3]);
@@ -118,51 +158,77 @@ __device__ __forceinline__ void flat_group(const GaussianAdamArgs& a, int64_t t)
             if (masked && (__float_as_uint(a.visibility[row]) == 0u)) continue;
             float m = a.m[G][e], v = a.v[G][e];
             const float p = a.param[G][e];
-            a.param[G][e] = adam_update(p, raw_gradient<G, REG>(a, row, col, p), m, v, lr, a.h);
+            a.param[G][e] = adam_update(p, raw_gradient<G, REG>(a, row, col, p), m, v, lr, h);
             a.m[G][e] = m;
             a.v[G][e] = v;
         }
     }
 }
 
-template <bool REG>
-__global__ void __launch_bounds__(256, 4) gaussian_adam_kernel(GaussianAdamArgs a) {
+// rotation = normalize(raw), one row (float4) per thread: d raw = (g - q (q . g)) / max(|raw|, 1e-12)   (torch.nn.functional.normalize,
+// eps 1e-12)
+template <class A>
+__device__ __forceinline__ void rotation_group(const A& a, int64_t t) {
+    const AdamHyper& h = group_hyper<2>(a);
+    const int64_t row = t;
+    if (row >= a.n) return;
+    if (h.selective && a.visibility && (__float_as_uint(a.visibility[row]) == 0u)) return;
+    const float lr = a.lr[2];
+    float4* P = reinterpret_cast<float4*>(a.param[2]) + row;
+    float4* M = reinterpret_cast<float4*>(a.m[2]) + row;
+    float4* V = reinterpret_cast<float4*>(a.v[2]) + row;
+    const float4 r = *P;
+    const float4 g = *reinterpret_cast<const float4*>(a.d_particles + row * 12 + 4);
+    const float len = fmaxf(sqrtf(r.x * r.x + r.y * r.y + r.z * r.z + r.w * r.w), 1e-12f);
+    const float il = 1.0f / len;
+    const float qx = r.x * il, qy = r.y * il, qz = r.z * il, qw = r.w * il;
+    const float dot = qx * g.x + qy * g.y + qz * g.z + qw * g.w;
+    float4 m = *M, v = *V, out;
+    out.x = adam_update(r.x, (g.x - qx * dot) * il, m.x, v.x, lr, h);
+    out.y = adam_update(r.y, (g.y - qy * dot) * il, m.y, v.y, lr, h);
+    out.z = adam_update(r.z, (g.z - qz * dot) * il, m.z, v.z, lr, h);
+    out.w = adam_update(r.w, (g.w - qw * dot) * il, m.w, v.w, lr, h);
+    *P = out;
+    *M = m;
+    *V = v;
+}
+
+// a block works on ONE group: the group whose block range holds blockIdx.x (empty ranges -- frozen groups -- are skipped)
+template <class A>
+__device__ __forceinline__ int block_group(const A& a, int64_t& t) {
     const unsigned blk = blockIdx.x;
     int group = 0;
 #pragma unroll
     for (int k = 0; k < 5; ++k) group += blk >= a.block_end[k] ? 1 : 0;
     const unsigned first = group == 0 ? 0u : a.block_end[group - 1];
-    const int64_t t = static_cast<int64_t>(blk - first) * blockDim.x + threadIdx.x;
-    switch (group) {
+    t = static_cast<int64_t>(blk - first) * blockDim.x + threadIdx.x;
+    return group;
+}
+
+template <bool REG>
+__global__ void __launch_bounds__(256, 4) gaussian_adam_kernel(GaussianAdamArgs a) {
+    int64_t t;
+    switch (block_group(a, t)) {
         case 0: flat_group<0, 3, REG>(a, t); break;
         case 1: flat_group<1, 1, REG>(a, t); break;
         case 3: flat_group<3, 3, REG>(a, t); break;
         case 4: flat_group<4, 3, REG>(a, t); break;
         case 5: flat_group<5, 45, REG>(a, t); break;
-        default: {
-            // rotation = normalize(raw): d raw = (g - q (q . g)) / max(|raw|, 1e-12)   (torch.nn.functional.normalize, eps 1e-12)
-            const int64_t row = t;
-            if (row >= a.n) return;
-            if (a.h.selective && a.visibility && (__float_as_uint(a.visibility[row]) == 0u)) return;
-            const float lr = a.lr[2];
-            float4* P = reinterpret_cast<float4*>(a.param[2]) + row;
-            float4* M = reinterpret_cast<float4*>(a.m[2]) + row;
-            float4* V = reinterpret_cast<float4*>(a.v[2]) + row;
-            const float4 r = *P;
-            const float4 g = *reinterpret_cast<const float4*>(a.d_particles + row * 12 + 4);
-            const float len = fmaxf(sqrtf(r.x * r.x + r.y * r.y + r.z * r.z + r.w * r.w), 1e-12f);
-            const float il = 1.0f / len;
-            const float qx = r.x * il, qy = r.y * il, qz = r.z * il, qw = r.w * il;
-            const float dot = qx * g.x + qy * g.y + qz * g.z + qw * g.w;
-            float4 m = *M, v = *V, out;
-            out.x = adam_update(r.x, (g.x - qx * dot) * il, m.x, v.x, lr, a.h);
-            out.y = adam_update(r.y, (g.y - qy * dot) * il, m.y, v.y, lr, a.h);
-            out.z = adam_update(r.z, (g.z - qz * dot) * il, m.z, v.z, lr, a.h);
-            out.w = adam_update(r.w, (g.w - qw * dot) * il, m.w, v.w, lr, a.h);
-            *P = out;
-            *M = m;
-            *V = v;
-        }
+        default: rotation_group(a, t);
+    }
+}
+
+// The NHT model's step: the Gaussian groups with [N,48] raw features, and the decoder's flat parameter vector as a sixth group
+template <bool REG>
+__global__ void __launch_bounds__(256, 4) nht_adam_kernel(NhtAdamArgs a) {
+    int64_t t;
+    switch (block_group(a, t)) {
+        case 0: flat_group<0, 3, REG>(a, t); break;
+        case 1: flat_group<1, 1, REG>(a, t); break;
+        case 3: flat_group<3, 3, REG>(a, t); break;
+        case 4: flat_group<4, 48, REG>(a, t); break;
+        case 5: flat_group<5, 1, REG>(a, t); break;
+        default: rotation_group(a, t);
     }
 }
 
@@ -218,6 +284,55 @@ int gaussian_adam_step(void* stream, int64_t n, float* const* params6, float* co
     return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 
+int nht_adam_step(void* stream, int64_t n, int64_t n_decoder, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6,
+                  const float* lr6, const int64_t* steps6, float b1, float b2, float eps, int32_t selective, float decoder_b1, float decoder_b2,
+                  float decoder_eps, float decoder_weight_decay, int32_t frozen_mask, const float* d_particles, const float* d_features,
+                  const float* d_decoder, const float* visibility, float reg_density, float reg_scale) {
+    if (n < 0 || n_decoder < 0 || !params6 || !exp_avg6 || !exp_avg_sq6 || !lr6 || !steps6) return 1;
+    NhtAdamArgs a;
+    const int widths[6] = {3, 1, 4, 3, 48, 1};
+    unsigned blocks = 0;
+    for (int k = 0; k < 6; ++k) {
+        const bool frozen = (frozen_mask >> k) & 1;
+        const int64_t count = k == 5 ? n_decoder : n;
+        a.param[k] = params6[k];
+        a.m[k] = exp_avg6[k];
+        a.v[k] = exp_avg_sq6[k];
+        a.lr[k] = lr6[k];
+        if (!frozen && count > 0) {
+            if (!params6[k] || !exp_avg6[k] || !exp_avg_sq6[k]) return 1;
+            if ((reinterpret_cast<uintptr_t>(a.param[k]) | reinterpret_cast<uintptr_t>(a.m[k]) | reinterpret_cast<uintptr_t>(a.v[k])) & 15) return 3;
+            const bool sel = k < 5 && selective;
+            if (!sel && steps6[k] < 1) return 1;
+            a.h[k] = k == 5 ? make_hyper(decoder_b1, decoder_b2, decoder_eps, steps6[k], 0) : make_hyper(b1, b2, eps, steps6[k], selective);
+            // rotation: one row per thread; flat groups: 4 floats per thread
+            const int64_t threads = k == 2 ? count : (count * widths[k] + 3) / 4;
+            blocks += static_cast<unsigned>((threads + 255) / 256);
+        } else {
+            a.h[k] = make_hyper(b1, b2, eps, 0, 1);  // never read: the group launches no block
+        }
+        a.block_end[k] = blocks;
+    }
+    const bool gaussians = (~frozen_mask & 0x1f) != 0 && n > 0, decoder = !(frozen_mask & 0x20) && n_decoder > 0;
+    if ((gaussians && !d_particles) || (gaussians && !(frozen_mask & 0x10) && !d_features) || (decoder && !d_decoder)) return 1;
+    if (reinterpret_cast<uintptr_t>(d_particles) & 15) return 3;
+    if (blocks == 0) return 0;
+    a.d_particles = d_particles;
+    a.d_features = d_features;
+    a.d_decoder = d_decoder;
+    a.visibility = visibility;
+    a.n = n;
+    a.n_decoder = n_decoder;
+    a.weight_decay = decoder_weight_decay;
+    a.reg_density = reg_density;
+    a.reg_scale = reg_scale;
+    if (reg_density == 0.f && reg_scale == 0.f)
+        nht_adam_kernel<false><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    else
+        nht_adam_kernel<true><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    return cudaGetLastError() == cudaSuccess ? 0 : 2;
+}
+
 }  // namespace
 
 }  // namespace gutb200
@@ -250,6 +365,16 @@ int gutb200_gaussian_adam_step_reg(void* stream, int64_t n, float* const* params
                                    const float* d_sph, const float* visibility, float reg_density, float reg_scale) {
     return gutb200::gaussian_adam_step(stream, n, params6, exp_avg6, exp_avg_sq6, lr6, b1, b2, eps, step, selective, d_particles, d_sph,
                                        visibility, reg_density, reg_scale);
+}
+
+int gutb200_nht_adam_step(void* stream, int64_t n, int64_t n_decoder, float* const* params6, float* const* exp_avg6,
+                          float* const* exp_avg_sq6, const float* lr6, const int64_t* steps6, float b1, float b2, float eps, int32_t selective,
+                          float decoder_b1, float decoder_b2, float decoder_eps, float decoder_weight_decay, int32_t frozen_mask,
+                          const float* d_particles, const float* d_features, const float* d_decoder, const float* visibility, float reg_density,
+                          float reg_scale) {
+    return gutb200::nht_adam_step(stream, n, n_decoder, params6, exp_avg6, exp_avg_sq6, lr6, steps6, b1, b2, eps, selective, decoder_b1,
+                                  decoder_b2, decoder_eps, decoder_weight_decay, frozen_mask, d_particles, d_features, d_decoder, visibility,
+                                  reg_density, reg_scale);
 }
 
 }  // extern "C"

@@ -57,7 +57,8 @@ def quaternion_to_so3(q: torch.Tensor) -> torch.Tensor:
 
 
 class GSDensifier:
-    """params: dict of raw tensors (GROUPS); moments: list of dicts with the same keys (e.g. [opt.exp_avg, opt.exp_avg_sq]).
+    """params: dict of raw tensors (GROUPS, or the NHT model's optimizers.NHT_GROUPS: every group in the dict is densified); moments:
+    list of dicts with the same keys (e.g. [opt.exp_avg, opt.exp_avg_sq]).
     Every mutating call replaces the tensors inside those dicts in place of the old ones (the dict objects stay the same, so an optimizer
     holding them sees the new tensors)."""
 
@@ -95,9 +96,10 @@ class GSDensifier:
             dist.all_reduce(self.grad_norm_accum, op=dist.ReduceOp.SUM, group=self.group)
             dist.all_reduce(self.grad_norm_denom, op=dist.ReduceOp.SUM, group=self.group)
 
-    def _apply(self, param_fn, moment_fn, names=GROUPS):
-        """base.py:78-107 on dicts: param_fn(name, tensor) -> new tensor, moment_fn(tensor) -> new tensor (None = keep)."""
-        for name in names:
+    def _apply(self, param_fn, moment_fn, names=None):
+        """base.py:78-107 on dicts: param_fn(name, tensor) -> new tensor, moment_fn(tensor) -> new tensor (None = keep).  names: every
+        group of the parameter dict (GROUPS for the SH model, optimizers.NHT_GROUPS for NHT) unless given."""
+        for name in (list(self.params) if names is None else names):
             if moment_fn is not None:
                 for m in self.moments:
                     m[name] = moment_fn(m[name]).contiguous()
@@ -276,7 +278,7 @@ class MCMCDensifier:
         if len(dead) == 0 or len(alive) == 0:
             return 0
         sampled, new_d, new_s = self._sample(len(dead), alive)
-        for name in GROUPS:
+        for name in list(self.params):  # every group the dict holds (SH or NHT features)
             p = self.params[name]
             if name == "density":
                 p[sampled] = new_d
@@ -296,7 +298,7 @@ class MCMCDensifier:
         if count == 0:
             return 0
         sampled, new_d, new_s = self._sample(count, None)
-        for name in GROUPS:
+        for name in list(self.params):  # every group the dict holds (SH or NHT features)
             p = self.params[name]
             if name == "density":
                 p[sampled] = new_d

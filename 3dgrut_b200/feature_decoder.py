@@ -66,16 +66,34 @@ class _Decode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_out):
         features, dirs, params = ctx.saved_tensors
-        cfg, n = ctx.cfg, features.shape[0]
-        lib = nat.nht_lib()
-        d_out = d_out.contiguous().float()
         d_features = torch.empty_like(features)
         d_params = torch.empty_like(params)
-        ws = torch.empty(lib.nhtb200_backward_workspace_bytes(C.byref(cfg), n), device=features.device, dtype=torch.uint8)
-        stream = torch.cuda.current_stream(features.device).cuda_stream
-        nat.nht_check(lib.nhtb200_backward(C.byref(cfg), stream, n, features.data_ptr(), dirs.data_ptr(), params.data_ptr(), d_out.data_ptr(),
-                                           d_features.data_ptr(), d_params.data_ptr(), ws.data_ptr()), "nhtb200_backward")
+        ws = backward_workspace(ctx.cfg, features.shape[0], features.device)
+        decode_backward(features, dirs, params, ctx.cfg, d_out.contiguous().float(), d_features, d_params, ws)
         return d_features, None, d_params, None
+
+
+def backward_workspace(cfg: nat.NhtConfig, n: int, device) -> torch.Tensor:
+    """The device workspace decode_backward needs for n rows (about 1.1 GB at 800 x 800 for the shipped decoder: allocate it once per
+    resolution where the backward runs every step)."""
+    return torch.empty(nat.nht_lib().nhtb200_backward_workspace_bytes(C.byref(cfg), int(n)), device=device, dtype=torch.uint8)
+
+
+def decode_backward(features: torch.Tensor, dirs: torch.Tensor, params: torch.Tensor, cfg: nat.NhtConfig, d_out: torch.Tensor,
+                    d_features: torch.Tensor, d_params: torch.Tensor, workspace: torch.Tensor) -> None:
+    """nhtb200_backward into caller tensors: d_out [n,3] -> d_features [n,F] and d_params [n_params] (overwritten, summed over the rows);
+    all contiguous fp32 CUDA tensors, e.g. d_params a view of a gradient exchange buffer.  workspace: backward_workspace(cfg, >= n)."""
+    n = int(features.shape[0])
+    for name, t, shape in (("features", features, None), ("dirs", dirs, (n, 3)), ("d_out", d_out, (n, 3)), ("d_features", d_features, tuple(features.shape)),
+                           ("d_params", d_params, tuple(params.shape))):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and (shape is None or tuple(t.shape) == shape)):
+            raise RuntimeError(f"decode_backward: {name} must be a contiguous float32 CUDA tensor{'' if shape is None else f' {list(shape)}'}")
+    lib = nat.nht_lib()
+    if workspace.numel() < lib.nhtb200_backward_workspace_bytes(C.byref(cfg), n):
+        raise RuntimeError("decode_backward: workspace is too small for this many rows")
+    stream = torch.cuda.current_stream(features.device).cuda_stream
+    nat.nht_check(lib.nhtb200_backward(C.byref(cfg), stream, n, features.data_ptr(), dirs.data_ptr(), params.data_ptr(), d_out.data_ptr(),
+                                       d_features.data_ptr(), d_params.data_ptr(), workspace.data_ptr()), "nhtb200_backward")
 
 
 def decode(features: torch.Tensor, dirs: torch.Tensor, params: torch.Tensor, cfg: nat.NhtConfig) -> torch.Tensor:

@@ -138,3 +138,107 @@ class FusedGaussianAdam:
             rc = getattr(native.load(), entry)(*args, *extra)
         if rc != 0:
             raise RuntimeError(f"{entry} failed ({rc})")
+
+
+NHT_GROUPS = ("positions", "density", "rotation", "scale", "features")
+NHT_WIDTHS = (3, 1, 4, 3, 48)
+
+
+class FusedNHTAdam:
+    """One-launch optimizer step for the NHT model and its feature decoder (gutb200_nht_adam_step).
+
+    params: dict name -> raw leaf tensor for NHT_GROUPS (features [N,48] are used raw, model.py:225); decoder_params: the decoder's flat
+    fp32 parameter vector (FeatureDecoder.network.params), updated in place as the group "decoder".  lrs: dict over NHT_GROUPS + "decoder"
+    (mutable, as FusedGaussianAdam's).  The Gaussian groups take betas / eps / selective as FusedGaussianAdam does; the decoder has an Adam
+    of its own, as in the reference (trainer.py:573-577): decoder_betas, decoder_eps, decoder_weight_decay (L2 on the gradient) and its own
+    step count, never selective.  step(..., frozen=names) skips those groups entirely: no block is launched for them, their parameters,
+    moments and step counts stay as they are (torch's Adam with grad None, the reference's colour refinement)."""
+
+    GROUPS = NHT_GROUPS + ("decoder",)
+
+    def __init__(self, params: dict, decoder_params: torch.Tensor, lrs: dict, betas=(0.9, 0.999), eps=1e-15, selective=False,
+                 decoder_betas=(0.9, 0.999), decoder_eps=1e-8, decoder_weight_decay=0.0):
+        # the dict itself is kept (not copied) when it holds exactly the five groups: densification replaces the tensors inside it
+        self.params = params if set(params.keys()) == set(NHT_GROUPS) else {k: params[k] for k in NHT_GROUPS}
+        self.decoder_params = decoder_params
+        self._validate()
+        self.lrs = {k: float(lrs[k]) for k in self.GROUPS}
+        self.betas, self.eps, self.selective = (float(betas[0]), float(betas[1])), float(eps), bool(selective)
+        self.decoder_betas, self.decoder_eps = (float(decoder_betas[0]), float(decoder_betas[1])), float(decoder_eps)
+        self.decoder_weight_decay = float(decoder_weight_decay)
+        self.exp_avg = {k: torch.zeros_like(t.data) for k, t in self.params.items()}
+        self.exp_avg_sq = {k: torch.zeros_like(t.data) for k, t in self.params.items()}
+        # the decoder's moments live apart from the per-Gaussian dicts, which the densifiers resize row by row
+        self.decoder_exp_avg = torch.zeros_like(decoder_params.data)
+        self.decoder_exp_avg_sq = torch.zeros_like(decoder_params.data)
+        self.steps = {k: 0 for k in self.GROUPS}
+        native.load()
+
+    @property
+    def n(self) -> int:
+        return int(self.params["positions"].shape[0])
+
+    def _validate(self):
+        n = self.n
+        for k, w in zip(NHT_GROUPS, NHT_WIDTHS):
+            t = self.params[k]
+            _check(t.data, k)
+            if tuple(t.shape) != (n, w):
+                raise RuntimeError(f"{k}: expected shape {(n, w)}, got {tuple(t.shape)}")
+        _check(self.decoder_params.data, "decoder params")
+        if self.decoder_params.dim() != 1:
+            raise RuntimeError("decoder params: expected the flat parameter vector")
+
+    def _tensors(self, which: str):
+        if which == "param":
+            return [self.params[k].data for k in NHT_GROUPS] + [self.decoder_params.data]
+        if which == "m":
+            return [self.exp_avg[k] for k in NHT_GROUPS] + [self.decoder_exp_avg]
+        return [self.exp_avg_sq[k] for k in NHT_GROUPS] + [self.decoder_exp_avg_sq]
+
+    @torch.no_grad()
+    def step(self, d_particles: torch.Tensor, d_features: torch.Tensor, d_decoder: torch.Tensor, visibility: torch.Tensor | None = None,
+             lambda_opacity: float = 0.0, lambda_scale: float = 0.0, frozen=()):
+        frozen = set(frozen)
+        unknown = frozen - set(self.GROUPS)
+        if unknown:
+            raise ValueError(f"frozen: unknown groups {sorted(unknown)} (groups: {', '.join(self.GROUPS)})")
+        for t, what in ((d_particles, "d_particles"), (d_features, "d_features"), (d_decoder, "d_decoder")):
+            _check(t, what)
+        self._validate()  # the tensors may have been replaced (densification); moments must have followed
+        for k in NHT_GROUPS:
+            if self.exp_avg[k].shape != self.params[k].shape or self.exp_avg_sq[k].shape != self.params[k].shape:
+                raise RuntimeError(f"{k}: optimizer state does not match the parameter shape {tuple(self.params[k].shape)}")
+        n_dec = int(self.decoder_params.numel())
+        if tuple(d_particles.shape) != (self.n, 12) or tuple(d_features.shape) != (self.n, 48) or tuple(d_decoder.shape) != (n_dec,):
+            raise RuntimeError(f"gradient shapes must be [N,12], [N,48] and [{n_dec}]")
+        vis_ptr = None
+        if self.selective:
+            if visibility is None:
+                raise RuntimeError("selective mode needs the renderer's visibility")
+            vis = visibility.reshape(-1)
+            if vis.dtype != torch.float32:
+                vis = vis.to(torch.float32)
+            vis = vis.contiguous()
+            _check(vis, "visibility")
+            vis_ptr = vis.data_ptr()
+        mask = 0
+        for i, k in enumerate(self.GROUPS):
+            if k in frozen:
+                mask |= 1 << i
+            else:
+                self.steps[k] += 1
+        arr = lambda ts: (C.c_void_p * 6)(*[t.data_ptr() for t in ts])  # noqa: E731
+        lr = (C.c_float * 6)(*[self.lrs[k] for k in self.GROUPS])
+        steps = (C.c_int64 * 6)(*[self.steps[k] for k in self.GROUPS])
+        reg_density, reg_scale = float(lambda_opacity) / max(self.n, 1), float(lambda_scale) / (3 * max(self.n, 1))
+        dev = d_particles.device
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):
+            rc = native.load().gutb200_nht_adam_step(stream, self.n, n_dec, arr(self._tensors("param")), arr(self._tensors("m")),
+                                                     arr(self._tensors("v")), lr, steps, self.betas[0], self.betas[1], self.eps,
+                                                     int(self.selective), self.decoder_betas[0], self.decoder_betas[1], self.decoder_eps,
+                                                     self.decoder_weight_decay, mask, d_particles.data_ptr(), d_features.data_ptr(),
+                                                     d_decoder.data_ptr(), vis_ptr, reg_density, reg_scale)
+        if rc != 0:
+            raise RuntimeError(f"gutb200_nht_adam_step failed ({rc})")

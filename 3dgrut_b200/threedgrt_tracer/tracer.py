@@ -166,14 +166,12 @@ class OptixTracer:
                   min_transmittance, out=None):
         """optixTracer.cpp:962-1031 -> (dDensity [N,12], dFeatures [N,48]).  out=(d_particles [N,12], d_sph [N,48]): contiguous float32
         tensors to write the gradients into (e.g. views of a flat exchange buffer); they are zeroed first and returned.  With NHT features
-        dFeatures is the fp32 [N,48] feature gradient.
+        dFeatures is the fp32 [N,48] feature gradient, and `out` is taken the same way.
         The reference's Slang backward reads the forward's features rounded to fp16 under render.feature_output_half; this one reads
         them as the forward wrote them, in fp32 (feature_output_half is not applied, DESIGN.md section 13)."""
         if self._nht is not None:
-            if out is not None:
-                raise NotImplementedError("trace_bwd(out=...) is not built for NHT features")
             return self._trace_bwd_nht(ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, particle_density,
-                                       particle_features, ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance)
+                                       particle_features, ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance, out)
         dev = ray_ori.device
         b, h, w = (int(v) for v in ray_ori.shape[:3])
         n = int(particle_density.shape[0])
@@ -184,14 +182,7 @@ class OptixTracer:
         g_d = ray_hit_distance_grd.contiguous().float()
         if g_d.shape[-1] != 1:
             g_d = g_d[..., 0:1].contiguous()
-        if out is None:
-            d_density = torch.empty((max(n, 1), 12), dtype=torch.float32, device=dev)
-            d_features = torch.empty((max(n, 1), 48), dtype=torch.float32, device=dev)
-        else:
-            d_density, d_features = out
-            for t, name, k in ((d_density, "d_particles", 12), (d_features, "d_sph", 48)):
-                if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (n, k)):
-                    raise RuntimeError(f"out: {name} must be a contiguous float32 CUDA tensor [{n},{k}]")
+        d_density, d_features = self._grad_out(out, n, dev)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
         self._context(dev).trace_bwd(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
@@ -199,8 +190,20 @@ class OptixTracer:
                                      ptr(g_d), ptr(d_density), ptr(d_features))
         return d_density[:n], d_features[:n]
 
+    @staticmethod
+    def _grad_out(out, n: int, dev):
+        """The (d_particles [N,12], d_features [N,48]) pair trace_bwd writes: `out` checked, or two new tensors."""
+        if out is None:
+            return (torch.empty((max(n, 1), 12), dtype=torch.float32, device=dev),
+                    torch.empty((max(n, 1), NHT_FEATURE_DIM), dtype=torch.float32, device=dev))
+        d_density, d_features = out
+        for t, name, k in ((d_density, "d_particles", 12), (d_features, "d_sph", NHT_FEATURE_DIM)):
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (n, k)):
+                raise RuntimeError(f"out: {name} must be a contiguous float32 CUDA tensor [{n},{k}]")
+        return d_density, d_features
+
     def _trace_bwd_nht(self, ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, particle_density, features,
-                       ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance):
+                       ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance, out=None):
         dev = ray_ori.device
         b, h, w = (int(v) for v in ray_ori.shape[:3])
         n = int(particle_density.shape[0])
@@ -211,8 +214,7 @@ class OptixTracer:
         g_d = ray_hit_distance_grd.contiguous().float()
         if g_d.shape[-1] != 1:
             g_d = g_d[..., 0:1].contiguous()
-        d_density = torch.empty((max(n, 1), 12), dtype=torch.float32, device=dev)
-        d_features = torch.empty((max(n, 1), NHT_FEATURE_DIM), dtype=torch.float32, device=dev)
+        d_density, d_features = self._grad_out(out, n, dev)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
         self._context(dev).trace_bwd_nht(stream, n, ptr(particle_density), ptr(feats), NHT_FEATURE_DIM, int(self._nht["half"]),

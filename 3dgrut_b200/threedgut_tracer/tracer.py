@@ -244,9 +244,7 @@ class SplatRaster:
                   ray_hit_distance, ray_hit_distance_grd, out=None):
         """splatRaster.cpp:264-350 -> (dDensity [N,12], dRadiance [N,48]).  `out` (extension): a pair of preallocated
         tensors to write into, e.g. two views of one flat buffer so that a single all-reduce covers both.  With NHT features dRadiance
-        is the fp32 [N,48] feature gradient."""
-        if self._nht is not None and out is not None:
-            raise NotImplementedError("trace_bwd(out=...) is not built for NHT features")
+        is the fp32 [N,48] feature gradient (and `out` the [N,12] and [N,48] pair)."""
         return self._backward("backward", n_active_features, particle_density, particle_radiance, ray_ori, ray_dir, sensor_params, pose_start,
                               pose_end, ray_radiance_density, ray_radiance_density_grd, ray_hit_distance, ray_hit_distance_grd, out)
 

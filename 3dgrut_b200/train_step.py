@@ -41,13 +41,13 @@ class TrainStep:
         turns on the replica-consistent strategy.  background: "black", "white", "random" or (r, g, b), composited onto the render before
         the loss (model.background.color); "random" draws from a generator seeded background_seed + rank.  lambda_opacity / lambda_scale:
         the regularisers of the loss (loss.lambda_opacity / loss.lambda_scale when use_opacity / use_scale)."""
-        self.params = {k: params[k] for k in optimizers.GROUPS}  # ONE dict shared with the optimizer and the densifier
+        self.params = {k: params[k] for k in self.GROUPS}  # ONE dict shared with the optimizer and the densifier
         self.device = self.params["positions"].device
         self.sph_degree = int(sph_degree)
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
         self._init_renderer(conf if conf is not None else {"render": {}})
-        self.optimizer = optimizers.FusedGaussianAdam(self.params, lrs, eps=eps, selective=selective)
+        self.optimizer = self._new_optimizer(lrs, eps, selective)
         self.exchange = self._new_exchange()
         self.frame = 0
         self.lambda_l1, self.lambda_ssim = float(lambda_l1), float(lambda_ssim)  # reference defaults: 0.8 / 0.2 (configs/base_gs.yaml:172-179)
@@ -63,6 +63,11 @@ class TrainStep:
             self.densifier = cls(self.params, [self.optimizer.exp_avg, self.optimizer.exp_avg_sq], densify_conf, group=group)
         self.phase_events = None  # set to [] to record (phase, cuda event) pairs at the end of the phases of `step` that mark one
 
+    GROUPS = optimizers.GROUPS  # the raw parameter tensors the step trains
+
+    def _new_optimizer(self, lrs, eps, selective):
+        return optimizers.FusedGaussianAdam(self.params, lrs, eps=eps, selective=selective)
+
     @property
     def n(self) -> int:
         return int(self.params["positions"].shape[0])
@@ -72,10 +77,7 @@ class TrainStep:
         """[N,12] = pos3, sigmoid(density), normalize(rotation) (wxyz), exp(scale), 0 and [N,48] = cat(albedo, specular)
         (threedgut_tracer/tracer.py:176-178, threedgrt_tracer/tracer.py:61, model.py:94-118)"""
         p = self.params
-        particles = torch.cat([p["positions"], torch.sigmoid(p["density"]), torch.nn.functional.normalize(p["rotation"]), torch.exp(p["scale"]),
-                               torch.zeros_like(p["density"])], dim=1).contiguous()
-        sph = torch.cat([p["features_albedo"], p["features_specular"]], dim=1).contiguous()
-        return particles, sph
+        return particle_record(p), torch.cat([p["features_albedo"], p["features_specular"]], dim=1).contiguous()
 
     def _mark(self, phase):
         if self.phase_events is not None:
@@ -114,17 +116,26 @@ class TrainStep:
             dist.all_reduce(vis, op=dist.ReduceOp.MAX, group=self.group)  # visible in any view of the batch (SURVEY 8e)
         self._mark("exchange")
         # the regularisers belong to the step once (every rank holds the same parameters): added after the exchange, no 1 / world
+        frozen = self._geometry_frozen()
         reg = {}
-        if self.lambda_opacity != 0.0 or self.lambda_scale != 0.0:
+        if (self.lambda_opacity != 0.0 or self.lambda_scale != 0.0) and not frozen:
             loss = loss + regulariser_loss(particles, self.lambda_opacity, self.lambda_scale)
             reg = dict(lambda_opacity=self.lambda_opacity, lambda_scale=self.lambda_scale)
-        self.optimizer.step(d_particles, d_sph, visibility=vis if self.optimizer.selective else None, **reg)
+        self._adam(d_particles, d_sph, vis if self.optimizer.selective else None, reg)
         self._mark("adam")
         self.frame += 1
-        if self.densifier is not None and self.densifier.post_optimizer_step(self.frame, self.scene_extent, positions_lr=self.optimizer.lrs["positions"]):
+        if self.densifier is not None and not frozen and self.densifier.post_optimizer_step(self.frame, self.scene_extent, positions_lr=self.optimizer.lrs["positions"]):
             self._densified()
         self._mark("densify")
         return loss
+
+    def _adam(self, d_particles, d_sph, vis, reg):
+        self.optimizer.step(d_particles, d_sph, visibility=vis, **reg)
+
+    def _geometry_frozen(self) -> bool:
+        """True while positions, density, rotation and scale are frozen (the NHT steps' colour refinement): the step then adds no
+        regulariser and does not densify."""
+        return False
 
     def _densified(self):
         """The number of Gaussians may have changed (identically on every rank): re-capacity the exchange buffers; the renderer's scratch
@@ -173,6 +184,12 @@ class GaussianTrainStep(TrainStep):
         positions = my_position[None] if all_sensor_positions is None else all_sensor_positions
         return self._update(loss, particles, vis, all_sensor_positions, my_position,
                             (self.sph_degree, particles, np.asarray(positions, np.float32)))
+
+
+def particle_record(p: dict) -> torch.Tensor:
+    """The activated [N,12] record of the raw parameter dict p: pos3, sigmoid(density), normalize(rotation) (wxyz), exp(scale), 0."""
+    return torch.cat([p["positions"], torch.sigmoid(p["density"]), torch.nn.functional.normalize(p["rotation"]), torch.exp(p["scale"]),
+                      torch.zeros_like(p["density"])], dim=1).contiguous()
 
 
 def regulariser_loss(particles, lambda_opacity: float, lambda_scale: float):

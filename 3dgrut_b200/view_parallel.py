@@ -138,22 +138,25 @@ class FlatGradientExchange:
     not apply: there a Gaussian's SH gradient in one view is basis(one direction) x g, while 3DGRT evaluates the radiance along every ray
     that hits the Gaussian, so its SH gradient is a sum over rays with different directions and has no 4-float summary."""
 
-    def __init__(self, n: int, device, group=None):
-        self.n, self.group = int(n), group
+    def __init__(self, n: int, device, group=None, tail: int = 0):
+        """tail: floats of one more gradient after the per-Gaussian rows, summed in the same all-reduce (`d_tail`, e.g. the NHT feature
+        decoder's parameter gradient); 0 for none."""
+        self.n, self.group, self.tail = int(n), group, int(tail)
         self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
-        self.bucket = GradientBucket([(self.n, 12), (self.n, 48)], device)
-        self.d_particles, self.d_sph = self.bucket.views
+        self.bucket = GradientBucket([(self.n, 12), (self.n, 48)] + ([(self.tail,)] if self.tail else []), device)
+        self.d_particles, self.d_sph = self.bucket.views[:2]
+        self.d_tail = self.bucket.views[2] if self.tail else None
 
     def out(self):
         """The (d_particles, d_sph) pair to pass as `out=` to OptixTracer.trace_bwd."""
         return self.d_particles, self.d_sph
 
     def exchange(self):
-        """Sums the buffer over the ranks (no-op on one rank); returns (d_particles [N,12], d_sph [N,48])."""
+        """Sums the buffer over the ranks (no-op on one rank), the tail included; returns (d_particles [N,12], d_sph [N,48])."""
         self.bucket.all_reduce(group=self.group)
         return self.d_particles, self.d_sph
 
     def bytes_on_wire(self) -> int:
-        """Bytes a rank sends + receives per step with a ring all-reduce: 2 (w-1)/w x 240 N."""
+        """Bytes a rank sends + receives per step with a ring all-reduce: 2 (w-1)/w x (240 N + 4 tail)."""
         w = self.world
-        return int(2 * (w - 1) / w * 240 * self.n) if w > 1 else 0
+        return int(2 * (w - 1) / w * (240 * self.n + 4 * self.tail)) if w > 1 else 0

@@ -142,6 +142,18 @@ int gutb200_gaussian_adam_step(void* stream, int64_t n, float* const* params6, f
 int gutb200_gaussian_adam_step_reg(void* stream, int64_t n, float* const* params6, float* const* exp_avg6, float* const* exp_avg_sq6,
                                    const float* lr6, float b1, float b2, float eps, int64_t step, int32_t selective, const float* d_particles,
                                    const float* d_sph, const float* visibility, float reg_density, float reg_scale);
+/* gutb200_nht_adam_step (ours): the same one-launch step for the NHT model plus its feature decoder.  params6 / exp_avg6 / exp_avg_sq6 =
+ * {positions [n,3], density [n,1], rotation [n,4], scale [n,3], features [n,48], decoder params [n_decoder]}; lr6 their learning rates;
+ * steps6 each group's own Adam step count (>= 1 where bias-corrected).  The four geometry groups take the chain rule of
+ * gutb200_gaussian_adam_step from d_particles [n,12]; features are raw, their gradient is d_features [n,48]; the decoder's gradient is
+ * d_decoder [n_decoder] plus decoder_weight_decay x param (torch.optim.Adam weight_decay), with decoder_b1 / decoder_b2 / decoder_eps and
+ * never the selective rule.  Bit k of frozen_mask freezes group k: it launches no block and its parameters and moments are not touched
+ * (their pointers and gradients may then be NULL).  reg_density / reg_scale as in gutb200_gaussian_adam_step_reg (0 = none). */
+int gutb200_nht_adam_step(void* stream, int64_t n, int64_t n_decoder, float* const* params6, float* const* exp_avg6,
+                          float* const* exp_avg_sq6, const float* lr6, const int64_t* steps6, float b1, float b2, float eps, int32_t selective,
+                          float decoder_b1, float decoder_b2, float decoder_eps, float decoder_weight_decay, int32_t frozen_mask,
+                          const float* d_particles, const float* d_features, const float* d_decoder, const float* visibility, float reg_density,
+                          float reg_scale);
 
 /* Image loss of the training step and its gradient (SURVEY.md 8f row 3): loss = lambda_l1 mean|x - y| + lambda_ssim (1 - SSIM(x, y))
  * (threedgrut/trainer.py:698-739, model/losses.py:20-33 -> fused_ssim(..., padding="valid"), third-party fused-ssim @ 1272e21).
