@@ -167,11 +167,12 @@ def leaves(particles, feats, device="cpu", requires_grad=True):
 
 
 def frame(cfg, particles, feats, rays_o, rays_d, ray_to_world, d_feat=None, d_alpha=None, d_dist=None, primitive="instances",
-          clamping=True, device="cpu"):
+          clamping=True, device="cpu", lists_f64=True):
     """Forward (and with the output gradients, the backward by autograd) of one frame.  Returns numpy arrays: feat [R,24], alpha [R],
-    dist [R,2] (integrated distance, last), hits [R], lists and, with gradients, dp [N,12] (pos, density, quat, scale, 0), df [N,48]."""
+    dist [R,2] (integrated distance, last), hits [R], lists and, with gradients, dp [N,12] (pos, density, quat, scale, 0), df [N,48].
+    lists_f64=False composites over the lists of the fp32 oracle instead (accept decisions in fp32): the other half of a yardstick."""
     n = np.asarray(particles).shape[0]
-    lists = trace_lists(cfg, particles, rays_o, rays_d, ray_to_world, clamping=clamping, f64=True, primitive=primitive)
+    lists = trace_lists(cfg, particles, rays_o, rays_d, ray_to_world, clamping=clamping, f64=lists_f64, primitive=primitive)
     o, d = world_rays(rays_o, rays_d, ray_to_world, device)
     params = leaves(particles, feats, device, requires_grad=d_feat is not None)
     F, A, D, H = composite(cfg, lists, o, d, params)

@@ -73,5 +73,13 @@ def rel_l2(a, b):
     return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
 
 
+def ray_sample(height, width, k, seed):
+    """Sorted flat pixel indices of a seeded uniform sample of k pixels of a height x width frame, plus its last row and last column
+    (the partly filled 8x4 ray blocks of a ragged frame)."""
+    idx = np.random.default_rng(seed).choice(height * width, size=k, replace=False)
+    edge = np.concatenate([(height - 1) * width + np.arange(width), np.arange(height) * width + width - 1])
+    return np.unique(np.concatenate([idx, edge]))
+
+
 def frac_within(a, b, atol):
     return float(np.mean(np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)) <= atol))
