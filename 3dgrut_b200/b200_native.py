@@ -92,6 +92,9 @@ SIGNATURES = {
     "gutb200_image_loss": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
     "gutb200_image_loss_rgb": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
     "gutb200_image_loss_composited": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp]),
+    "gutb200_hybrid_rays": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gutb200_hybrid_composite": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp]),
+    "gutb200_hybrid_composite_bwd": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),
     "gutb200_forward_host": (_int, [_vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_backward_host": (_int, [_vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_last_stats": (_int, [_vp, _i64p, _i64p, _i64p, _i64p]),
@@ -111,6 +114,7 @@ SIGNATURES = {
     "grtb200_build_bvh_packed": (_int, [_vp, _vp, _i64, _vp]),
     "grtb200_trace": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_bwd": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "grtb200_trace_bwd_accumulate": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_nht": (_int, _grt_trace_nht + [_vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_bwd_nht": (_int, _grt_trace_nht + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "grtb200_scene_aabb": (_int, [_vp, _vp]),
@@ -371,10 +375,11 @@ class GrtContext(_Handle):
                                             r2w_host, out_rgb, out_alpha, out_dist, out_hits, visibility), "grtb200_trace")
 
     def trace_bwd(self, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d, r2w_host, out_rgb, out_alpha,
-                  out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph):
-        self._check(self._lib.grtb200_trace_bwd(self._h, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d,
-                                                r2w_host, out_rgb, out_alpha, out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph),
-                    "grtb200_trace_bwd")
+                  out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph, accumulate=False):
+        """accumulate: add to d_particles / d_sph instead of zeroing them first (grtb200_trace_bwd_accumulate)."""
+        name = "grtb200_trace_bwd_accumulate" if accumulate else "grtb200_trace_bwd"
+        self._check(getattr(self._lib, name)(self._h, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d,
+                                             r2w_host, out_rgb, out_alpha, out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph), name)
 
     def trace_nht(self, stream, n, particles, features, feature_dim, features_half, min_t, batch, height, width, rays_o, rays_d, r2w_host,
                   out_features, out_alpha, out_dist, out_hits, visibility):

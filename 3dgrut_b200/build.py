@@ -33,6 +33,8 @@ UNITS = {
     "gut_debug.cu": [],
     # NHT feature decoder: fp16 tensor-core MLP, IEEE fp32 encoding and epilogues
     "nht_decoder.cu": [],
+    # 3DGRUT hybrid: mirror rays and the composite, no contraction so that they match hybrid.py's torch expressions bit for bit
+    "hybrid.cu": ["-fmad=false"],
 }
 
 

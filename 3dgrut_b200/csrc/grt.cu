@@ -1371,11 +1371,12 @@ int grtb200_set_replay(grtb200_ctx* c, int32_t enable) {
     return 0;
 }
 
-// Backward of either feature kind (see trace_fwd); d_sph is the [N,48] fp32 SH or feature gradient.
+// Backward of either feature kind (see trace_fwd); d_sph is the [N,48] fp32 SH or feature gradient.  The replay and the re-trace add
+// into d_particles / d_sph; accumulate = false zeroes them first.
 static int trace_bwd(grtb200_ctx* c, int fk, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
                      float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o, const float* rays_d,
                      const float* ray_to_world_host, const float* out_rgb, const float* out_alpha, const float* out_dist,
-                     const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles, float* d_sph) {
+                     const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles, float* d_sph, bool accumulate = false) {
     if (!c) return 1;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     GRT_CUDA(c, cudaSetDevice(c->device));
@@ -1384,7 +1385,7 @@ static int trace_bwd(grtb200_ctx* c, int fk, void* stream, int64_t n, const floa
     P.out_rgb = const_cast<float*>(out_rgb); P.out_alpha = const_cast<float*>(out_alpha); P.out_dist = const_cast<float*>(out_dist);
     P.d_rgb = d_rgb; P.d_alpha = d_alpha; P.d_dist = d_dist;
     P.d_particles = d_particles; P.d_sph = d_sph;
-    if (n > 0) {
+    if (n > 0 && !accumulate) {
         GRT_CUDA(c, cudaMemsetAsync(d_particles, 0, static_cast<size_t>(n) * 48, s));
         GRT_CUDA(c, cudaMemsetAsync(d_sph, 0, static_cast<size_t>(n) * 192, s));
     }
@@ -1425,6 +1426,15 @@ int grtb200_trace_bwd(grtb200_ctx* c, void* stream, int64_t n, const float* part
                       const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles, float* d_sph) {
     return trace_bwd(c, kFeatSH, stream, n, particles, sph, sph_degree, min_transmittance, batch, height, width, rays_o, rays_d,
                      ray_to_world_host, out_rgb, out_alpha, out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph);
+}
+
+int grtb200_trace_bwd_accumulate(grtb200_ctx* c, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
+                                 float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                                 const float* rays_d, const float* ray_to_world_host, const float* out_rgb, const float* out_alpha,
+                                 const float* out_dist, const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles,
+                                 float* d_sph) {
+    return trace_bwd(c, kFeatSH, stream, n, particles, sph, sph_degree, min_transmittance, batch, height, width, rays_o, rays_d,
+                     ray_to_world_host, out_rgb, out_alpha, out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph, true);
 }
 
 int grtb200_trace_bwd_nht(grtb200_ctx* c, void* stream, int64_t n, const float* particles, const void* features, int32_t feature_dim,

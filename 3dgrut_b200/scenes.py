@@ -210,3 +210,16 @@ def scene_c3(n: int = 6_000_000, seed: int = 11, width: int = 1237, height: int 
     quat = rng.normal(size=(n, 4)).astype(np.float32)
     dns = rng.beta(2.0, 2.0, n).astype(np.float32)
     return Scene("c3_bicycle_like_6m", width, height, 1040.0, 1040.0, _pack(pos, dns, quat, scl), _sph(rng, n, -1.0, 2.0, 0.15), 3, 4.5)
+
+
+# C5's mirror: the floor plane z = -1.2 with render_hybrid's reflectivity (hybrid.py); on C5's orbit (elevation 15-35 deg, vertical half-angle
+# 21.6 deg) most pixels look down onto it, only the top rows of the lowest views look above the horizon
+C5_MIRROR = dict(plane_point=(0.0, 0.0, -1.2), plane_normal=(0.0, 0.0, 1.0), reflectivity=0.3)
+
+
+def scene_c5(n: int = 5_000_000, seed: int = 23, width: int = 1237, height: int = 822) -> Scene:
+    """C5: garden-like unbounded scene for the 3DGRUT hybrid (primary rays through 3DGUT, C5_MIRROR reflections through 3DGRT): C3's
+    generator at 5M Gaussians with a seed of its own."""
+    sc = scene_c3(n=n, seed=seed, width=width, height=height)
+    sc.name = "c5_garden_like_5m"
+    return sc

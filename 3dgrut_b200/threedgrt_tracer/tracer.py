@@ -163,12 +163,15 @@ class OptixTracer:
 
     def trace_bwd(self, frame_id, ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, ray_normals, particle_density,
                   particle_features, ray_features_grd, ray_density_grd, ray_hit_distance_grd, ray_normals_grd, render_opts, sph_degree,
-                  min_transmittance, out=None):
+                  min_transmittance, out=None, accumulate=False):
         """optixTracer.cpp:962-1031 -> (dDensity [N,12], dFeatures [N,48]).  out=(d_particles [N,12], d_sph [N,48]): contiguous float32
-        tensors to write the gradients into (e.g. views of a flat exchange buffer); they are zeroed first and returned.  With NHT features
-        dFeatures is the fp32 [N,48] feature gradient, and `out` is taken the same way.
+        tensors to write the gradients into (e.g. views of a flat exchange buffer); they are zeroed first and returned.  accumulate=True
+        (SH radiance, with `out`): this trace's gradients are added to what `out` holds instead (grtb200_trace_bwd_accumulate), so that
+        two passes can write one buffer.  With NHT features dFeatures is the fp32 [N,48] feature gradient, and `out` is taken the same way.
         The reference's Slang backward reads the forward's features rounded to fp16 under render.feature_output_half; this one reads
         them as the forward wrote them, in fp32 (feature_output_half is not applied, DESIGN.md section 13)."""
+        if accumulate and (out is None or self._nht is not None):
+            raise NotImplementedError("trace_bwd(accumulate=True) adds SH radiance gradients into a given `out` pair")
         if self._nht is not None:
             return self._trace_bwd_nht(ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, particle_density,
                                        particle_features, ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance, out)
@@ -187,7 +190,7 @@ class OptixTracer:
         stream = torch.cuda.current_stream(dev).cuda_stream
         self._context(dev).trace_bwd(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
                                      ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(rf), ptr(rd_), ptr(rh), ptr(g_f), ptr(g_a),
-                                     ptr(g_d), ptr(d_density), ptr(d_features))
+                                     ptr(g_d), ptr(d_density), ptr(d_features), accumulate=accumulate)
         return d_density[:n], d_features[:n]
 
     @staticmethod

@@ -76,6 +76,13 @@ int grtb200_trace_bwd(grtb200_ctx* ctx, void* stream, int64_t n, const float* pa
                       const float* rays_d, const float* ray_to_world_host, const float* out_rgb, const float* out_alpha,
                       const float* out_dist, const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles,
                       float* d_sph);
+/* grtb200_trace_bwd that adds this trace's gradients to what d_particles / d_sph already hold instead of zeroing them first (ours): two
+ * passes -- e.g. the 3DGUT primary and the 3DGRT secondary rays of the hybrid step -- write one gradient buffer. */
+int grtb200_trace_bwd_accumulate(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
+                                 float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                                 const float* rays_d, const float* ray_to_world_host, const float* out_rgb, const float* out_alpha,
+                                 const float* out_dist, const float* d_rgb, const float* d_alpha, const float* d_dist, float* d_particles,
+                                 float* d_sph);
 
 /* Neural Harmonic Texture (NHT) features instead of SH radiance (model.feature_type: nht; <- the referenceSlang / referenceSlangBwd
  * pipelines, src/kernels/cuda/referenceSlangOptix.cu:103-200, referenceSlangBwdOptix.cu:103-230).  features: [N,feature_dim] rows,

@@ -178,6 +178,23 @@ int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, i
                                   const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
                                   float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2);
 
+/* 3DGRUT hybrid (ours; hybrid.py's mirror_rays and render_hybrid as device code for train_step_hybrid): primary rays through 3DGUT, one
+ * mirror bounce off a plane through 3DGRT.  No context: one launch each on `stream` of the current device, no synchronisation; 0 on success.
+ * gutb200_hybrid_rays: rays_o / rays_d [pixels,3] in camera space, T_to_world_host the 12 floats of the camera-to-world [R | t] (row-major
+ * 3x4, host), plane_point_host / plane_normal_host 3 host floats each (unit normal) -> out_o / out_d [pixels,3] world-space secondary rays
+ * and out_hit [pixels] (1 where the ray meets the plane in front of it from its front side, else 0; a ray that misses keeps its own world
+ * origin and direction).  gutb200_hybrid_composite: out_rgb [pixels,3] = primary rgb + reflectivity (1 - primary alpha) hit secondary_rgb
+ * from primary_rgba [pixels,4] (gutb200_forward's out_rgba, 16-byte aligned) and secondary_rgb [pixels,3] (grtb200_trace's out_rgb).
+ * gutb200_hybrid_composite_bwd: from d_rgb [pixels,3] and d_alpha [pixels] (NULL = 0; the loss's gradient on the primary alpha) writes every
+ * element of d_primary_rgba [pixels,4] (16-byte aligned; rgb = d_rgb, alpha = d_alpha - reflectivity hit <d_rgb, secondary_rgb>) and
+ * d_secondary_rgb [pixels,3] = reflectivity (1 - primary alpha) hit d_rgb. */
+int gutb200_hybrid_rays(void* stream, int64_t pixels, const float* rays_o, const float* rays_d, const float* T_to_world_host,
+                        const float* plane_point_host, const float* plane_normal_host, float* out_o, float* out_d, float* out_hit);
+int gutb200_hybrid_composite(void* stream, int64_t pixels, const float* primary_rgba, const float* secondary_rgb, const float* hit,
+                             float reflectivity, float* out_rgb);
+int gutb200_hybrid_composite_bwd(void* stream, int64_t pixels, const float* primary_rgba, const float* secondary_rgb, const float* hit,
+                                 float reflectivity, const float* d_rgb, const float* d_alpha, float* d_primary_rgba, float* d_secondary_rgb);
+
 int gutb200_forward_host(gutb200_ctx* ctx, const gutb200_camera* cam, int64_t n, const float* particles,
                          const float* sph, int32_t sph_degree, const float* rays_o, const float* rays_d,
                          float* out_rgba, float* out_dist, float* out_hits, float* visibility);
