@@ -57,6 +57,18 @@ class OptixTracer:
         if nht is None and int(particle_radiance_sph_degree) != 3:
             raise NotImplementedError("this build stores 16 SH coefficients per particle")
         self._nht = nht
+        # kind-dependent parts of trace / trace_bwd, resolved once: ray-feature channels, how the per-particle features are handed to the
+        # kernels, and the native forward / backward with the arguments that select the kind (SH degree, or the NHT row layout)
+        if nht is None:
+            self._out_channels, self._features = 3, torch.Tensor.contiguous
+            self._native_trace = native.GrtContext.trace
+            self._native_trace_bwd = lambda ctx, *args, accumulate: ctx.trace_bwd(*args, accumulate=accumulate)
+            self._kind_args = lambda sph_degree: (int(sph_degree),)
+        else:
+            self._out_channels, self._features = NHT_FEATURE_DIM // 2, self._nht_features
+            self._native_trace = native.GrtContext.trace_nht
+            self._native_trace_bwd = lambda ctx, *args, accumulate: ctx.trace_bwd_nht(*args)  # accumulate=True is refused for NHT
+            self._kind_args = lambda sph_degree: (NHT_FEATURE_DIM, int(nht["half"]))
         cfg = native.grt_default_config()
         cfg.kernel_degree = int(particle_kernel_degree)
         cfg.min_response = float(particle_kernel_min_response)
@@ -106,39 +118,21 @@ class OptixTracer:
     def trace(self, frame_id, ray_to_world, ray_ori, ray_dir, particle_density, particle_features, render_opts, sph_degree, min_transmittance):
         """optixTracer.cpp:893-960 -> (feat [B,H,W,3], alpha [B,H,W,1], hit [B,H,W,2], normals [B,H,W,3], hits [B,H,W,1], vis [N,1]);
         with NHT features feat is [B,H,W,24] and particle_features the [N,48] features."""
-        if self._nht is not None:
-            return self._trace_nht(ray_to_world, ray_ori, ray_dir, particle_density, particle_features, min_transmittance)
         dev = ray_ori.device
         b, h, w = (int(v) for v in ray_ori.shape[:3])
         n = int(particle_density.shape[0])
-        particle_density, particle_features = particle_density.contiguous(), particle_features.contiguous()
+        particle_density, particle_features = particle_density.contiguous(), self._features(particle_features)
         ray_ori, ray_dir = ray_ori.contiguous(), ray_dir.contiguous()
         opts = dict(dtype=torch.float32, device=dev)
-        feat, alpha = torch.empty((b, h, w, 3), **opts), torch.empty((b, h, w, 1), **opts)
+        feat, alpha = torch.empty((b, h, w, self._out_channels), **opts), torch.empty((b, h, w, 1), **opts)
         hit, hits = torch.empty((b, h, w, 2), **opts), torch.empty((b, h, w, 1), **opts)
         nrm = torch.zeros((b, h, w, 3), **opts)
         vis = torch.empty((max(n, 1), 1), **opts)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).trace(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
-                                 ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(feat), ptr(alpha), ptr(hit), ptr(hits), ptr(vis))
-        return feat, alpha, hit, nrm, hits, vis[:n]
-
-    def _trace_nht(self, ray_to_world, ray_ori, ray_dir, particle_density, features, min_transmittance):
-        dev = ray_ori.device
-        b, h, w = (int(v) for v in ray_ori.shape[:3])
-        n = int(particle_density.shape[0])
-        particle_density, feats = particle_density.contiguous(), self._nht_features(features)
-        ray_ori, ray_dir = ray_ori.contiguous(), ray_dir.contiguous()
-        opts = dict(dtype=torch.float32, device=dev)
-        feat, alpha = torch.empty((b, h, w, NHT_FEATURE_DIM // 2), **opts), torch.empty((b, h, w, 1), **opts)
-        hit, hits = torch.empty((b, h, w, 2), **opts), torch.empty((b, h, w, 1), **opts)
-        nrm = torch.zeros((b, h, w, 3), **opts)
-        vis = torch.empty((max(n, 1), 1), **opts)
-        r2w = self._r2w(ray_to_world)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).trace_nht(stream, n, ptr(particle_density), ptr(feats), NHT_FEATURE_DIM, int(self._nht["half"]), float(min_transmittance),
-                                     b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(feat), ptr(alpha), ptr(hit), ptr(hits), ptr(vis))
+        self._native_trace(self._context(dev), stream, n, ptr(particle_density), ptr(particle_features), *self._kind_args(sph_degree),
+                           float(min_transmittance), b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(feat), ptr(alpha), ptr(hit),
+                           ptr(hits), ptr(vis))
         return feat, alpha, hit, nrm, hits, vis[:n]
 
     def set_replay(self, enable, device):
@@ -172,13 +166,10 @@ class OptixTracer:
         them as the forward wrote them, in fp32 (feature_output_half is not applied, DESIGN.md section 13)."""
         if accumulate and (out is None or self._nht is not None):
             raise NotImplementedError("trace_bwd(accumulate=True) adds SH radiance gradients into a given `out` pair")
-        if self._nht is not None:
-            return self._trace_bwd_nht(ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, particle_density,
-                                       particle_features, ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance, out)
         dev = ray_ori.device
         b, h, w = (int(v) for v in ray_ori.shape[:3])
         n = int(particle_density.shape[0])
-        particle_density, particle_features = particle_density.contiguous(), particle_features.contiguous()
+        particle_density, particle_features = particle_density.contiguous(), self._features(particle_features)
         ray_ori, ray_dir = ray_ori.contiguous(), ray_dir.contiguous()
         rf, rd_, rh = ray_features.contiguous(), ray_density.contiguous(), ray_hit_distance.contiguous()
         g_f, g_a = ray_features_grd.contiguous().float(), ray_density_grd.contiguous().float()
@@ -188,9 +179,9 @@ class OptixTracer:
         d_density, d_features = self._grad_out(out, n, dev)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).trace_bwd(stream, n, ptr(particle_density), ptr(particle_features), int(sph_degree), float(min_transmittance), b, h, w,
-                                     ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(rf), ptr(rd_), ptr(rh), ptr(g_f), ptr(g_a),
-                                     ptr(g_d), ptr(d_density), ptr(d_features), accumulate=accumulate)
+        self._native_trace_bwd(self._context(dev), stream, n, ptr(particle_density), ptr(particle_features), *self._kind_args(sph_degree),
+                               float(min_transmittance), b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(rf), ptr(rd_), ptr(rh),
+                               ptr(g_f), ptr(g_a), ptr(g_d), ptr(d_density), ptr(d_features), accumulate=accumulate)
         return d_density[:n], d_features[:n]
 
     @staticmethod
@@ -204,26 +195,6 @@ class OptixTracer:
             if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (n, k)):
                 raise RuntimeError(f"out: {name} must be a contiguous float32 CUDA tensor [{n},{k}]")
         return d_density, d_features
-
-    def _trace_bwd_nht(self, ray_to_world, ray_ori, ray_dir, ray_features, ray_density, ray_hit_distance, particle_density, features,
-                       ray_features_grd, ray_density_grd, ray_hit_distance_grd, min_transmittance, out=None):
-        dev = ray_ori.device
-        b, h, w = (int(v) for v in ray_ori.shape[:3])
-        n = int(particle_density.shape[0])
-        particle_density, feats = particle_density.contiguous(), self._nht_features(features)
-        ray_ori, ray_dir = ray_ori.contiguous(), ray_dir.contiguous()
-        rf, rd_, rh = ray_features.contiguous(), ray_density.contiguous(), ray_hit_distance.contiguous()
-        g_f, g_a = ray_features_grd.contiguous().float(), ray_density_grd.contiguous().float()
-        g_d = ray_hit_distance_grd.contiguous().float()
-        if g_d.shape[-1] != 1:
-            g_d = g_d[..., 0:1].contiguous()
-        d_density, d_features = self._grad_out(out, n, dev)
-        r2w = self._r2w(ray_to_world)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        self._context(dev).trace_bwd_nht(stream, n, ptr(particle_density), ptr(feats), NHT_FEATURE_DIM, int(self._nht["half"]),
-                                         float(min_transmittance), b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(rf), ptr(rd_), ptr(rh),
-                                         ptr(g_f), ptr(g_a), ptr(g_d), ptr(d_density), ptr(d_features))
-        return d_density[:n], d_features[:n]
 
     def native_context(self, device=None) -> native.GrtContext:
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
