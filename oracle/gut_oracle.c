@@ -886,7 +886,7 @@ void gut_oracle_render_forward(const gut_oracle_config* cfg, const gut_oracle_ca
 /* G6 with a k-buffer (GAUSSIAN_K_BUFFER_SIZE = K > 0, "sorted" 3DGUT: renderers/gutKBufferRenderer.cuh:62-112 insert / closestHit,
  * :150-225 processHitParticle forward branch, :274-352 evalKBuffer).  Hits enter a per-ray buffer of the K farthest-so-far hits sorted
  * by hit distance; when it is full the closest one is composited before the new hit is inserted; the rest is composited in order at the
- * end.  Groundwork for the next round: the CUDA path builds K = 0 only (threedgut_tracer/tracer.py raises for k_buffer_size > 0). */
+ * end.  The CUDA twin is 3dgrut_b200/csrc/gut_render_kbuffer.cu (walk in kbuffer_walk.cuh); tests/test_kbuffer_gpu.py compares the two. */
 typedef struct { int idx; real t, alpha; } khit_t;
 
 void gut_oracle_render_forward_kbuffer(const gut_oracle_config* cfg, const gut_oracle_camera* cam, int32_t K, const float* rays_o,

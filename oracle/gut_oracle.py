@@ -180,7 +180,7 @@ def render_forward(cfg, cam, rays_o, rays_d, particles, pr: Projection, bn: Binn
 
 
 def render_forward_kbuffer(cfg, cam, k: int, rays_o, rays_d, particles, pr: Projection, bn: Binning, f64: bool = False):
-    """Sorted 3DGUT forward (GAUSSIAN_K_BUFFER_SIZE = k > 0, gutKBufferRenderer.cuh:62-112,274-352); groundwork, no CUDA twin yet."""
+    """Sorted 3DGUT forward (GAUSSIAN_K_BUFFER_SIZE = k > 0, gutKBufferRenderer.cuh:62-112,274-352); CUDA twin: gut_render_kbuffer.cu."""
     rays_o, rays_d, particles = _f32(rays_o).reshape(-1, 3), _f32(rays_d).reshape(-1, 3), _f32(particles)
     h, w = cam.height, cam.width
     rgba = np.zeros((h, w, 4), np.float32)

@@ -60,6 +60,25 @@ def oracle_frame(sc, c2w, seed=0, pose=None, with_f64=False):
     return out
 
 
+def kbuffer_premises(label, cfg, cam, k, ro, rd, particles, pr, bn, hits):
+    """What a k-buffer case exercises, from the oracle on the same lists: the longest tile list, the share of pixels whose ray accepts more
+    than k hits (the full buffer flushes its closest hit before the list ends), and the pixels whose ray stops below min_transmittance
+    before its last accepted hit -- at a flush (the walk stops inside the list) or while the buffer drains after the list.  `hits` are the
+    case's composited hit counts.  The accepted hits of every ray come from the float64 oracle with min_transmittance = 0 (nothing stops,
+    nothing underflows)."""
+    lens = bn.ranges[:, 1].astype(np.int64) - bn.ranges[:, 0]
+    open_cfg = type(cfg).from_buffer_copy(cfg)
+    open_cfg.min_transmittance = 0.0
+    accepted = go.render_forward_kbuffer(open_cfg, cam, k, ro, rd, particles, pr, bn, f64=True)[2].reshape(-1)
+    hits = np.asarray(hits, np.float32).reshape(-1)
+    stopped = hits < accepted
+    out = dict(longest=int(lens.max()) if lens.size else 0, over_k=float(np.mean(accepted > k)),
+               at_flush=float(np.mean(stopped & (hits <= accepted - k))), in_drain=float(np.mean(stopped & (hits > accepted - k))))
+    print(f"[kbuffer] {label} K={k}: longest tile list {out['longest']}, pixels with > K accepted hits {out['over_k'] * 100:.2f} %, "
+          f"stopped below min_transmittance at a flush {out['at_flush'] * 100:.2f} % / while draining {out['in_drain'] * 100:.2f} %")
+    return out
+
+
 def image_error_report(name, got, ref, atol=1e-4):
     """(mean abs err, max abs err, number of pixels with any channel off by more than atol)"""
     e = np.abs(np.asarray(got, np.float64) - np.asarray(ref, np.float64)).reshape(ref.shape[0] * ref.shape[1], -1).max(1)

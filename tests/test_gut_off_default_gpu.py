@@ -52,8 +52,16 @@ def _set(cfg, settings):
     return cfg
 
 
-def _oracle(sc, pose, settings, deg, seed, ro=None, rd=None, with_f64=False):
-    """Oracle forward + backward with `settings` applied to go.default_config(), SH degree `deg`; optional per-pixel rays."""
+def _oracle(sc, pose, settings, deg, seed, ro=None, rd=None, with_f64=False, k=0):
+    """Oracle forward + backward with `settings` applied to go.default_config(), SH degree `deg`; optional per-pixel rays.  k > 0: the
+    sorted variant (the oracle's k-buffer forward and backward with a buffer of k hits), its float64 pair included."""
+    if k:
+        from test_kbuffer_gpu import kbuffer_oracle
+
+        cam = go.make_camera(sc.width, sc.height, sc.fx, sc.fy, sc.cx, sc.cy, pose)
+        out = kbuffer_oracle(sc, cam, k, settings, deg, seed, ro=ro, rd=rd, with_f64=with_f64)
+        out["cam"] = cam
+        return out
     cfg = _set(go.default_config(), settings)
     cam = go.make_camera(sc.width, sc.height, sc.fx, sc.fy, sc.cx, sc.cy, pose)
     if ro is None:
@@ -68,6 +76,15 @@ def _oracle(sc, pose, settings, deg, seed, ro=None, rd=None, with_f64=False):
         r64, d64, _ = go.render_forward(cfg, cam, ro, rd, sc.particles, pr, bn, f64=True)
         out["dp_64"], out["ds_64"] = go.render_backward(cfg, cam, ro, rd, sc.particles, sc.sph, deg, pr, bn, r64, d64, d_rgba, d_dist, f64=True)
     return out
+
+
+def _premises(label, sc, ref, k):
+    """kbuffer_premises of a k > 0 case (nothing for k = 0)."""
+    if not k:
+        return None
+    from helpers import kbuffer_premises
+
+    return kbuffer_premises(label, ref["cfg"], ref["cam"], k, ref["ro"], ref["rd"], sc.particles, ref["pr"], ref["bn"], ref["hits"])
 
 
 def _native_camera(sc, pose):
@@ -196,13 +213,13 @@ class _Gaussians:
         return self._sph
 
 
-def _tracer_render(sc, c2w, deg, ref):
+def _tracer_render(sc, c2w, deg, ref, k=0):
     """Tracer.render + autograd with the oracle's output gradients; returns (rgba, dist, hits, dp [N,12], ds [N,48])."""
     import threedgut_tracer
     from test_gut_parity_gpu import _Batch
 
     dev = torch.device("cuda", 0)
-    tr = threedgut_tracer.Tracer({"render": {}})
+    tr = threedgut_tracer.Tracer({"render": {"splat": {"k_buffer_size": k}}})
     g = _Gaussians(sc, deg, dev)
     out = tr.render(g, _Batch(sc, c2w, dev), train=True)
     loss = (out["pred_features"] * torch.from_numpy(ref["d_rgba"][None, ..., :3]).to(dev)).sum() \
@@ -217,23 +234,40 @@ def _tracer_render(sc, c2w, deg, ref):
     return rgba, out["pred_dist"][0].detach().cpu().numpy(), out["hits_count"][0].detach().cpu().numpy(), dp, g._sph.grad.cpu().numpy()
 
 
-@pytest.mark.parametrize("frame", ["c1_cam0", "dense"])
-@pytest.mark.parametrize("deg", [0, 1, 2])
-def test_sh_degree_parity(deg, frame):
+def _cases(*axes):
+    """pytest.param over the product of `axes` (lists of (value, id)) and k in {0, 16}; the k = 0 cases keep the ids they had before k
+    became an input, the k = 16 ones end in -k16."""
+    import itertools
+
+    out = []
+    for k in (0, 16):
+        for combo in itertools.product(*axes):
+            ident = "-".join(i for _, i in combo) + ("-k16" if k else "")
+            out.append(pytest.param(*[v for v, _ in combo], k, id=ident))
+    return out
+
+
+@pytest.mark.parametrize("deg,frame,k", _cases([(d, str(d)) for d in (0, 1, 2)], [(f, f) for f in ("c1_cam0", "dense")]))
+def test_sh_degree_parity(deg, frame, k):
     """n_active_features = deg < 3 through the C ABI and through Tracer.render: the projection's radiance (DBG_RGB), the image, the five
     gradients, and exact zeros in d_sph beyond (deg + 1)^2 coefficients and on invisible particles.  At degree 0 the radiance does not
-    depend on the view direction, so d_pos carries no direction term; it is checked on its own as well."""
+    depend on the view direction, so d_pos carries no direction term; it is checked on its own as well.  k = 16: the sorted variant against
+    the oracle's k-buffer, and Tracer.render + autograd against the C ABI (the same trace / trace_bwd kernels: equal up to the order of the
+    float atomics)."""
     sc, cam_index, n_cams = _c1_frame(frame)
     sc = dataclasses.replace(sc, sph_degree=deg)
     c2w = sc.camera(cam_index, n_cams)
     pose = tracer_pose(c2w)
     dense = frame == "dense"
-    ref = _oracle(sc, pose, {}, deg, seed=10 + deg, with_f64=dense)
+    ref = _oracle(sc, pose, {}, deg, seed=10 + deg, with_f64=dense, k=k)
     if dense:
         assert _list_stats(f"{frame} sh{deg}", ref["bn"]).max() > 256
+    pre = _premises(f"{frame} sh{deg}", sc, ref, k)
+    if k:
+        assert pre["over_k"] > 0.05
     visible = ref["pr"].tiles_count > 0
-    label = f"{frame} sh{deg} c-abi"
-    got = _native(sc, pose, {}, deg, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
+    label = f"{frame} sh{deg}{f' K={k}' if k else ''} c-abi"
+    got = _native(sc, pose, dict(k_buffer_size=k), deg, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
     _check_integers(label, got, ref)
     rgb_err = float(np.abs(got["rgb"][visible] - ref["pr"].rgb[visible]).max())
     print(f"[off-default] {label}: projected radiance max |diff| {rgb_err:.2e} (bar 2e-6 + 1e-6 rel)")
@@ -245,23 +279,28 @@ def test_sh_degree_parity(deg, frame):
         e = rel_l2(got["dp"][:, 0:3], ref["dp"][:, 0:3])
         print(f"[off-default] {label}: d_pos rel-L2 {e:.2e} (no direction term at degree 0)")
         assert e <= 1e-3 or dense  # dense: covered by the yardstick rule above
-    label = f"{frame} sh{deg} Tracer.render"
-    rgba, dist, hits, dp, ds = _tracer_render(sc, c2w, deg, ref)
+    label = f"{frame} sh{deg}{f' K={k}' if k else ''} Tracer.render"
+    rgba, dist, hits, dp, ds = _tracer_render(sc, c2w, deg, ref, k)
     _check_image(label, rgba, dist, hits, ref)
     _check_gradients(label, dp, ds, ref)
     _check_sh_zeros(label, ds, deg, visible)
+    e = max(rel_l2(dp, got["dp"]), rel_l2(ds, got["ds"]))
+    print(f"[off-default] {label}: gradients vs the C ABI's rel-L2 {e:.2e}{' (bar 1e-5)' if k else ''}")
+    if k:
+        assert np.array_equal(hits, got["hits"]) and e <= 1e-5
 
 
-@pytest.mark.parametrize("deg", [0, 1, 2])
-def test_compact_exchange_at_sh_degree(deg):
+@pytest.mark.parametrize("deg,k", _cases([(d, str(d)) for d in (0, 1, 2)]))
+def test_compact_exchange_at_sh_degree(deg, k):
     """gutb200_backward_compact + gutb200_sph_grad_from_views at an active degree below 3: the SH gradient rebuilt from two views'
-    [N,4] radiance gradients equals the sum of the two views' full d_sph rows, zeros beyond (deg + 1)^2 included."""
+    [N,4] radiance gradients equals the sum of the two views' full d_sph rows, zeros beyond (deg + 1)^2 included.  k = 16: the compact
+    backward of the sorted variant (G8's COMPACT, non-canonical instantiation, which reads final gradients from the accumulator rows)."""
     import threedgut_tracer
     from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1()
-    raster = threedgut_tracer.Tracer({"render": {}}).tracer_wrapper
+    raster = threedgut_tracer.Tracer({"render": {"splat": {"k_buffer_size": k}}}).tracer_wrapper
     particles, sph = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
@@ -280,44 +319,20 @@ def test_compact_exchange_at_sh_degree(deg):
         full_ds.append(ds.clone())
         rgba, dst, hits, vis = raster.trace(0, deg, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
         dp2, g = raster.trace_bwd_compact(0, deg, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst, d_dist)
-        assert rel_l2(dp2.cpu().numpy(), dp.cpu().numpy()) <= 2e-5
+        e = rel_l2(dp2.cpu().numpy(), dp.cpu().numpy())
+        print(f"[off-default] compact exchange sh{deg} K={k} view {view}: compact vs full d_particles rel-L2 {e:.2e} (bar 2e-5)")
+        assert e <= 2e-5 and float(dp.abs().max()) > 0
         gs.append(g.clone())
         pos.append(raster.sensor_position(sensor, pose, pose, W, H))
     ds_sum = (full_ds[0] + full_ds[1]).cpu().numpy()
     rebuilt = raster.sph_grad_from_views(deg, particles, np.stack(pos), torch.stack(gs)).cpu().numpy()
     err = rel_l2(rebuilt, ds_sum)
-    print(f"[off-default] compact exchange sh{deg}: rebuilt d_sph rel-L2 {err:.2e} (bar 2e-6)")
+    print(f"[off-default] compact exchange sh{deg} K={k}: rebuilt d_sph rel-L2 {err:.2e} (bar 2e-6)")
     assert np.abs(ds_sum).max() > 0
     assert err <= 2e-6
     assert np.abs(rebuilt - ds_sum).max() <= 1e-5 * max(1.0, float(np.abs(ds_sum).max()))
     used = (deg + 1) ** 2
     assert np.all(rebuilt.reshape(-1, 16, 3)[:, used:] == 0) and np.all(ds_sum.reshape(-1, 16, 3)[:, used:] == 0)
-
-
-def test_kbuffer_at_sh_degree_1():
-    """The sorted (k-buffer, K = 16) variant at active SH degree 1 against the oracle's k-buffer forward and backward."""
-    import b200_native as nat
-
-    deg, k = 1, 16
-    sc = scenes.scene_c1()
-    sc.particles[:, 8:11] *= 2.0  # overlapping Gaussians: the per-ray hit order differs from the depth order of the lists
-    c2w = sc.camera(3, 10)
-    pose = tracer_pose(c2w)
-    cfg = go.default_config()
-    cam, _ = oracle_camera(sc, c2w, pose)
-    ro, rd = sc.rays()
-    pr = go.project(cfg, cam, sc.particles, sc.sph, deg)
-    bn = go.bin_tiles(cfg, cam, pr)
-    rgba_ref, dist_ref, hits_ref = go.render_forward_kbuffer(cfg, cam, k, ro, rd, sc.particles, pr, bn)
-    rng = np.random.default_rng(1)
-    d_rgba = rng.normal(size=rgba_ref.shape).astype(np.float32)
-    d_dist = (0.1 * rng.normal(size=dist_ref.shape)).astype(np.float32)
-    dp_ref, ds_ref = go.render_backward_kbuffer(cfg, cam, k, ro, rd, sc.particles, sc.sph, deg, pr, bn, rgba_ref, dist_ref, d_rgba, d_dist)
-    got = _native(sc, pose, dict(k_buffer_size=k), deg, ro, rd, d_rgba, d_dist)
-    ref = dict(rgba=rgba_ref, dist=dist_ref, hits=hits_ref, dp=dp_ref, ds=ds_ref)
-    _check_image("kbuffer K=16 sh1", got["rgba"], got["dist"], got["hits"], ref)
-    _check_gradients("kbuffer K=16 sh1", got["dp"], got["ds"], ref)
-    _check_sh_zeros("kbuffer K=16 sh1", got["ds"], deg, pr.tiles_count > 0)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
@@ -344,25 +359,31 @@ def _opaque(sc):
     return dataclasses.replace(sc, particles=particles)
 
 
-@pytest.mark.parametrize("frame", ["c1_cam0", "c1_cam7", "c1_ragged", "dense"])
-@pytest.mark.parametrize("setting", list(SETTINGS))
-def test_render_setting_parity(setting, frame):
+@pytest.mark.parametrize("setting,frame,k", _cases([(s, s) for s in SETTINGS], [(f, f) for f in ("c1_cam0", "c1_cam7", "c1_ragged", "dense")]))
+def test_render_setting_parity(setting, frame, k):
+    """k = 16: the sorted variant against the oracle's k-buffer.  min_transmittance=0.03 there stops rays both at a flush of the full buffer
+    and while it drains; ut_alpha=0.1 on the dense frame gives one tile list of ~23k entries (the binning's global-sort path)."""
     sc, cam_index, n_cams = _c1_frame(frame)
     if setting.startswith("max_alpha"):
         sc = _opaque(sc)
     pose = tracer_pose(sc.camera(cam_index, n_cams))
     settings = SETTINGS[setting]
     dense = frame == "dense"
-    ref = _oracle(sc, pose, settings, 3, seed=cam_index, with_f64=dense)
-    label = f"{setting} {frame}"
+    ref = _oracle(sc, pose, settings, 3, seed=cam_index, with_f64=dense, k=k)
+    label = f"{setting} {frame}{f' K={k}' if k else ''}"
     lens = _list_stats(label, ref["bn"])
     if dense:
         assert lens.max() > 256
+    pre = _premises(label, sc, ref, k)
+    if k and setting == "min_transmittance=0.03":
+        assert pre["at_flush"] > 0 and pre["in_drain"] > 0, "rays must stop both at a flush and while the buffer drains"
+    if k and setting == "ut_alpha=0.1" and dense:
+        assert lens.max() > 4096, "the case is meant to take the binning's global-sort path"
     # the setting changes what the oracle computes on this frame (else the case would test nothing new)
-    base = _oracle(sc, pose, {}, 3, seed=cam_index)
+    base = _oracle(sc, pose, {}, 3, seed=cam_index, k=k)
     assert not (np.array_equal(base["bn"].sorted_values, ref["bn"].sorted_values) and np.array_equal(base["rgba"], ref["rgba"])
                 and np.array_equal(base["dp"], ref["dp"])), f"{setting} does not change the oracle's output on {frame}"
-    got = _native(sc, pose, settings, 3, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
+    got = _native(sc, pose, dict(settings, k_buffer_size=k), 3, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
     _check_integers(label, got, ref)
     _check_image(label, got["rgba"], got["dist"], got["hits"], ref)
     _check_gradients(label, got["dp"], got["ds"], ref)
@@ -440,21 +461,46 @@ def _equal_depth_runs(keys):
     return int((lens >= 2).sum()), int(lens.max()), int((lens >= 32).sum())
 
 
-def check_cloned_particles_3dgut():
-    """The clone comparison on its own (also run in a child process with GUTB200_SORT_MATCH=1)."""
+def _equal_t_clone_pairs(sc, group, ref):
+    """Clone pairs whose hits are accepted at equal distance t on the ray through the first copy's projected centre (oracle hit test)."""
+    cfg = ref["cfg"] if "cfg" in ref else go.default_config()
+    inv = go.sensor_matrices(ref["cam"])[1]
+    ro, rd = ref["ro"].reshape(sc.height, sc.width, 3), ref["rd"].reshape(sc.height, sc.width, 3)
+    pairs = 0
+    for g in np.flatnonzero(np.bincount(group) >= 2)[:200]:
+        a, b = np.flatnonzero(group == g)[:2]
+        if ref["pr"].tiles_count[a] == 0:
+            continue
+        px, py = np.clip(np.round(ref["pr"].proj_pos[a]).astype(int), 0, [sc.width - 1, sc.height - 1])
+        o = (inv[:3].T @ ro[py, px] + inv[3]).astype(np.float32)
+        d = (inv[:3].T @ rd[py, px]).astype(np.float32)
+        ha, hb = go.hit_forward(cfg, o, d, sc.particles[a]), go.hit_forward(cfg, o, d, sc.particles[b])
+        pairs += bool(ha[0] and hb[0] and ha[2] == hb[2])
+    return pairs
+
+
+def check_cloned_particles_3dgut(k=0):
+    """The clone comparison on its own (also run in a child process with GUTB200_SORT_MATCH=1).  k > 0: the sorted variant, where equal
+    hit distances leave the buffer's strict insertion order to decide which copy is composited first and so how the gradients split."""
     base = scenes.scene_c2(n=50_000, width=256, height=256)
-    sc, _ = clone_scene(base, 6000, 300, 8)
+    sc, group = clone_scene(base, 6000, 300, 8)
     c2w = sc.camera(2, 10)
     pose = tracer_pose(c2w)
-    ref = _oracle(sc, pose, {}, 3, seed=5, with_f64=True)
+    ref = _oracle(sc, pose, {}, 3, seed=5, with_f64=True, k=k)
     runs, longest, long_runs = _equal_depth_runs(ref["bn"].sorted_keys)
     lens = _list_stats(f"clones N={sc.n}", ref["bn"])
     print(f"[off-default] clones: {runs} equal-depth runs in the sorted stream, longest {longest}, {long_runs} of >= 32 entries")
     assert runs > 1000 and longest >= 32 and lens.max() > 256
-    got = _native(sc, pose, {}, 3, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
-    _check_integers("clones", got, ref)
-    _check_image("clones", got["rgba"], got["dist"], got["hits"], ref)
-    _check_gradients("clones", got["dp"], got["ds"], ref)
+    label = f"clones{f' K={k}' if k else ''}"
+    if k:
+        pre = _premises(label, sc, ref, k)
+        pairs = _equal_t_clone_pairs(sc, group, ref)
+        print(f"[off-default] {label}: {pairs} clone pairs accepted at bit-equal hit distances on a sampled ray")
+        assert pre["over_k"] > 0.05 and pairs >= 50
+    got = _native(sc, pose, dict(k_buffer_size=k), 3, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
+    _check_integers(label, got, ref)
+    _check_image(label, got["rgba"], got["dist"], got["hits"], ref)
+    _check_gradients(label, got["dp"], got["ds"], ref)
 
 
 def test_cloned_particles_3dgut():
@@ -462,6 +508,12 @@ def test_cloned_particles_3dgut():
     so tile_sort orders each run by particle index in its fix-up pass (the atomic slot claims arrive in any order): sorted keys, values
     and ranges bit-exact, and -- (depth, index) being a total order -- the image and the per-particle gradients within the bars."""
     check_cloned_particles_3dgut()
+
+
+def test_cloned_particles_3dgut_sorted():
+    """The same clones through the sorted variant (a k-buffer of 16 hits): equal hit distances, so kb_insert's strict > decides which copy
+    is composited first and how the gradients split between the copies."""
+    check_cloned_particles_3dgut(16)
 
 
 def test_cloned_particles_3dgut_match_any_sort():

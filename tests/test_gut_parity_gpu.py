@@ -286,12 +286,23 @@ def test_work_counters_are_consistent():
 
 def test_empty_and_offscreen_inputs():
     """Edge cases: zero particles, and particles all behind the camera (I = 0)."""
+    _empty_and_offscreen_inputs(0)
+
+
+def test_empty_offscreen_and_single_particle_inputs_sorted():
+    """The same edge cases through the sorted variant (a k-buffer of 16 hits), and a single particle in view against the oracle's k-buffer."""
+    _empty_and_offscreen_inputs(16)
+
+
+def _empty_and_offscreen_inputs(k):
     import b200_native as nat
 
     sc = scenes.scene_c1(n=64)
     c2w = sc.camera(0, 4)
     ref = oracle_frame(sc, c2w)
-    ctx = nat.Context(nat.default_config(), 0)
+    cfg = nat.default_config()
+    cfg.k_buffer_size = k
+    ctx = nat.Context(cfg, 0)
     cam = nat.Camera()
     cam.width, cam.height = sc.width, sc.height
     cam.principal[:] = [sc.cx, sc.cy]
@@ -315,13 +326,56 @@ def test_empty_and_offscreen_inputs():
         ctx.backward_host(cam, n, p(buf), p(sph), 3, p(ro), p(rd), p(rgba), p(rgba), p(dist), p(dist), p(dp), p(ds))
         if n:
             assert np.all(dp == 0) and np.all(ds == 0)
+    if k:
+        _single_particle_kbuffer(ctx, cam, sc, ref, k)
     ctx.close()
+
+
+def _single_particle_kbuffer(ctx, cam, sc, ref, k):
+    """One particle in view, the largest of the scene in the frame: every ray holds at most one hit, which leaves the buffer in the drain."""
+    from oracle import gut_oracle as go
+
+    vis = np.flatnonzero(ref["pr"].tiles_count > 0)
+    one = sc.particles[vis[np.argmax(ref["pr"].tiles_count[vis])]][None].copy()
+    one[:, 3] = 0.9
+    sph = np.ascontiguousarray(sc.sph[vis[:1]])
+    cfg = go.default_config()
+    pr = go.project(cfg, ref["cam"], one, sph, 3)
+    bn = go.bin_tiles(cfg, ref["cam"], pr)
+    rgba_ref, dist_ref, hits_ref = go.render_forward_kbuffer(cfg, ref["cam"], k, ref["ro"], ref["rd"], one, pr, bn)
+    d_rgba, d_dist = ref["d_rgba"], ref["d_dist"]
+    dp_ref, ds_ref = go.render_backward_kbuffer(cfg, ref["cam"], k, ref["ro"], ref["rd"], one, sph, 3, pr, bn, rgba_ref, dist_ref, d_rgba, d_dist)
+    assert hits_ref.max() == 1 and hits_ref.sum() >= 16
+    hw = sc.width * sc.height
+    p = lambda a: a.ctypes.data  # noqa: E731
+    ro, rd = np.ascontiguousarray(ref["ro"]), np.ascontiguousarray(ref["rd"])
+    rgba, dist, hits, vis1 = (np.zeros((hw, 4), np.float32), np.zeros(hw, np.float32), np.zeros(hw, np.float32), np.zeros(1, np.float32))
+    ctx.forward_host(cam, 1, p(one), p(sph), 3, p(ro), p(rd), p(rgba), p(dist), p(hits), p(vis1))
+    mean_e, max_e, bad = image_error_report(f"single particle K={k} rgba", rgba.reshape(rgba_ref.shape), rgba_ref)
+    assert mean_e <= 1e-5 and max_e <= 2e-2 and bad <= 3
+    assert np.array_equal(hits.reshape(hits_ref.shape), hits_ref)
+    dp, ds = np.zeros((1, 12), np.float32), np.zeros((1, 48), np.float32)
+    ctx.backward_host(cam, 1, p(one), p(sph), 3, p(ro), p(rd), p(rgba), p(np.ascontiguousarray(d_rgba)), p(dist),
+                      p(np.ascontiguousarray(d_dist)), p(dp), p(ds))
+    errs = (rel_l2(dp, dp_ref), rel_l2(ds, ds_ref))
+    print(f"[parity] single particle K={k}: {int(hits_ref.sum())} hit pixels, gradient rel-L2 {errs[0]:.2e} / {errs[1]:.2e} (bar 1e-3)")
+    assert max(errs) <= 1e-3
 
 
 def test_per_pixel_ray_origins_take_the_general_path():
     """Rays whose origins differ inside a tile must not use the common-origin fast path (render kernels pick it per tile).  Three bands of
     tiles: the frame's first-ray origin (forward UNIFORM, backward FAST: canonical sums relative to that origin), ANOTHER origin common to
     the tile (forward UNIFORM with exact hit words, backward GENERAL with the origin-offset correction terms), per-pixel jitter (both general)."""
+    _per_pixel_ray_origins(0)
+
+
+def test_per_pixel_ray_origins_sorted():
+    """The same three bands through the sorted variant (a k-buffer of 16 hits), whose walk sets up every ray from its own origin, against the
+    oracle's k-buffer."""
+    _per_pixel_ray_origins(16)
+
+
+def _per_pixel_ray_origins(k):
     import b200_native as nat
     from oracle import gut_oracle as go
 
@@ -336,11 +390,24 @@ def test_per_pixel_ray_origins_take_the_general_path():
     # columns 64..: per-pixel jitter
     cfg = go.default_config()
     ocam = go.make_camera(sc.width, sc.height, sc.fx, sc.fy, sc.cx, sc.cy, pose)
-    pr, bn, rgba_ref, dist_ref, hits_ref = go.forward_all(cfg, ocam, ro, rd, sc.particles, sc.sph, 3)
+    pr = go.project(cfg, ocam, sc.particles, sc.sph, 3)
+    bn = go.bin_tiles(cfg, ocam, pr)
+    if k:
+        rgba_ref, dist_ref, hits_ref = go.render_forward_kbuffer(cfg, ocam, k, ro, rd, sc.particles, pr, bn)
+    else:
+        rgba_ref, dist_ref, hits_ref = go.render_forward(cfg, ocam, ro, rd, sc.particles, pr, bn)
     d_rgba = rng.normal(size=rgba_ref.shape).astype(np.float32)
     d_dist = (0.1 * rng.normal(size=dist_ref.shape)).astype(np.float32)
-    dp_ref, ds_ref = go.render_backward(cfg, ocam, ro, rd, sc.particles, sc.sph, 3, pr, bn, rgba_ref, dist_ref, d_rgba, d_dist)
-    ctx = nat.Context(nat.default_config(), 0)
+    if k:
+        dp_ref, ds_ref = go.render_backward_kbuffer(cfg, ocam, k, ro, rd, sc.particles, sc.sph, 3, pr, bn, rgba_ref, dist_ref, d_rgba, d_dist)
+        from helpers import kbuffer_premises
+
+        assert kbuffer_premises("jittered origins", cfg, ocam, k, ro, rd, sc.particles, pr, bn, hits_ref)["over_k"] > 0.05
+    else:
+        dp_ref, ds_ref = go.render_backward(cfg, ocam, ro, rd, sc.particles, sc.sph, 3, pr, bn, rgba_ref, dist_ref, d_rgba, d_dist)
+    ncfg = nat.default_config()
+    ncfg.k_buffer_size = k
+    ctx = nat.Context(ncfg, 0)
     cam = nat.Camera()
     cam.width, cam.height = sc.width, sc.height
     cam.principal[:] = [sc.cx, sc.cy]
@@ -356,7 +423,10 @@ def test_per_pixel_ray_origins_take_the_general_path():
     assert mean_e <= 1e-5 and max_e <= 2e-2 and bad <= 3
     dp, ds = np.zeros((n, 12), np.float32), np.zeros((n, 48), np.float32)
     ctx.backward_host(cam, n, p(sc.particles), p(sc.sph), 3, p(ro_c), p(rd_c), p(rgba), p(d_rgba), p(dist), p(d_dist), p(dp), p(ds))
-    assert rel_l2(dp, dp_ref) <= 1e-3 and rel_l2(ds, ds_ref) <= 1e-3
+    assert float(np.mean(hits.reshape(hits_ref.shape) == hits_ref)) >= 0.999
+    errs = (rel_l2(dp, dp_ref), rel_l2(ds, ds_ref))
+    print(f"[parity] jittered origins K={k}: gradient rel-L2 d_particles {errs[0]:.2e}, d_sph {errs[1]:.2e} (bar 1e-3)")
+    assert max(errs) <= 1e-3
     ctx.close()
 
 

@@ -14,7 +14,8 @@ from test_grt_train_step_gpu import CONFIGS, LRS, _Batch, _free_port, _ImageLoss
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
-KINDS = ("gut", "grt_instances", "grt_icosahedron_paper")
+KINDS = ("gut", "gut_sorted", "grt_instances", "grt_icosahedron_paper")
+SORTED = {"render": {"splat": {"k_buffer_size": 16}}}  # configs/paper/3dgut/sorted_*.yaml: the k-buffer of 16 hits
 
 
 class _RawGaussians:
@@ -42,14 +43,16 @@ class _RawGaussians:
 
 
 class _Harness:
-    """One scene (C1, 600 Gaussians, 96x96, 6 views) driven through either training step."""
+    """One scene (C1, 600 Gaussians, 96x96, 6 views) driven through either training step.  gut_sorted: the 3DGUT step with the k-buffer
+    (sorted 3DGUT), whose compact backward reads final gradients from the accumulator rows."""
 
     def __init__(self, kind):
         self.kind = kind
+        self.gut = kind.startswith("gut")
         self.sc, self.rays_o, self.rays_d, self.P, self.S, self.poses = _setup()
         self.dev = self.P.device
         self.H, self.W = self.sc.height, self.sc.width
-        if kind == "gut":
+        if self.gut:
             from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
             sc = self.sc
@@ -57,27 +60,27 @@ class _Harness:
                                                                  np.array([sc.cx, sc.cy], np.float32), np.array([sc.fx, sc.fy], np.float32),
                                                                  np.zeros(6, np.float32), np.zeros(2, np.float32), np.zeros(4, np.float32))
             self.views = [scenes.pose7_from_c2w(sc.camera(i, 6)) for i in range(6)]
-            self.conf = None
+            self.conf = SORTED if kind == "gut_sorted" else None
         else:
             self.conf = CONFIGS[kind[len("grt_"):]]
 
     def make(self, raw, **kw):
-        if self.kind == "gut":
+        if self.gut:
             import train_step
 
-            return train_step.GaussianTrainStep(raw, LRS, **kw)
+            return train_step.GaussianTrainStep(raw, LRS, conf=self.conf, **kw)
         import train_step_grt
 
         return train_step_grt.GaussianTrainStepGRT(raw, LRS, conf=self.conf, **kw)
 
     def step(self, st, v, target, mask=None):
-        if self.kind == "gut":
+        if self.gut:
             return st.step(self.rays_o, self.rays_d, self.sensor, self.views[v], target, mask=mask)
         return st.step(self.rays_o, self.rays_d, self.poses[v], target, mask=mask)
 
     def render(self, st, v):
         """(rgb [H,W,3], alpha [H,W,1]) of the step's current parameters."""
-        if self.kind == "gut":
+        if self.gut:
             rgba = st.render(self.rays_o, self.rays_d, self.sensor, self.views[v])[0].reshape(self.H, self.W, 4)
             return rgba[..., :3], rgba[..., 3:]
         out = st.render(self.rays_o, self.rays_d, self.poses[v])
@@ -85,10 +88,10 @@ class _Harness:
 
     def autograd_render(self, leaves, v):
         """Tracer.render's autograd node on the activated raw leaves: (rgb [H,W,3], alpha [H,W,1])."""
-        if self.kind == "gut":
+        if self.gut:
             from threedgut_tracer.tracer import SensorPose3D, SplatRaster, Tracer
 
-            raster = SplatRaster({"render": {}})
+            raster = SplatRaster(self.conf or {"render": {}})
             pose = self.views[v]
             rgba, _, _, _ = Tracer._Autograd.apply(raster, 0, 3, self.rays_o, self.rays_d, leaves["positions"],
                                                    torch.nn.functional.normalize(leaves["rotation"]), torch.exp(leaves["scale"]),
@@ -152,7 +155,7 @@ def test_one_step_matches_autograd(kind, background):
     errs, got_loss, want_loss = _step_against_autograd(hz, background, True, 0.01, 0.02)
     assert abs(got_loss - want_loss) <= 1e-5, (got_loss, want_loss)
     floor = {}
-    if kind == "gut":
+    if kind.startswith("gut"):
         # The 3DGUT step differentiates through the compact backward, the autograd node through the full one; their rotation gradients
         # differ by ~1e-5 rel-L2 on the parent's path already (black, no mask, no regulariser), and the new terms must add nothing to it.
         floor, _, _ = _step_against_autograd(hz, "black", False, 0.0, 0.0)
@@ -160,6 +163,35 @@ def test_one_step_matches_autograd(kind, background):
         bar = max(1e-5, 2.0 * floor.get(k, 0.0))
         print(f"[loss-terms step] {kind} {background} {k}: exp_avg / (1 - b1) vs autograd rel-L2 {err:.2e} (bar {bar:.2e}"
               f"{f'; plain step {floor[k]:.2e}' if k in floor else ''})")
+        assert err <= bar, k
+
+
+@pytest.mark.parametrize("weights", [(1.0, 0.0), (0.8, 0.2)])
+def test_sorted_gut_step_matches_autograd(weights):
+    """The sorted 3DGUT step (k-buffer of 16 hits: the COMPACT, non-canonical G8 and sph_grad_from_views) with plain L1 and with L1 + SSIM,
+    black background, no mask: one step's gradients against autograd through Tracer.render with the same config."""
+    from threedgut_tracer.tracer import SplatRaster
+
+    hz = _Harness("gut_sorted")
+    errs, got_loss, want_loss = _step_against_autograd(hz, "black", False, 0.0, 0.0, weights=weights)
+    assert abs(got_loss - want_loss) <= 1e-5, (got_loss, want_loss)
+    # the compact-vs-full floor of the rotation on this frame: trace_bwd_compact against trace_bwd, same inputs
+    raster = SplatRaster(SORTED)
+    particles = torch.cat([hz.P[:, 0:11], torch.zeros_like(hz.P[:, :1])], 1).contiguous()
+    pose = hz.views[1]
+    gen = torch.Generator(device=hz.dev).manual_seed(7)
+    d_rgba = torch.randn((hz.H, hz.W, 4), device=hz.dev, generator=gen)
+    d_dist = torch.zeros((hz.H, hz.W, 1), device=hz.dev)
+    args = (0, 3, particles, hz.S, hz.rays_o, hz.rays_d, None, hz.sensor, 0, 1, pose, pose)
+    rgba, dst, _, _ = raster.trace(*args)
+    dp_full, _ = raster.trace_bwd(*args, rgba, d_rgba, dst, d_dist)
+    rgba, dst, _, _ = raster.trace(*args)
+    dp_compact, _ = raster.trace_bwd_compact(*args, rgba, d_rgba, dst, d_dist)
+    floor = rel_l2(dp_compact[:, 4:8].cpu().numpy(), dp_full[:, 4:8].cpu().numpy())
+    for k, err in errs.items():
+        bar = max(1e-5, 2.0 * floor) if k == "rotation" else 1e-5
+        print(f"[loss-terms step] gut_sorted L1 {weights[0]} SSIM {weights[1]} {k}: exp_avg / (1 - b1) vs autograd rel-L2 {err:.2e} (bar {bar:.2e}"
+              f"{f'; compact vs full rotation {floor:.2e}' if k == 'rotation' else ''})")
         assert err <= bar, k
 
 

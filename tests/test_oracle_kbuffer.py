@@ -1,5 +1,6 @@
-"""Groundwork for the sorted (k-buffer) 3DGUT variant (SURVEY.md 8f row 4; renderers/gutKBufferRenderer.cuh:62-112,274-352): the
-oracle's k-buffer forward against its defining properties.  There is no CUDA twin yet (the tracer raises for k_buffer_size > 0)."""
+"""The oracle of the sorted (k-buffer) 3DGUT variant (SURVEY.md 8f row 4; renderers/gutKBufferRenderer.cuh:62-112,274-352) against its
+defining properties.  Its CUDA twin (gut_render_kbuffer.cu) is compared with it in test_kbuffer_gpu.py, test_kbuffer_host_emul.py and the
+k = 16 cases of test_gut_off_default_gpu.py."""
 import numpy as np
 
 import scenes
