@@ -40,16 +40,65 @@ def tracer_pose(c2w):
     return Tracer._pose_from_c2w(np.asarray(c2w, np.float32))
 
 
-def oracle_frame(sc, c2w, seed=0, pose=None, with_f64=False):
+D_DIST_MODES = ("random", "zero", "mixed")
+
+
+def warp_blocks(height, width):
+    """[H, W] index of the 8x4 pixel block each pixel belongs to: the pixels of one warp of the render kernels (tile_pixel,
+    render_tile.cuh).  Tiles are 16x16 and start on multiples of 16, so the blocks tile the frame from its origin."""
+    y, x = np.mgrid[0:height, 0:width]
+    return (y // 4) * ((width + 7) // 8) + x // 8
+
+
+def dist_grad_mask(height, width, mode, seed=0):
+    """[H, W] bool: the pixels whose distance gradient is non-zero.  "random": all; "zero": none (every training step: no loss term
+    reads the distance, so each warp of the backward skips its depth branch); "mixed": every third 8x4 warp block plus a seeded 1 % of
+    the other pixels, so warps with and without the depth branch add into the same gradient rows, and some warps run it with most lanes
+    at zero."""
+    if mode == "random":
+        return np.ones((height, width), bool)
+    if mode == "zero":
+        return np.zeros((height, width), bool)
+    if mode == "mixed":
+        rng = np.random.default_rng(1000 + seed)
+        return (warp_blocks(height, width) % 3 == 0) | (rng.random((height, width)) < 0.01)
+    raise ValueError(mode)
+
+
+def dist_grad_blocks(d_dist):
+    """(warp blocks with a non-zero distance gradient on some pixel, warp blocks without) of an [H, W(, 1)] gradient."""
+    h, w = d_dist.shape[:2]
+    blocks = warp_blocks(h, w).reshape(-1)
+    has = np.zeros(blocks.max() + 1, bool)
+    np.logical_or.at(has, blocks, np.asarray(d_dist).reshape(h * w, -1).any(1))
+    return int(has.sum()), int((~has).sum())
+
+
+def output_grads(shape_rgba, seed=0, d_dist="random", d_alpha="random"):
+    """The seeded output gradients (d_rgba [H,W,C], d_dist [H,W,1]) of a backward; d_dist in D_DIST_MODES (dist_grad_mask), d_alpha
+    "zero" clears the last channel (an L1 / L2 image loss on a black background never reads the opacity).  "random" in both draws
+    what this helper always drew."""
+    h, w = shape_rgba[:2]
+    rng = np.random.default_rng(seed)
+    d_rgba = rng.normal(size=shape_rgba).astype(np.float32)
+    dd = (0.1 * rng.normal(size=(h, w, 1))).astype(np.float32)
+    dd *= dist_grad_mask(h, w, d_dist, seed)[..., None]
+    if d_alpha == "zero":
+        d_rgba[..., -1] = 0.0
+    elif d_alpha != "random":
+        raise ValueError(d_alpha)
+    return d_rgba, dd
+
+
+def oracle_frame(sc, c2w, seed=0, pose=None, with_f64=False, d_dist="random", d_alpha="random"):
     """Full oracle forward + backward for one camera; returns a dict of numpy arrays.  with_f64 adds the
-    double-precision evaluation of the compositing on the same lists (keys *_64): the tolerance yardstick."""
+    double-precision evaluation of the compositing on the same lists (keys *_64): the tolerance yardstick.  d_dist / d_alpha: which
+    output gradients the backward gets (output_grads); the float64 backward gets the same ones."""
     cfg = go.default_config()
     cam, pose = oracle_camera(sc, c2w, pose)
     ro, rd = sc.rays()
     pr, bn, rgba, dist, hits = go.forward_all(cfg, cam, ro, rd, sc.particles, sc.sph, sc.sph_degree)
-    rng = np.random.default_rng(seed)
-    d_rgba = rng.normal(size=rgba.shape).astype(np.float32)
-    d_dist = (0.1 * rng.normal(size=dist.shape)).astype(np.float32)
+    d_rgba, d_dist = output_grads(rgba.shape, seed, d_dist, d_alpha)
     dp, ds = go.render_backward(cfg, cam, ro, rd, sc.particles, sc.sph, sc.sph_degree, pr, bn, rgba, dist, d_rgba, d_dist)
     out = dict(cfg=cfg, cam=cam, pose=pose, ro=ro, rd=rd, pr=pr, bn=bn, rgba=rgba, dist=dist, hits=hits, d_rgba=d_rgba,
                d_dist=d_dist, dp=dp, ds=ds)

@@ -48,89 +48,155 @@ def features_at(P: torch.Tensor, f: torch.Tensor) -> torch.Tensor:
 
 
 def rot_rows(q):
-    r, x, y, z = q[0], q[1], q[2], q[3]
+    """[..., 4] quaternions (wxyz) -> [..., 3, 3] rotation rows."""
+    r, x, y, z = q.unbind(-1)
     return torch.stack([
-        torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y + r * z), 2 * (x * z - r * y)]),
-        torch.stack([2 * (x * y - r * z), 1 - 2 * (x * x + z * z), 2 * (y * z + r * x)]),
-        torch.stack([2 * (x * z + r * y), 2 * (y * z - r * x), 1 - 2 * (x * x + y * y)])])
+        torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y + r * z), 2 * (x * z - r * y)], -1),
+        torch.stack([2 * (x * y - r * z), 1 - 2 * (x * x + z * z), 2 * (y * z + r * x)], -1),
+        torch.stack([2 * (x * z + r * y), 2 * (y * z - r * x), 1 - 2 * (x * x + y * y)], -1)], -2)
 
 
-def render(cfg, cam_inv, width, height, ro, rd, pos, dns, quat, scl, feats, sorted_values, ranges):
-    """Composite NHT features over the sorted tile lists.  cam_inv: the [4,3] sensor->world columns of gut_oracle.sensor_matrices;
-    ro / rd [H*W,3] sensor-space rays; pos [N,3], dns [N], quat [N,4] (wxyz), scl [N,3], feats [N,48] (float64 tensors, optionally
-    requiring grad).  Returns (features + opacity [H,W,25], dist [H,W,1], hits [H,W,1]) as float64 tensors."""
-    dev = pos.device
-    inv = torch.as_tensor(np.asarray(cam_inv), dtype=F64, device=dev)
-    o_w = torch.as_tensor(np.asarray(ro).reshape(-1, 3), dtype=F64, device=dev) @ inv[:3] + inv[3]
-    d_w = torch.as_tensor(np.asarray(rd).reshape(-1, 3), dtype=F64, device=dev) @ inv[:3]
-    deg4 = int(cfg.kernel_degree) == 4
+def _pairs(cfg, o, d, pos, R, scl, dns):
+    """Exact test of (ray, particle) pairs, broadcast over the leading dimensions: o, d, pos, scl [..., 3], R [..., 3, 3], dns [...].
+    Returns (canonical origin gro, direction grd, pd = -grd . gro, alpha (clamped at max_alpha), hit distance t, accepted, clamped:
+    response x density above max_alpha)."""
+    gro = ((o - pos)[..., None, :] * R).sum(-1) / scl
+    grdu = (d[..., None, :] * R).sum(-1) / scl
+    grd = grdu / grdu.norm(dim=-1, keepdim=True)
+    gray = torch.linalg.cross(grd, gro).pow(2).sum(-1)
+    gres = torch.exp(-0.0555555555556 * gray * gray) if int(cfg.kernel_degree) == 4 else torch.exp(-0.5 * gray)
+    raw = gres * dns
+    alpha = torch.clamp(raw, max=float(cfg.max_alpha))
+    pd = -(grd * gro).sum(-1, keepdim=True)
+    t = (scl * grd * pd).norm(dim=-1)
+    acc = (gres > float(cfg.min_kernel_density)) & (alpha > float(cfg.min_alpha)) & (t > 0)
+    return gro, grd, pd, alpha, t, acc, raw > float(cfg.max_alpha)
+
+
+def tile_pixels(tile, width, height):
+    """Flat indices of the pixels of 16x16 tile `tile` (row-major tiles, partial on the right and bottom edges)."""
     gx = (width + 15) // 16
+    tx, ty = tile % gx, tile // gx
+    ys, xs = np.meshgrid(np.arange(ty * 16, min(height, ty * 16 + 16)), np.arange(tx * 16, min(width, tx * 16 + 16)), indexing="ij")
+    return (ys * width + xs).reshape(-1)
+
+
+def accepted_pairs(cfg, o, d, pos, quat, scl, dns, entries, max_pairs=1 << 18):
+    """Without gradients: which entries of one tile's list each pixel composites.  o, d [m,3] world rays; entries [L] particle indices in
+    list order.  The walk of every pixel accepts a pair when response > min_kernel_density, alpha > min_alpha and t > 0, and stops
+    once its transmittance is below min_transmittance.  Entries are tested in chunks of at most max_pairs (pixel, entry) pairs; the
+    transmittance carries from chunk to chunk.  Returns ([m, K] list positions of the composited entries, front to back, padded with
+    0; [m, K] validity), K = the largest count of the tile."""
+    m, L = o.shape[0], entries.shape[0]
+    dev = o.device
+    chunk = max(1, max_pairs // max(m, 1))
+    T = torch.ones(m, dtype=o.dtype, device=dev)
+    taken = []
+    with torch.no_grad():
+        for c in range(0, L, chunk):
+            i = entries[c:c + chunk]
+            _, _, _, alpha, _, acc, _ = _pairs(cfg, o[:, None], d[:, None], pos[i], rot_rows(quat[i]), scl[i], dns[i])
+            cp = torch.cumprod(torch.where(acc, 1 - alpha, torch.ones_like(alpha)), 1)
+            T_before = T[:, None] * torch.cat([torch.ones_like(cp[:, :1]), cp[:, :-1]], 1)
+            taken.append(acc & (T_before >= float(cfg.min_transmittance)))
+            T = T * cp[:, -1]
+        taken = torch.cat(taken, 1) if taken else torch.zeros((m, 0), dtype=torch.bool, device=dev)
+        K = int(taken.sum(1).max()) if L else 0
+        order = torch.sort(torch.where(taken, torch.arange(L, device=dev), torch.full_like(taken, L, dtype=torch.long)), 1).values[:, :K]
+    valid = order < L
+    return torch.where(valid, order, torch.zeros_like(order)), valid
+
+
+def render_tile(cfg, o_w, d_w, width, height, pos, dns, quat, scl, feats, sorted_values, ranges, tile):
+    """One tile: (pixel indices [m], features + opacity [m,25], dist [m], hits [m], longest composited list K, number of composited
+    pairs whose alpha is clamped at max_alpha).  Autograd runs over
+    the gathered composited pairs only, with the transmittance in front of each from a cumprod."""
+    dev = pos.device
+    pix = torch.as_tensor(tile_pixels(tile, width, height), device=dev)
+    o, d = o_w[pix], d_w[pix]
+    b, e = (int(v) for v in ranges[tile])
+    entries = torch.as_tensor(np.asarray(sorted_values[b:e], np.int64), device=dev)
+    k, valid = accepted_pairs(cfg, o, d, pos, quat, scl, dns, entries)
+    i = entries[k]
+    gro, grd, pd, alpha, t, _, clamped = _pairs(cfg, o[:, None], d[:, None], pos[i], rot_rows(quat[i]), scl[i], dns[i])
+    alpha = torch.where(valid, alpha, torch.zeros_like(alpha))
+    cp = torch.cumprod(1 - alpha, 1)
+    w = alpha * torch.cat([torch.ones_like(cp[:, :1]), cp[:, :-1]], 1)
+    Fe = (w[..., None] * features_at(gro + grd * pd, feats[i])).sum(1)
+    T = cp[:, -1] if cp.shape[1] else torch.ones(len(pix), dtype=pos.dtype, device=dev)
+    D = (w * t).sum(1)
+    H = (valid & (w > 0)).sum(1).to(pos.dtype)
+    return pix, torch.cat([Fe, (1 - T)[:, None]], 1), D, H, k.shape[1], int((clamped & valid).sum())
+
+
+def world_rays(cam_inv, ro, rd, dtype, device):
+    inv = torch.as_tensor(np.asarray(cam_inv), dtype=dtype, device=device)
+    o_w = torch.as_tensor(np.asarray(ro).reshape(-1, 3), dtype=dtype, device=device) @ inv[:3] + inv[3]
+    d_w = torch.as_tensor(np.asarray(rd).reshape(-1, 3), dtype=dtype, device=device) @ inv[:3]
+    return o_w, d_w
+
+
+def render(cfg, cam_inv, width, height, ro, rd, pos, dns, quat, scl, feats, sorted_values, ranges, tiles=None):
+    """Composite NHT features over the sorted tile lists.  cam_inv: the [4,3] sensor->world columns of gut_oracle.sensor_matrices;
+    ro / rd [H*W,3] sensor-space rays; pos [N,3], dns [N], quat [N,4] (wxyz), scl [N,3], feats [N,48] (tensors of one floating
+    dtype -- float64 for the oracle, float32 for its yardstick -- optionally requiring grad).  tiles: the tile indices to render
+    (default all); other pixels stay zero.  Returns (features + opacity [H,W,25], dist [H,W,1], hits [H,W,1]) in that dtype."""
+    dt, dev = pos.dtype, pos.device
+    o_w, d_w = world_rays(cam_inv, ro, rd, dt, dev)
+    tiles = range(ranges.shape[0]) if tiles is None else tiles
+    out = [render_tile(cfg, o_w, d_w, width, height, pos, dns, quat, scl, feats, sorted_values, ranges, int(t)) for t in tiles]
     P = width * height
-    out = [None] * ranges.shape[0]
-    for tile in range(ranges.shape[0]):
-        b, e = (int(v) for v in ranges[tile])
-        tx, ty = tile % gx, tile // gx
-        ys, xs = np.meshgrid(np.arange(ty * 16, min(height, ty * 16 + 16)), np.arange(tx * 16, min(width, tx * 16 + 16)), indexing="ij")
-        pix = torch.as_tensor((ys * width + xs).reshape(-1), device=dev)
-        o, d = o_w[pix], d_w[pix]
-        m = len(pix)
-        T = torch.ones(m, dtype=F64, device=dev)
-        alive = torch.ones(m, dtype=torch.bool, device=dev)
-        Fe = torch.zeros((m, NHT_OUT), dtype=F64, device=dev)
-        D = torch.zeros(m, dtype=F64, device=dev)
-        H = torch.zeros(m, dtype=F64, device=dev)
-        for k in range(b, e):
-            i = int(sorted_values[k])
-            R = rot_rows(quat[i])
-            gro = ((o - pos[i]) @ R.T) / scl[i]
-            grdu = (d @ R.T) / scl[i]
-            grd = grdu / grdu.norm(dim=1, keepdim=True)
-            gray = torch.linalg.cross(grd, gro).pow(2).sum(1)
-            gres = torch.exp(-0.0555555555556 * gray * gray) if deg4 else torch.exp(-0.5 * gray)
-            alpha = torch.clamp(gres * dns[i], max=float(cfg.max_alpha))
-            pd = -(grd * gro).sum(1, keepdim=True)
-            t = (scl[i] * grd * pd).norm(dim=1)
-            acc = alive & (gres > float(cfg.min_kernel_density)) & (alpha > float(cfg.min_alpha)) & (t > 0)
-            if not bool(acc.any()):
-                continue
-            w = torch.where(acc, alpha * T, torch.zeros_like(T))
-            Fe = Fe + w[:, None] * features_at(gro + grd * pd, feats[i])
-            D = D + w * t
-            H = H + (acc & (w > 0)).to(F64)
-            T = torch.where(acc, T * (1 - alpha), T)
-            alive = alive & ~(T < float(cfg.min_transmittance))
-        out[tile] = (pix, torch.cat([Fe, (1 - T)[:, None]], 1), D, H)
-    img = torch.zeros((P, NHT_OUT + 1), dtype=F64, device=dev)
-    dist = torch.zeros(P, dtype=F64, device=dev)
-    hits = torch.zeros(P, dtype=F64, device=dev)
-    pix = torch.cat([t[0] for t in out])
-    img = img.index_put((pix,), torch.cat([t[1] for t in out]))
-    dist = dist.index_put((pix,), torch.cat([t[2] for t in out]))
-    hits = hits.index_put((pix,), torch.cat([t[3] for t in out]))
+    pix = torch.cat([r[0] for r in out]) if out else torch.zeros(0, dtype=torch.long, device=dev)
+    cat = lambda j, shape: torch.cat([r[j] for r in out]) if out else torch.zeros(shape, dtype=dt, device=dev)  # noqa: E731
+    img = torch.zeros((P, NHT_OUT + 1), dtype=dt, device=dev).index_put((pix,), cat(1, (0, NHT_OUT + 1)))
+    dist = torch.zeros(P, dtype=dt, device=dev).index_put((pix,), cat(2, (0,)))
+    hits = torch.zeros(P, dtype=dt, device=dev).index_put((pix,), cat(3, (0,)))
     return img.reshape(height, width, NHT_OUT + 1), dist.reshape(height, width, 1), hits.reshape(height, width, 1)
 
 
-def leaves(particles: np.ndarray, feats: np.ndarray, device="cpu", requires_grad=True):
-    """float64 leaf tensors (pos, dns, quat, scl, feats) of a [N,12] particle record and [N,48] features."""
-    p = torch.as_tensor(np.asarray(particles, np.float32), device=device).to(F64)
-    ts = [p[:, 0:3], p[:, 3], p[:, 4:8], p[:, 8:11], torch.as_tensor(np.asarray(feats, np.float32), device=device).to(F64)]
+def leaves(particles: np.ndarray, feats: np.ndarray, device="cpu", requires_grad=True, dtype=F64):
+    """Leaf tensors (pos, dns, quat, scl, feats) of a [N,12] particle record and [N,48] features, in `dtype`."""
+    p = torch.as_tensor(np.asarray(particles, np.float32), device=device).to(dtype)
+    ts = [p[:, 0:3], p[:, 3], p[:, 4:8], p[:, 8:11], torch.as_tensor(np.asarray(feats, np.float32), device=device).to(dtype)]
     return [t.clone().requires_grad_(requires_grad) for t in ts]
 
 
-def frame(cfg, cam, sc_particles, feats, ro, rd, go, d_out=None, d_dist=None, device="cpu"):
-    """Forward (and with d_out / d_dist, the backward by autograd) of one frame over the C oracle's lists.  Returns a dict of numpy
-    arrays: out, dist, hits and, with gradients, dp [N,12] (pos, density, quat, scale, 0) and df [N,48]."""
+def frame(cfg, cam, sc_particles, feats, ro, rd, go, d_out=None, d_dist=None, device="cpu", tiles=None, dtype=F64, pr=None, bn=None):
+    """Forward (and with d_out / d_dist, the backward by autograd) of one frame over the C oracle's lists (or the given pr / bn).
+    tiles: the tiles to render (default all); with gradients, those outside them must be zero there to mean the full frame's backward.
+    The backward runs tile by tile, so the autograd graph of one tile is alive at a time.  Returns a dict of numpy arrays (float64):
+    out, dist, hits, longest (the longest composited list of a pixel), clamped (composited pairs with alpha clamped) and, with gradients, dp [N,12] (pos, density,
+    quat, scale, 0) and df [N,48]."""
     n = sc_particles.shape[0]
-    pr = go.project(cfg, cam, sc_particles, np.zeros((n, 48), np.float32), 0)
-    bn = go.bin_tiles(cfg, cam, pr)
+    if pr is None:
+        pr = go.project(cfg, cam, sc_particles, np.zeros((n, 48), np.float32), 0)
+        bn = go.bin_tiles(cfg, cam, pr)
     _, inv, _ = go.sensor_matrices(cam)
-    pos, dns, quat, scl, ft = leaves(sc_particles, feats, device, requires_grad=d_out is not None)
-    img, dist, hits = render(cfg, inv, cam.width, cam.height, ro, rd, pos, dns, quat, scl, ft, bn.sorted_values, bn.ranges)
-    res = dict(out=img.detach().cpu().numpy(), dist=dist.detach().cpu().numpy(), hits=hits.detach().cpu().numpy(), pr=pr, bn=bn)
-    if d_out is not None:
-        loss = (img * torch.as_tensor(d_out, dtype=F64, device=device)).sum() + (dist * torch.as_tensor(d_dist, dtype=F64, device=device)).sum()
-        gp, gd, gq, gs, gf = torch.autograd.grad(loss, [pos, dns, quat, scl, ft], allow_unused=True)
-        z = lambda g, shape: torch.zeros(shape, dtype=F64, device=device) if g is None else g  # noqa: E731
-        dp = torch.cat([z(gp, (n, 3)), z(gd, (n,))[:, None], z(gq, (n, 4)), z(gs, (n, 3)), torch.zeros((n, 1), dtype=F64, device=device)], 1)
-        res.update(dp=dp.cpu().numpy(), df=z(gf, (n, 48)).cpu().numpy())
+    W, H = cam.width, cam.height
+    grads = d_out is not None
+    lv = leaves(sc_particles, feats, device, requires_grad=grads, dtype=dtype)
+    o_w, d_w = world_rays(inv, ro, rd, dtype, device)
+    if grads:
+        g_out = torch.as_tensor(np.asarray(d_out).reshape(W * H, NHT_OUT + 1), dtype=dtype, device=device)
+        g_dist = torch.as_tensor(np.asarray(d_dist).reshape(W * H), dtype=dtype, device=device)
+        acc = [torch.zeros_like(t) for t in lv]
+    img = np.zeros((W * H, NHT_OUT + 1))
+    dist, hits = np.zeros(W * H), np.zeros(W * H)
+    longest = clamped = 0
+    for t in (range(bn.ranges.shape[0]) if tiles is None else tiles):
+        pix, o, dd, hh, K, nc = render_tile(cfg, o_w, d_w, W, H, *lv, bn.sorted_values, bn.ranges, int(t))
+        longest, clamped = max(longest, K), clamped + nc
+        p = pix.cpu().numpy()
+        img[p], dist[p], hits[p] = o.detach().cpu().double().numpy(), dd.detach().cpu().double().numpy(), hh.cpu().double().numpy()
+        if grads and o.requires_grad:
+            loss = (o * g_out[pix]).sum() + (dd * g_dist[pix]).sum()
+            for a, g in zip(acc, torch.autograd.grad(loss, lv, allow_unused=True)):
+                if g is not None:
+                    a += g
+    res = dict(out=img.reshape(H, W, NHT_OUT + 1), dist=dist.reshape(H, W, 1), hits=hits.reshape(H, W, 1), longest=longest, clamped=clamped,
+               pr=pr, bn=bn)
+    if grads:
+        gp, gd, gq, gs, gf = (a.detach().cpu().double() for a in acc)
+        dp = torch.cat([gp, gd[:, None], gq, gs, torch.zeros((n, 1), dtype=torch.float64)], 1)
+        res.update(dp=dp.numpy(), df=gf.numpy())
     return res

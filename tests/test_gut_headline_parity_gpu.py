@@ -22,7 +22,7 @@ import numpy as np
 import pytest
 
 import scenes
-from helpers import image_error_report, oracle_frame, rel_l2, tracer_pose
+from helpers import dist_grad_blocks, image_error_report, oracle_frame, rel_l2, tracer_pose
 
 pytestmark = pytest.mark.gpu
 
@@ -41,15 +41,19 @@ def _native_camera(sc, pose):
     return cam
 
 
-def _check_frame(label, sc, cam_index, n_cams, seed):
+def _check_frame(label, sc, cam_index, n_cams, seed, d_dist="random", d_alpha="random"):
+    """d_dist / d_alpha: the output gradients of the backward (helpers.output_grads); "zero" d_dist is what every training step passes."""
     import b200_native as nat
 
     c2w = sc.camera(cam_index, n_cams)
     pose = tracer_pose(c2w)
-    ref = oracle_frame(sc, c2w, seed=seed, pose=pose, with_f64=True)
+    ref = oracle_frame(sc, c2w, seed=seed, pose=pose, with_f64=True, d_dist=d_dist, d_alpha=d_alpha)
     lens = ref["bn"].ranges[:, 1].astype(np.int64) - ref["bn"].ranges[:, 0]
+    if d_dist != "random" or d_alpha != "random":
+        label = f"{label} d_dist={d_dist} d_alpha={d_alpha}"
     print(f"[headline] {label} cam{cam_index}: N={sc.n} I={len(ref['bn'].sorted_keys)} longest tile list {int(lens.max())} "
-          f"(batches of 256: {int(np.ceil(lens.max() / 256))}), hits {int(ref['hits'].sum())}")
+          f"(batches of 256: {int(np.ceil(lens.max() / 256))}), hits {int(ref['hits'].sum())}, warp blocks with / without a distance "
+          f"gradient {dist_grad_blocks(ref['d_dist'])}")
     assert lens.max() > 512, "the case is meant to exercise several staged batches per tile"
 
     ctx = nat.Context(nat.default_config(), 0)
@@ -109,16 +113,27 @@ def _check_frame(label, sc, cam_index, n_cams, seed):
     ctx.close()
 
 
-@pytest.mark.parametrize("cam_index", [3, 41])
-def test_c2_full_scale_oracle_parity(cam_index):
-    """BASELINE configs[1]: the bench workload itself (scenes.scene_c2(): 300k Gaussians, 800x800), two of its 100 orbit cameras."""
-    _check_frame("c2", scenes.scene_c2(), cam_index, 100, seed=cam_index)
+@pytest.mark.parametrize("cam_index,d_dist,d_alpha", [
+    pytest.param(3, "random", "random", id="3"), pytest.param(41, "random", "random", id="41"),
+    pytest.param(3, "zero", "random", id="3-zero_d_dist"), pytest.param(3, "zero", "zero", id="3-zero_d_dist-zero_d_alpha"),
+    pytest.param(41, "mixed", "random", id="41-mixed_d_dist")])
+def test_c2_full_scale_oracle_parity(cam_index, d_dist, d_alpha):
+    """BASELINE configs[1]: the bench workload itself (scenes.scene_c2(): 300k Gaussians, 800x800), two of its 100 orbit cameras.
+    zero d_dist: the backward as training runs it (each warp skips the depth branch: the closed-form normalize adjoint, 4 flushed
+    gradient columns), with zero d_alpha as well for an image loss on a black background; mixed: warps with and without the depth branch
+    in one frame (helpers.dist_grad_mask)."""
+    _check_frame("c2", scenes.scene_c2(), cam_index, 100, seed=cam_index, d_dist=d_dist, d_alpha=d_alpha)
 
 
 def test_c3_like_oracle_parity():
     """C3-like unbounded scene (70 % within radius 3, background to radius 50, particles partly behind the camera) at the C3 resolution
     1237x822 (ragged: 78 x 52 tiles, partial tiles on both edges) with 400k Gaussians: tile lists beyond 1000 entries."""
     _check_frame("c3_small", scenes.scene_c3(n=400_000), 1, 10, seed=11)
+
+
+def test_c3_like_oracle_parity_without_distance_gradient():
+    """The C3-like frame above with the backward as training runs it: d_dist = 0 on every pixel."""
+    _check_frame("c3_small", scenes.scene_c3(n=400_000), 1, 10, seed=11, d_dist="zero")
 
 
 def _dense(model):

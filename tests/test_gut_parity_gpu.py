@@ -93,8 +93,9 @@ def _run(sc, c2w, ref):
     dbg = {k: ctx.debug_copy(v) for k, v in dict(count=nat.DBG_TILES_COUNT, keys=nat.DBG_SORTED_KEYS, vals=nat.DBG_SORTED_VALUES,
                                                  ranges=nat.DBG_TILE_RANGES, depth=nat.DBG_DEPTH, rgb=nat.DBG_RGB).items()}
     loss = (out["pred_features"] * torch.from_numpy(ref["d_rgba"][None, ..., :3]).to(dev)).sum() \
-        + (out["pred_opacity"] * torch.from_numpy(ref["d_rgba"][None, ..., 3:]).to(dev)).sum() \
-        + (out["pred_dist"] * torch.from_numpy(ref["d_dist"][None]).to(dev)).sum()
+        + (out["pred_opacity"] * torch.from_numpy(ref["d_rgba"][None, ..., 3:]).to(dev)).sum()
+    if np.any(ref["d_dist"]):  # else a loss that never reads pred_dist, as in training: autograd hands the tracer no distance gradient
+        loss = loss + (out["pred_dist"] * torch.from_numpy(ref["d_dist"][None]).to(dev)).sum()
     loss.backward()
     torch.cuda.synchronize()
     return tr, g, out, dbg
@@ -116,12 +117,19 @@ def test_c1_integer_artifacts_bit_exact(cam_index, bands, size):
     assert np.allclose(dbg["rgb"][vis], ref["pr"].rgb[vis], atol=2e-6, rtol=1e-6)
 
 
-@pytest.mark.parametrize("cam_index,size", [(0, (128, 128)), (3, (128, 128)), (7, (128, 128)), (5, (75, 53))])
-def test_c1_forward_and_gradients(cam_index, size):
-    """size (75, 53): ragged image -- partial tiles and partially filled warps in the render kernels and their culling."""
+C1_FRAMES = [(0, (128, 128)), (3, (128, 128)), (7, (128, 128)), (5, (75, 53))]
+
+
+@pytest.mark.parametrize("cam_index,size,d_dist", [pytest.param(c, s, "random", id=f"{c}-size{i}") for i, (c, s) in enumerate(C1_FRAMES)]
+                         + [pytest.param(c, s, m, id=f"{c}-size{i}-{m}_d_dist") for m in ("zero", "mixed") for i, (c, s) in enumerate(C1_FRAMES)
+                            if i in (1, 3)])
+def test_c1_forward_and_gradients(cam_index, size, d_dist):
+    """size (75, 53): ragged image -- partial tiles and partially filled warps in the render kernels and their culling.  d_dist "zero":
+    Tracer.render + autograd with a loss that never reads pred_dist (the backward as training runs it: no warp takes the depth branch);
+    "mixed": warps with and without it in one frame (helpers.dist_grad_mask)."""
     sc = scenes.scene_c1(width=size[0], height=size[1])
     c2w = sc.camera(cam_index, 10)
-    ref = oracle_frame(sc, c2w, seed=cam_index, pose=tracer_pose(c2w))
+    ref = oracle_frame(sc, c2w, seed=cam_index, pose=tracer_pose(c2w), d_dist=d_dist)
     tr, g, out, _ = _run(sc, c2w, ref)
     rgba = torch.cat([out["pred_features"], out["pred_opacity"]], -1)[0].detach().cpu().numpy()
     dist = out["pred_dist"][0].detach().cpu().numpy()
@@ -137,7 +145,7 @@ def test_c1_forward_and_gradients(cam_index, size):
     errs = dict(pos=rel_l2(g.positions.grad.cpu().numpy(), dp[:, 0:3]), dns=rel_l2(g._dns.grad.cpu().numpy(), dp[:, 3:4]),
                 quat=rel_l2(g._rot.grad.cpu().numpy(), dp[:, 4:8]), scl=rel_l2(g._scl.grad.cpu().numpy(), dp[:, 8:11]),
                 sph=rel_l2(g._sph.grad.cpu().numpy(), ref["ds"]))
-    print("[parity] c1 cam%d gradient rel-L2:" % cam_index, {k: f"{v:.2e}" for k, v in errs.items()})
+    print(f"[parity] c1 cam{cam_index} d_dist={d_dist} gradient rel-L2:", {k: f"{v:.2e}" for k, v in errs.items()})
     assert max(errs.values()) <= 1e-3
     t = tr.timings
     assert "forward_render" in t or "backward_render" in t
@@ -525,7 +533,19 @@ def test_backward_rejects_a_camera_other_than_the_forwards():
 
 def test_compact_exchange_rebuilds_the_sh_gradient():
     """View-parallel exchange (gutb200_backward_compact + gutb200_sph_grad_from_views): the SH gradient rebuilt from the [N,4]
-    radiance gradients of two views equals the sum of the two views' full [N,48] gradients, and d_particles is unchanged."""
+    radiance gradients of two views equals the sum of the two views' full [N,48] gradients, and d_particles is unchanged.  The output
+    gradients are the oracle's (helpers.oracle_frame), so both backwards are compared with it too."""
+    _compact_exchange("random")
+
+
+@pytest.mark.parametrize("d_dist", ["zero", "mixed"])
+def test_compact_exchange_without_distance_gradient(d_dist):
+    """The exchange above with d_dist "zero" (what GaussianTrainStep passes: no warp of the backward takes the depth branch) and "mixed"
+    (warps with and without it in one frame, helpers.dist_grad_mask)."""
+    _compact_exchange(d_dist)
+
+
+def _compact_exchange(d_dist):
     import threedgut_tracer
     from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
@@ -539,19 +559,24 @@ def test_compact_exchange_rebuilds_the_sh_gradient():
     sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
                                                     np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
                                                     np.zeros(4, np.float32))
-    gen = torch.Generator(device=dev).manual_seed(7)
-    full_dp, full_ds, gs, pos = [], [], [], []
+    full_dp, full_ds, gs, pos, ref_ds = [], [], [], [], []
     for view in (2, 7):
         pose = scenes.pose7_from_c2w(sc.camera(view, 10))
-        d_rgba = torch.randn((H, W, 4), device=dev, generator=gen)
-        d_dist = 0.05 * torch.randn((H, W, 1), device=dev, generator=gen)
+        ref = oracle_frame(sc, sc.camera(view, 10), seed=view, pose=pose, d_dist=d_dist)
+        d_rgba = torch.from_numpy(ref["d_rgba"]).to(dev)
+        d_dist_t = torch.from_numpy(ref["d_dist"]).to(dev)
         rgba, dst, hits, vis = raster.trace(0, 3, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
-        dp, ds = raster.trace_bwd(0, 3, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst, d_dist)
+        dp, ds = raster.trace_bwd(0, 3, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst, d_dist_t)
+        errs = dict(d_particles=rel_l2(dp.cpu().numpy(), ref["dp"]), d_sph=rel_l2(ds.cpu().numpy(), ref["ds"]))
+        print(f"[parity] compact exchange d_dist={d_dist} view {view}: full backward vs oracle", {k: f"{v:.2e}" for k, v in errs.items()})
+        assert max(errs.values()) <= 1e-3, errs
         full_dp.append(dp.clone())
         full_ds.append(ds.clone())
+        ref_ds.append(ref["ds"].astype(np.float64))
         rgba, dst, hits, vis = raster.trace(0, 3, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
-        dp2, g = raster.trace_bwd_compact(0, 3, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst, d_dist)
+        dp2, g = raster.trace_bwd_compact(0, 3, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst, d_dist_t)
         assert rel_l2(dp2.cpu().numpy(), dp.cpu().numpy()) <= 2e-5  # atomics order only (through the per-particle maps of G8)
+        assert rel_l2(dp2.cpu().numpy(), ref["dp"]) <= 1e-3
         gs.append(g.clone())
         pos.append(raster.sensor_position(sensor, pose, pose, W, H))
     assert np.allclose(pos[0], np.asarray(sc.camera(2, 10))[:3, 3], atol=1e-5)
@@ -559,6 +584,7 @@ def test_compact_exchange_rebuilds_the_sh_gradient():
     rebuilt = raster.sph_grad_from_views(3, particles, np.stack(pos), torch.stack(gs)).cpu().numpy()
     assert np.abs(ds_sum).max() > 0
     assert rel_l2(rebuilt, ds_sum) <= 2e-6
+    assert rel_l2(rebuilt, ref_ds[0] + ref_ds[1]) <= 1e-3
     assert np.abs(rebuilt - ds_sum).max() <= 1e-5 * max(1.0, float(np.abs(ds_sum).max()))
     # a single view reproduces that view's rows (no summation: bit pattern of basis x g)
     one = raster.sph_grad_from_views(3, particles, pos[1][None], gs[1][None]).cpu().numpy()

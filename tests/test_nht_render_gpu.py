@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import scenes
-from helpers import image_error_report, rel_l2
+from helpers import dist_grad_blocks, dist_grad_mask, image_error_report, rel_l2
 from oracle import gut_oracle as go
 
 pytestmark = pytest.mark.gpu
@@ -85,10 +85,14 @@ class _Gpu:
         return dp.cpu().numpy(), df.cpu().numpy()
 
 
-def _check_frame(tag, sc, cfg, cam, feats, g, ro, rd, seed=1):
+def _check_frame(tag, sc, cfg, cam, feats, g, ro, rd, seed=1, d_dist_mode="random"):
+    """d_dist_mode: helpers.dist_grad_mask ("zero" is what training passes: no warp of the backward takes the depth branch)."""
     rng = np.random.default_rng(seed)
     d_out = rng.normal(size=(sc.height, sc.width, 25)).astype(np.float32)
     d_dist = (0.1 * rng.normal(size=(sc.height, sc.width, 1))).astype(np.float32)
+    d_dist *= dist_grad_mask(sc.height, sc.width, d_dist_mode, seed)[..., None]
+    if d_dist_mode != "random":
+        tag = f"{tag} d_dist={d_dist_mode} (warp blocks with / without a distance gradient {dist_grad_blocks(d_dist)})"
     ref = nro.frame(cfg, cam, sc.particles, feats, ro, rd, go, d_out=d_out, d_dist=d_dist, device="cuda")
     g.forward()
     out, dist, hits = g.out.cpu().numpy(), g.dist.cpu().numpy(), g.hits.cpu().numpy()
@@ -107,14 +111,16 @@ def _check_frame(tag, sc, cfg, cam, feats, g, ro, rd, seed=1):
 
 
 FRAMES = [("c1", 0, 2, False), ("c1", 3, 4, True), ("odd", 0, 4, False), ("odd", 3, 2, True), ("dense", 0, 2, False), ("dense", 3, 4, True)]
+CASES = [pytest.param(*f, "random", id="-".join(map(str, f))) for f in FRAMES] \
+    + [pytest.param(*f, m, id="-".join(map(str, f)) + f"-{m}_d_dist") for m in ("zero", "mixed") for f in FRAMES]
 
 
-@pytest.mark.parametrize("name,cam_i,deg,half", FRAMES)
-def test_nht_matches_the_f64_oracle(name, cam_i, deg, half):
+@pytest.mark.parametrize("name,cam_i,deg,half,d_dist", CASES)
+def test_nht_matches_the_f64_oracle(name, cam_i, deg, half, d_dist):
     sc, cfg, cam, feats = _setup(name, cam_i, deg, half)
     ro, rd = sc.rays()
     g = _Gpu(sc, deg, cam, feats, half)
-    ref = _check_frame(f"{name} cam{cam_i} deg{deg} {'fp16' if half else 'fp32'}", sc, cfg, cam, feats, g, ro, rd)
+    ref = _check_frame(f"{name} cam{cam_i} deg{deg} {'fp16' if half else 'fp32'}", sc, cfg, cam, feats, g, ro, rd, d_dist_mode=d_dist)
     if name == "dense":
         assert np.diff(ref["bn"].ranges.astype(np.int64), axis=1).max() > 256
 

@@ -59,9 +59,21 @@ def _scene(seed=20, n=90, w=48, h=40):
     return sc, cam, feats
 
 
-def test_alpha_dist_hits_equal_the_sh_forward_in_f64():
-    sc, cam, feats = _scene()
+# render settings off the default the pins run at as well: earlier termination, and the *_3dgut_mcmc_nht configs' sigma-point spread
+# (ut_delta follows ut_alpha as threedgut_tracer._native_config sets it)
+SETTINGS = {"min_transmittance=0.03": dict(min_transmittance=0.03), "ut_alpha=0.1": dict(ut_alpha=0.1, ut_delta=math.sqrt(0.03))}
+
+
+def _config(settings=None):
     cfg = go.default_config()
+    for k, v in (settings or {}).items():
+        setattr(cfg, k, v)
+    return cfg
+
+
+def _alpha_dist_hits(settings=None):
+    sc, cam, feats = _scene()
+    cfg = _config(settings)
     ro, rd = sc.rays()
     fr = nro.frame(cfg, cam, sc.particles, feats, ro, rd, go)
     assert fr["bn"].sorted_values.size > 200
@@ -69,13 +81,18 @@ def test_alpha_dist_hits_equal_the_sh_forward_in_f64():
     assert np.abs(fr["out"][..., 24] - rgba[..., 3]).max() < 1e-6
     assert np.abs(fr["dist"] - dist).max() < 1e-5 * max(1.0, np.abs(dist).max())
     assert np.array_equal(fr["hits"], hits)
+    return fr
 
 
-def test_density_adjoint_equals_the_sh_adjoint_with_a_zero_rgb_gradient():
+def test_alpha_dist_hits_equal_the_sh_forward_in_f64():
+    _alpha_dist_hits()
+
+
+def _sh_adjoint(settings=None):
     """d_features = 0 on an unclamped scene: the NHT adjoint of alpha and distance is the SH path's, which the C oracle pins."""
     sc, cam, feats = _scene(seed=21)
     assert sc.particles[:, 3].max() < 0.99  # alpha = response * density never reaches the clamp
-    cfg = go.default_config()
+    cfg = _config(settings)
     ro, rd = sc.rays()
     rng = np.random.default_rng(5)
     h, w = sc.height, sc.width
@@ -95,10 +112,14 @@ def test_density_adjoint_equals_the_sh_adjoint_with_a_zero_rgb_gradient():
     assert np.abs(fr["df"]).max() == 0.0
 
 
-def test_autograd_matches_central_differences_including_a_clamped_pair():
+def test_density_adjoint_equals_the_sh_adjoint_with_a_zero_rgb_gradient():
+    _sh_adjoint()
+
+
+def _central_differences(settings=None):
     sc, cam, feats = _scene(seed=22, n=40, w=32, h=32)
     particles = sc.particles.copy()
-    cfg = go.default_config()
+    cfg = _config(settings)
     ro, rd = sc.rays()
     fr0 = nro.frame(cfg, cam, particles, feats, ro, rd, go)
     # the particle with the most hits gets a density high enough to clamp alpha at 0.99 in its centre
@@ -143,6 +164,61 @@ def test_autograd_matches_central_differences_including_a_clamped_pair():
             assert abs(fd - fr["df"][i, col]) <= 1e-5 * max(1.0, abs(fd)), (i, col, fd, fr["df"][i, col])
             checked += 1
     assert checked == 36
+
+
+def test_autograd_matches_central_differences_including_a_clamped_pair():
+    _central_differences()
+
+
+@pytest.mark.parametrize("setting", list(SETTINGS))
+def test_oracle_pins_at_other_render_settings(setting):
+    """The three pins above at min_transmittance = 0.03 and at ut_alpha = 0.1: the f64 forward against the C oracle, the SH-adjoint
+    equality, and central differences including a clamped pair."""
+    fr = _alpha_dist_hits(SETTINGS[setting])
+    sc, cam, feats = _scene()
+    base = nro.frame(go.default_config(), cam, sc.particles, feats, *sc.rays(), go)
+    if setting.startswith("min_t"):  # rays stop earlier: fewer composited hits
+        assert fr["hits"].sum() < base["hits"].sum()
+    else:  # the smaller sigma-point spread changes the lists
+        assert not np.array_equal(fr["bn"].ranges, base["bn"].ranges)
+    _sh_adjoint(SETTINGS[setting])
+    _central_differences(SETTINGS[setting])
+
+
+def test_tile_subset_backward_is_the_masked_full_frame_backward():
+    """The sampling premise of tests/test_nht_render_headline_gpu.py: with output gradients zero outside a set of tiles, the backward of
+    the whole frame (one autograd graph over every tile) equals the tile-subset oracle's, and the subset's forward is the full frame's
+    at its pixels.  Tiles are independent: each pixel composites its own tile's list only."""
+    sc, cam, feats = _scene(seed=23, n=300, w=75, h=53)  # ragged: 5 x 4 tiles, partial on both edges
+    particles = sc.particles.copy()
+    particles[::7, 3] = 3.0  # clamped pairs
+    cfg = _config(SETTINGS["ut_alpha=0.1"])
+    ro, rd = sc.rays()
+    n_tiles = ((sc.width + 15) // 16) * ((sc.height + 15) // 16)
+    tiles = [0, 4, 7, 18, 19]
+    mask = np.zeros(sc.width * sc.height, bool)
+    for t in tiles:
+        mask[nro.tile_pixels(t, sc.width, sc.height)] = True
+    mask = mask.reshape(sc.height, sc.width, 1)
+    rng = np.random.default_rng(4)
+    d_out = rng.normal(size=(sc.height, sc.width, 25)) * mask
+    d_dist = 0.1 * rng.normal(size=(sc.height, sc.width, 1)) * mask
+    part = nro.frame(cfg, cam, particles, feats, ro, rd, go, d_out=d_out, d_dist=d_dist, tiles=tiles)
+    assert part["hits"][mask[..., 0]].sum() > 4 * mask.sum() and np.all(part["hits"][~mask[..., 0]] == 0)
+    _, inv, _ = go.sensor_matrices(cam)
+    lv = nro.leaves(particles, feats)
+    img, dist, hits = nro.render(cfg, inv, cam.width, cam.height, ro, rd, *lv, part["bn"].sorted_values, part["bn"].ranges)
+    assert part["bn"].ranges.shape[0] == n_tiles
+    for name, a, b in (("out", img, part["out"]), ("dist", dist, part["dist"]), ("hits", hits, part["hits"])):
+        assert np.array_equal(a.detach().numpy()[mask[..., 0]], b[mask[..., 0]]), name
+    loss = (img * torch.tensor(d_out)).sum() + (dist * torch.tensor(d_dist)).sum()
+    gp, gd, gq, gs, gf = torch.autograd.grad(loss, lv)
+    full_dp = torch.cat([gp, gd[:, None], gq, gs, torch.zeros((sc.n, 1), dtype=torch.float64)], 1).numpy()
+    assert np.abs(part["dp"]).max() > 0 and np.abs(part["df"]).max() > 0 and part["clamped"] > 0
+    for name, a, b in (("d_particles", full_dp, part["dp"]), ("d_features", gf.numpy(), part["df"])):
+        err = rel_l2(b, a)
+        print(f"[sample] NHT {name}: tile subset vs masked full frame rel-L2 {err:.2e}")
+        assert err <= 1e-12, name
 
 
 @pytest.mark.parametrize("key,value", [
