@@ -92,6 +92,7 @@ SIGNATURES = {
     "gutb200_image_loss": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
     "gutb200_image_loss_rgb": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
     "gutb200_image_loss_composited": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp]),
+    "gutb200_image_loss_postprocessed": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp, _i32]),
     "gutb200_hybrid_rays": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_hybrid_composite": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp]),
     "gutb200_hybrid_composite_bwd": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),

@@ -323,6 +323,15 @@ void drain_timers(gutb200_ctx* c) {
 
 }  // namespace
 
+namespace gutb200 {
+
+// The message of the last failed call that takes no context (gutb200_image_loss_postprocessed), per host thread.
+static thread_local std::string g_context_free_error;
+
+void set_context_free_error(const std::string& msg) { g_context_free_error = msg; }
+
+}  // namespace gutb200
+
 extern "C" {
 
 const char* gutb200_version(void) { return "3dgrut_b200 0.1 (sm_90a)"; }
@@ -389,7 +398,10 @@ void gutb200_destroy(gutb200_ctx* c) {
     delete c;
 }
 
-const char* gutb200_last_error(const gutb200_ctx* c) { return c ? c->error.c_str() : "null context"; }
+const char* gutb200_last_error(const gutb200_ctx* c) {
+    if (c) return c->error.c_str();
+    return gutb200::g_context_free_error.empty() ? "null context" : gutb200::g_context_free_error.c_str();
+}
 
 int64_t gutb200_launch_count(const gutb200_ctx* c) { return c ? c->launches : 0; }
 

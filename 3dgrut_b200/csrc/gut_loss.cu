@@ -20,12 +20,23 @@
 //     x = (rgb + bg (1 - alpha)) m,  y = target m          bg: constant colour or [H,W,3] image; m: optional [H,W] mask
 //     d rgb_c = m dL/dx_c,  d alpha = -sum_c bg_c m dL/dx_c
 // The background mode (BG) and the mask (MASK) are template parameters beside the strides; BG = 0 (black) with no mask is the plain loss.
+//
+// gutb200_image_loss_postprocessed adds the reference's `post_processing.method: linear-to-srgb` (threedgrut/utils/
+// post_processing_linear_to_srgb.py, applied after the background and before the loss, trainer.py:1165-1172) as a third template
+// parameter, POST (0 none, 1 linear-to-sRGB), between the composite and the mask:
+//     x = s(c) m,  c = rgb + bg (1 - alpha),   s(c) = 1.055 max(c, 1e-8)^(1/2.4) - 0.055 if c > 0.0031308, else 12.92 c   (no clamp: HDR)
+//     d rgb_c = m s'(c_c) dL/dx_c,  d alpha = -sum_c bg_c m s'(c_c) dL/dx_c
+// POST = 0 compiles every existing instantiation to the code it had without this parameter.
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <string>
 
 #include "../../include/gut_b200.h"
 
 namespace gutb200 {
+
+void set_context_free_error(const std::string& msg);  // gut_api.cu: the message gutb200_last_error(NULL) returns
 
 namespace {
 
@@ -49,17 +60,38 @@ struct Composite {
     float bg[3];            // constant background (BG == 1)
 };
 
-// x and y of pixel p, channel c, as the loss sees them: the prediction composited onto the background, both multiplied by the mask.
-template <int PS, int BG, bool MASK>
-__device__ __forceinline__ void load_xy(const float* __restrict__ pred, const float* __restrict__ target, const Composite& cp, int64_t p, int c,
-                                        float& x, float& y) {
-    x = pred[p * PS + c];
-    y = target[p * 3 + c];
+constexpr float kSrgbLimit = 0.0031308f, kSrgbExp = 1.0f / 2.4f;
+
+// linear-to-sRGB (post_processing_linear_to_srgb.py:43-67): the branch is taken on c itself, the power on max(c, 1e-8)
+__device__ __forceinline__ float linear_to_srgb(float c) {
+    return c > kSrgbLimit ? 1.055f * powf(fmaxf(c, 1e-8f), kSrgbExp) - 0.055f : 12.92f * c;
+}
+
+// its derivative through the branch taken (torch.where): (1.055 / 2.4) c^(1/2.4 - 1) above the limit, 12.92 below
+__device__ __forceinline__ float linear_to_srgb_slope(float c) {
+    return c > kSrgbLimit ? (1.055f / 2.4f) * powf(c, kSrgbExp - 1.0f) : 12.92f;
+}
+
+// x = the prediction of pixel p, channel c, composited onto the background (before any post-processing and the mask).
+template <int PS, int BG>
+__device__ __forceinline__ float composite(float x, const float* __restrict__ pred, const Composite& cp, int64_t p, int c) {
     if constexpr (BG != 0) {
         const float a = PS == 4 ? pred[p * 4 + 3] : cp.alpha[p];
         const float b = BG == 1 ? cp.bg[c] : cp.bg_image[p * 3 + c];
         x = x + b * (1.0f - a);
     }
+    return x;
+}
+
+// x and y of pixel p, channel c, as the loss sees them: the prediction composited onto the background and post-processed (POST), both
+// multiplied by the mask.
+template <int PS, int BG, bool MASK, int POST = 0>
+__device__ __forceinline__ void load_xy(const float* __restrict__ pred, const float* __restrict__ target, const Composite& cp, int64_t p, int c,
+                                        float& x, float& y) {
+    x = pred[p * PS + c];
+    y = target[p * 3 + c];
+    x = composite<PS, BG>(x, pred, cp, p, c);
+    if constexpr (POST == 1) x = linear_to_srgb(x);
     if constexpr (MASK) {
         const float m = cp.mask[p];
         x = x * m;
@@ -84,7 +116,7 @@ __device__ __forceinline__ float block_sum(float v, float* scratch) {
 }
 
 // PS: floats per pixel of the prediction (4: the 3DGUT [H,W,4] image, 3: the 3DGRT rgb [H,W,3]); only the loads depend on it.
-template <int PS, int BG = 0, bool MASK = false>
+template <int PS, int BG = 0, bool MASK = false, int POST = 0>
 __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
                                                              Composite cp, Window win, float g_scale /* -lambda_ssim / count */,
                                                              float* __restrict__ dmaps,
@@ -105,7 +137,7 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
             const bool in = (gx >= 0) && (gy >= 0) && (gx < W) && (gy < H);
             const int64_t p = static_cast<int64_t>(gy) * W + gx;
             float xv = 0.f, yv = 0.f;
-            if (in) load_xy<PS, BG, MASK>(pred_rgba, target, cp, p, c, xv, yv);
+            if (in) load_xy<PS, BG, MASK, POST>(pred_rgba, target, cp, p, c, xv, yv);
             sx[ly][lx] = xv;
             sy[ly][lx] = yv;
         }
@@ -149,7 +181,7 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
     const float l1_block = block_sum(l1_acc, scratch);
     const float ss_block = block_sum(ssim_acc, scratch);
     if (tid == 0) {
-        if constexpr (BG != 0 || MASK) {  // fp64 totals: the 1e-6 bar of the means holds at 800x800 with masked (partly constant) images
+        if constexpr (BG != 0 || MASK || POST != 0) {  // fp64 totals: the 1e-6 bar of the means holds at 800x800 with masked (partly constant) images
             atomicAdd(cp.acc + 0, static_cast<double>(l1_block));
             atomicAdd(cp.acc + 1, static_cast<double>(ss_block));
         } else {
@@ -161,7 +193,7 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
 
 // GS: floats per pixel of the gradient (4: d_rgba, one 16-byte store, its alpha gradient zero unless BG != 0; 3: d_rgb, plus cp.d_alpha
 // in the composited entry).
-template <int PS, int GS, int BG = 0, bool MASK = false>
+template <int PS, int GS, int BG = 0, bool MASK = false, int POST = 0>
 __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
                                                             Composite cp, Window win, float l1_scale /* lambda_l1 / (H W 3) */,
                                                             const float* __restrict__ dmaps, float* __restrict__ d_rgba) {
@@ -171,13 +203,14 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
     const int x0 = blockIdx.x * kT, y0 = blockIdx.y * kT;
     const int px = x0 + tx, py = y0 + ty;
     const bool inside = (px < W) && (py < H);
-    if constexpr (BG != 0 || MASK) {
+    if constexpr (BG != 0 || MASK || POST != 0) {
         if (blockIdx.x == 0 && blockIdx.y == 0 && tid == 0) {  // every block of ssim_stats_kernel has finished (stream order)
             cp.sums[0] = static_cast<float>(cp.acc[0]);
             cp.sums[1] = static_cast<float>(cp.acc[1]);
         }
     }
     float grad[3] = {0.f, 0.f, 0.f};
+    float slope[3];  // s'(c) of the post-processing (POST)
     for (int c = 0; c < 3; ++c) {
         for (int i = tid; i < kS * kS; i += kT * kT) {
             const int ly = i / kS, lx = i - ly * kS;
@@ -209,7 +242,8 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
         if (inside) {
             const int64_t p = static_cast<int64_t>(py) * W + px;
             float xv, yv;
-            load_xy<PS, BG, MASK>(pred_rgba, target, cp, p, c, xv, yv);
+            load_xy<PS, BG, MASK, POST>(pred_rgba, target, cp, p, c, xv, yv);
+            if constexpr (POST == 1) slope[c] = linear_to_srgb_slope(composite<PS, BG>(pred_rgba[p * PS + c], pred_rgba, cp, p, c));
             const float diff = xv - yv;
             const float sgn = diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f);
             grad[c] = c0 + 2.f * xv * c1 + yv * c2 + l1_scale * sgn;
@@ -218,7 +252,10 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
     }
     if (!inside) return;
     const int64_t p = static_cast<int64_t>(py) * W + px;
-    // chain rule through the mask and the composite: grad is d loss / d x of the masked composite
+    // chain rule through the mask, the post-processing and the composite: grad is d loss / d x of the masked composite
+    if constexpr (POST != 0) {
+        grad[0] *= slope[0]; grad[1] *= slope[1]; grad[2] *= slope[2];
+    }
     if constexpr (MASK) {
         const float m = cp.mask[p];
         grad[0] *= m; grad[1] *= m; grad[2] *= m;
@@ -235,11 +272,11 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
         d_rgba[p * GS + 0] = grad[0];
         d_rgba[p * GS + 1] = grad[1];
         d_rgba[p * GS + 2] = grad[2];
-        if constexpr (BG != 0 || MASK) cp.d_alpha[p] = d_alpha;
+        if constexpr (BG != 0 || MASK || POST != 0) cp.d_alpha[p] = d_alpha;
     }
 }
 
-template <int PS, int GS, int BG = 0, bool MASK = false>
+template <int PS, int GS, int BG = 0, bool MASK = false, int POST = 0>
 int image_loss(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1, float lambda_ssim,
                void* scratch, float* d_pred, float* sums2, Composite cp = Composite{}) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -254,7 +291,7 @@ int image_loss(void* stream, int32_t height, int32_t width, const float* pred, c
     const double count = (height > 10 && width > 10) ? static_cast<double>(height - 10) * (width - 10) * 3.0 : 1.0;
     const dim3 block(kT, kT), grid((width + kT - 1) / kT, (height + kT - 1) / kT);
     float* dmaps = static_cast<float*>(scratch);
-    if constexpr (BG != 0 || MASK) {
+    if constexpr (BG != 0 || MASK || POST != 0) {
         // the composited kernels keep their two sums in fp64 at the head of the scratch (its 16 spare bytes), the maps after them
         cp.acc = static_cast<double*>(scratch);
         cp.sums = sums2;
@@ -263,17 +300,31 @@ int image_loss(void* stream, int32_t height, int32_t width, const float* pred, c
     } else {
         if (cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s) != cudaSuccess) return 2;
     }
-    ssim_stats_kernel<PS, BG, MASK><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win, static_cast<float>(-lambda_ssim / count),
-                                                           dmaps, sums2);
-    loss_grad_kernel<PS, GS, BG, MASK><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win,
-                                                              static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)), dmaps,
-                                                              d_pred);
+    ssim_stats_kernel<PS, BG, MASK, POST><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win,
+                                                                 static_cast<float>(-lambda_ssim / count), dmaps, sums2);
+    loss_grad_kernel<PS, GS, BG, MASK, POST><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win,
+                                                                    static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)),
+                                                                    dmaps, d_pred);
     return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 
 template <int L>
 int image_loss_composited(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1,
-                          float lambda_ssim, void* scratch, float* d_pred, float* sums2, const Composite& cp, int bg_mode, bool mask) {
+                          float lambda_ssim, void* scratch, float* d_pred, float* sums2, const Composite& cp, int bg_mode, bool mask,
+                          int post = 0) {
+    if (post == 1) {
+        // every background and mask goes through the post-processed kernels (a black, unmasked one too: the encode is not the identity)
+#define GUT_LOSS_POST_CASE(BG_, M_) \
+    if (bg_mode == BG_ && mask == M_) return image_loss<L, L, BG_, M_, 1>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp);
+        GUT_LOSS_POST_CASE(0, false)
+        GUT_LOSS_POST_CASE(0, true)
+        GUT_LOSS_POST_CASE(1, false)
+        GUT_LOSS_POST_CASE(1, true)
+        GUT_LOSS_POST_CASE(2, false)
+        GUT_LOSS_POST_CASE(2, true)
+#undef GUT_LOSS_POST_CASE
+        return 1;
+    }
     if (bg_mode == 0 && !mask) {
         // black, no mask: the plain loss; the split layout's alpha gradient is zero
         if (L == 3 && cudaMemsetAsync(cp.d_alpha, 0, static_cast<size_t>(height) * width * sizeof(float), static_cast<cudaStream_t>(stream)) != cudaSuccess)
@@ -320,9 +371,9 @@ int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const fl
 //   layout 3: pred [H,W,3] rgb + pred_alpha [H,W], d_pred [H,W,3] = d_rgb + d_alpha [H,W]
 // background_rgb: 3 host floats, or NULL (black); background_image: [H,W,3] device image (takes precedence), or NULL.  A black background
 // is skipped entirely: no alpha gradient.  mask: [H,W] device floats, or NULL.
-int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
-                                  const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
-                                  float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2) {
+static int image_loss_entry(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                            const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                            float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2, int post) {
     if (height <= 0 || width <= 0 || !pred || !target_rgb || !scratch || !d_pred || !sums2) return 1;
     if (layout != 3 && layout != 4) return 1;
     if (layout == 3 && (!pred_alpha || !d_alpha)) return 1;
@@ -341,9 +392,32 @@ int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, i
     }
     if (layout == 4)
         return gutb200::image_loss_composited<4>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp,
-                                                 bg_mode, mask != nullptr);
+                                                 bg_mode, mask != nullptr, post);
     return gutb200::image_loss_composited<3>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp, bg_mode,
-                                             mask != nullptr);
+                                             mask != nullptr, post);
+}
+
+int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                                  const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                                  float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2) {
+    return image_loss_entry(stream, height, width, layout, pred, pred_alpha, target_rgb, background_rgb, background_image, mask, lambda_l1,
+                            lambda_ssim, scratch, d_pred, d_alpha, sums2, 0);
+}
+
+// The composited loss with the post-processing of the reference trainer applied after the background and before the mask:
+// post_processing 0 = none (gutb200_image_loss_composited itself), 1 = linear-to-sRGB.  Any other value returns 1 and names itself in
+// gutb200_last_error(NULL).
+int gutb200_image_loss_postprocessed(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                                     const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                                     float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2,
+                                     int32_t post_processing) {
+    if (post_processing != 0 && post_processing != 1) {
+        gutb200::set_context_free_error("gutb200_image_loss_postprocessed: post_processing=" + std::to_string(post_processing) +
+                                        " is not built (0 = none, 1 = linear-to-sRGB)");
+        return 1;
+    }
+    return image_loss_entry(stream, height, width, layout, pred, pred_alpha, target_rgb, background_rgb, background_image, mask, lambda_l1,
+                            lambda_ssim, scratch, d_pred, d_alpha, sums2, post_processing);
 }
 
 }  // extern "C"

@@ -6,7 +6,12 @@ w.r.t. the rendered image in two launches (csrc/gut_loss.cu), replacing l1_loss 
 With `background=` and / or `mask=`, the loss is taken on the prediction composited onto the background and multiplied by the mask, as the
 reference trainer does (model/background.py:80-93, trainer.py:691-694), in the same two launches (gutb200_image_loss_composited): the
 gradient then has a live alpha part.  image_loss_rgb_alpha is that loss on the 3DGRT layout (rgb and alpha as separate tensors).
-`Background` and `mask_hw` resolve the training steps' `background=` / `mask=` arguments.  No CPU fallback."""
+`Background` and `mask_hw` resolve the training steps' `background=` / `mask=` arguments.
+
+With `post_processing="linear-to-srgb"` (the reference's post_processing.method, configs/base_gs.yaml:188-197), the composited prediction is
+encoded to sRGB before the mask and the loss (threedgrut/utils/post_processing_linear_to_srgb.py, trainer.py:1165-1172), still in the same
+two launches (gutb200_image_loss_postprocessed): use it when the ground-truth images are display-referred sRGB and the renderer outputs
+linear radiance.  `linear_to_srgb` is that encode for rendered images outside the loss.  No CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -16,6 +21,23 @@ import torch
 import b200_native as native
 
 _scratch = {}
+
+POST_PROCESSING = {None: 0, "linear-to-srgb": 1}  # post_processing.method -> the post_processing code of gutb200_image_loss_postprocessed
+
+
+def post_processing_code(method) -> int:
+    """The device code of a post_processing.method: None -> 0, "linear-to-srgb" -> 1.  "ppisp" (a third-party package) and any other value
+    raise NotImplementedError naming the key.  Pure config logic: needs no GPU."""
+    if method is None or (isinstance(method, str) and method in POST_PROCESSING):
+        return POST_PROCESSING[method]
+    raise NotImplementedError(f"post_processing.method={method!r}: only null and 'linear-to-srgb' are built (PPISP is not)")
+
+
+def linear_to_srgb(x: torch.Tensor) -> torch.Tensor:
+    """Linear RGB -> sRGB, elementwise, as the reference Renderer applies post_processing.method linear-to-srgb to a rendered image
+    (render.py:307, post_processing_linear_to_srgb.py:43-67): 1.055 max(x, 1e-8)^(1/2.4) - 0.055 where x > 0.0031308, else 12.92 x; no
+    clamp, so values above 1 encode above 1.  Same shape, dtype and device as x."""
+    return torch.where(x > 0.0031308, 1.055 * torch.pow(torch.clamp(x, min=1e-8), 1.0 / 2.4) - 0.055, 12.92 * x)
 
 
 def _check_image(t, what, ch):
@@ -59,8 +81,9 @@ def _run(entry, pred, tgt, ch_pred, lambda_l1, lambda_ssim, d_pred, name):
     return (*_scalars(sums, H, W, lambda_l1, lambda_ssim), d_pred)
 
 
-def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background, mask, d_pred, d_alpha):
-    """gutb200_image_loss_composited.  background: None (black), 3 floats, or a float32 CUDA image [H,W,3]; mask: None or [H,W]."""
+def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background, mask, d_pred, d_alpha, post=0):
+    """gutb200_image_loss_composited, or gutb200_image_loss_postprocessed with post != 0.  background: None (black), 3 floats, or a float32
+    CUDA image [H,W,3]; mask: None or [H,W]."""
     _check_image(pred, "pred_rgba" if layout == 4 else "pred_rgb", layout)
     _check_image(tgt, "target_rgb", 3)
     H, W = int(pred.shape[0]), int(pred.shape[1])
@@ -91,50 +114,64 @@ def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background
     sums = torch.empty(2, dtype=torch.float32, device=dev)
     stream = torch.cuda.current_stream(dev).cuda_stream
     ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+    args = (stream, H, W, layout, pred.data_ptr(), ptr(alpha), tgt.data_ptr(), bg_rgb, ptr(bg_img), ptr(mask), float(lambda_l1),
+            float(lambda_ssim), scratch.data_ptr(), d_pred.data_ptr(), ptr(d_alpha), sums.data_ptr())
+    entry = "gutb200_image_loss_postprocessed" if post else "gutb200_image_loss_composited"
     with torch.cuda.device(dev):
-        rc = lib.gutb200_image_loss_composited(stream, H, W, layout, pred.data_ptr(), ptr(alpha), tgt.data_ptr(), bg_rgb, ptr(bg_img), ptr(mask),
-                                               float(lambda_l1), float(lambda_ssim), scratch.data_ptr(), d_pred.data_ptr(), ptr(d_alpha),
-                                               sums.data_ptr())
+        rc = lib.gutb200_image_loss_postprocessed(*args, post) if post else lib.gutb200_image_loss_composited(*args)
     if rc != 0:
-        raise RuntimeError(f"gutb200_image_loss_composited failed ({rc})")
+        raise RuntimeError(f"{entry} failed ({rc})")
     return (*_scalars(sums, H, W, lambda_l1, lambda_ssim), d_pred, d_alpha)
 
 
 def image_loss(pred_rgba: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: float = 0.8, lambda_ssim: float = 0.2, d_rgba: torch.Tensor | None = None,
-               background=None, mask: torch.Tensor | None = None):
+               background=None, mask: torch.Tensor | None = None, post_processing=None):
     """pred_rgba [H,W,4] (or [1,H,W,4]), target_rgb [H,W,3] float32 CUDA tensors.
     Returns (loss, l1, ssim, d_rgba): three device scalars and d loss / d pred_rgba [H,W,4].
     background: None (black), (r, g, b), or a float32 CUDA image [H,W,3]; mask: None or a float CUDA tensor [H,W] ([H,W,1], [1,H,W,1]).
-    With either, the loss is taken on (rgb + background (1 - alpha)) * mask against target * mask and d_rgba carries the alpha gradient."""
+    With either, the loss is taken on (rgb + background (1 - alpha)) * mask against target * mask and d_rgba carries the alpha gradient.
+    post_processing: None or "linear-to-srgb" (the composite is encoded to sRGB before the mask; see linear_to_srgb)."""
+    post = post_processing_code(post_processing)
     pred = pred_rgba.reshape(pred_rgba.shape[-3:])
     tgt = target_rgb.reshape(target_rgb.shape[-3:])
+    if post:
+        return _run_composited(4, pred, None, tgt, lambda_l1, lambda_ssim, background, mask, d_rgba, None, post)[:4]
     if background is None and mask is None:
         return _run("gutb200_image_loss", pred, tgt, 4, lambda_l1, lambda_ssim, d_rgba, "pred_rgba")
     return _run_composited(4, pred, None, tgt, lambda_l1, lambda_ssim, background, mask, d_rgba, None)[:4]
 
 
-def image_loss_rgb(pred_rgb: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: float = 0.8, lambda_ssim: float = 0.2, d_rgb: torch.Tensor | None = None):
+def image_loss_rgb(pred_rgb: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: float = 0.8, lambda_ssim: float = 0.2, d_rgb: torch.Tensor | None = None,
+                   post_processing=None):
     """The same loss on the 3DGRT layout: pred_rgb [H,W,3] (or [1,H,W,3], the tracer's rgb output; its alpha takes no part), target_rgb
     [H,W,3].  Returns (loss, l1, ssim, d_rgb) with d_rgb [H,W,3] -- directly the rgb gradient of OptixTracer.trace_bwd.  Bit-identical to
-    image_loss on cat([rgb, alpha], -1)."""
+    image_loss on cat([rgb, alpha], -1).  post_processing as in image_loss."""
+    post = post_processing_code(post_processing)
     pred = pred_rgb.reshape(pred_rgb.shape[-3:])
     tgt = target_rgb.reshape(target_rgb.shape[-3:])
+    if post:
+        # black and unmasked: the alpha is never read and its gradient is zero, but the split layout takes both
+        H, W = int(pred.shape[0]), int(pred.shape[1])
+        alpha = torch.zeros((H, W, 1), dtype=torch.float32, device=pred.device)
+        return _run_composited(3, pred, alpha, tgt, lambda_l1, lambda_ssim, None, None, d_rgb, None, post)[:4]
     return _run("gutb200_image_loss_rgb", pred, tgt, 3, lambda_l1, lambda_ssim, d_rgb, "pred_rgb")
 
 
 def image_loss_rgb_alpha(pred_rgb: torch.Tensor, pred_alpha: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: float = 0.8,
                          lambda_ssim: float = 0.2, background=None, mask: torch.Tensor | None = None, d_rgb: torch.Tensor | None = None,
-                         d_alpha: torch.Tensor | None = None):
+                         d_alpha: torch.Tensor | None = None, post_processing=None):
     """The composited, masked loss on the 3DGRT layout: pred_rgb [H,W,3] and pred_alpha [H,W,1] (or [1,H,W,3] / [1,H,W,1], the tracer's
     outputs), target_rgb [H,W,3]; background / mask as in image_loss.  Returns (loss, l1, ssim, d_rgb [H,W,3], d_alpha [H,W,1]) -- directly
-    the rgb and alpha gradients of OptixTracer.trace_bwd.  A black background with no mask gives d_rgb of image_loss_rgb and d_alpha = 0."""
+    the rgb and alpha gradients of OptixTracer.trace_bwd.  A black background with no mask gives d_rgb of image_loss_rgb and d_alpha = 0.
+    post_processing as in image_loss."""
+    post = post_processing_code(post_processing)
     pred = pred_rgb.reshape(pred_rgb.shape[-3:])
     tgt = target_rgb.reshape(target_rgb.shape[-3:])
     H, W = int(pred.shape[0]), int(pred.shape[1])
     if not (isinstance(pred_alpha, torch.Tensor) and pred_alpha.is_cuda and pred_alpha.dtype == torch.float32 and pred_alpha.is_contiguous()
             and pred_alpha.numel() == H * W and pred_alpha.shape[-1] == 1):
         raise RuntimeError("pred_alpha: expected a contiguous float32 CUDA tensor [H,W,1] (there is no CPU fallback)")
-    return _run_composited(3, pred, pred_alpha, tgt, lambda_l1, lambda_ssim, background, mask, d_rgb, d_alpha)
+    return _run_composited(3, pred, pred_alpha, tgt, lambda_l1, lambda_ssim, background, mask, d_rgb, d_alpha, post)
 
 
 def mask_hw(mask: torch.Tensor, H: int, W: int) -> torch.Tensor:

@@ -4,8 +4,8 @@ Replaces the render + backward + optimizer part of Trainer.run_train_iter (three
 repository wired together -- no autograd graph, no per-parameter all-reduce, no separate activation backward:
 
     activations (sigmoid / exp / normalize, model.py:102-118)  ->  SplatRaster.trace
-    -> loss gradient on the image (L1, trainer.py:698-704 + losses.py:20-21; or L1 + SSIM, with the background composited and the mask
-       applied, by losses.image_loss)  ->  SplatRaster.trace_bwd_compact
+    -> loss gradient on the image (L1, trainer.py:698-704 + losses.py:20-21; or L1 + SSIM, with the background composited, the
+       linear-to-sRGB post-processing and the mask applied, by losses.image_loss)  ->  SplatRaster.trace_bwd_compact
     -> CompactGradientExchange (all-reduce [N,12], all-gather [N,4], rebuild [N,48])  ->  FusedGaussianAdam.step (+ the opacity and
        scale regularisers, once per step after the exchange)
 
@@ -34,13 +34,17 @@ class TrainStep:
 
     def __init__(self, params: dict, lrs: dict, conf=None, sph_degree: int = 3, selective: bool = False, group=None, eps: float = 1e-15,
                  densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0, background="black",
-                 background_seed: int = 0, lambda_opacity: float = 0.0, lambda_scale: float = 0.0):
+                 background_seed: int = 0, lambda_opacity: float = 0.0, lambda_scale: float = 0.0, post_processing=None):
         """params: raw leaf tensors for optimizers.GROUPS (positions, density, rotation, scale, features_albedo, features_specular).
         conf: a config with a `render:` section, read as the step's renderer reads it.
         densify_conf: a densify.DensifyConfig (GS strategy: clone / split / prune / reset) or densify.MCMCConfig (relocate / add / perturb)
         turns on the replica-consistent strategy.  background: "black", "white", "random" or (r, g, b), composited onto the render before
         the loss (model.background.color); "random" draws from a generator seeded background_seed + rank.  lambda_opacity / lambda_scale:
-        the regularisers of the loss (loss.lambda_opacity / loss.lambda_scale when use_opacity / use_scale)."""
+        the regularisers of the loss (loss.lambda_opacity / loss.lambda_scale when use_opacity / use_scale).  post_processing: None or
+        "linear-to-srgb" (post_processing.method): the composited render is encoded to sRGB before the mask and the loss, for sRGB targets
+        and linear radiance; "ppisp" raises NotImplementedError.  It has no parameters and adds 0 to the loss."""
+        losses.post_processing_code(post_processing)  # refuse what is not built before anything is allocated
+        self.post_processing = post_processing
         self.params = {k: params[k] for k in self.GROUPS}  # ONE dict shared with the optimizer and the densifier
         self.device = self.params["positions"].device
         self.sph_degree = int(sph_degree)
@@ -89,9 +93,9 @@ class TrainStep:
         """This view's loss and its gradient in the renderer's layout.  pred: the render as `_image_loss` / `_l1_grads` take it; rgb: its
         colour channels [H,W,3]; target: [H,W,3].  The gradient carries the global-batch normalisation (1 / world); the loss returned
         does not."""
-        if not self.background.black or mask is not None or self.lambda_ssim != 0.0:
-            # composited onto the background and masked (then with an alpha gradient), or lambda_l1 L1 + lambda_ssim (1 - SSIM): two
-            # launches (gut_loss.cu)
+        if not self.background.black or mask is not None or self.lambda_ssim != 0.0 or self.post_processing is not None:
+            # composited onto the background, post-processed and masked (then with an alpha gradient), or lambda_l1 L1 + lambda_ssim
+            # (1 - SSIM): two launches (gut_loss.cu).  The L1 shortcut below does not apply in encoded space.
             loss, grads = self._image_loss(pred, target.contiguous(), self.lambda_l1 / self.world, self.lambda_ssim / self.world,
                                            self.background.draw(H, W), mask)
             return loss * self.world, grads
@@ -129,6 +133,10 @@ class TrainStep:
         self._mark("densify")
         return loss
 
+    def _post_process(self, rgb):
+        """render()'s rgb as the loss sees it over a black background: linear_to_srgb(rgb) under post_processing, else rgb itself."""
+        return rgb if self.post_processing is None else losses.linear_to_srgb(rgb)
+
     def _adam(self, d_particles, d_sph, vis, reg):
         self.optimizer.step(d_particles, d_sph, visibility=vis, **reg)
 
@@ -152,7 +160,8 @@ class GaussianTrainStep(TrainStep):
         return view_parallel.CompactGradientExchange(self.raster, self.n, self.device, group=self.group)
 
     def _image_loss(self, rgba, target, lambda_l1, lambda_ssim, background, mask):
-        loss, _, _, d_rgba = losses.image_loss(rgba, target, lambda_l1, lambda_ssim, background=background, mask=mask)
+        loss, _, _, d_rgba = losses.image_loss(rgba, target, lambda_l1, lambda_ssim, background=background, mask=mask,
+                                               post_processing=self.post_processing)
         return loss, d_rgba  # d_rgba carries the alpha gradient when composited (gut_loss.cu)
 
     def _l1_grads(self, rgba, diff):
@@ -162,8 +171,11 @@ class GaussianTrainStep(TrainStep):
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, pose):
+        """Forward only: (rgba [H,W,4], dist, hits, visibility); under post_processing the rgb channels are encoded, alpha is not."""
         particles, sph = self.activated()
         rgba, dist_, hits, vis = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
+        if self.post_processing is not None:
+            rgba = torch.cat([self._post_process(rgba[..., :3]), rgba[..., 3:]], -1)
         return rgba, dist_, hits, vis
 
     @torch.no_grad()

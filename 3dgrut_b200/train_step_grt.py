@@ -4,8 +4,8 @@ Replaces Tracer.render + loss + autograd + per-parameter Adam of the reference t
 renderer) by the pieces of this repository wired together, with no autograd graph:
 
     activations (model.py:102-118)  ->  LBVH build from the [N,12] record (cadence of Tracer.build_acc, threedgrt_tracer/tracer.py:198-216)
-    -> OptixTracer.trace (hit lists recorded)  ->  image loss gradient (L1, or L1 + SSIM with losses.image_loss_rgb; with a background
-       or a mask, losses.image_loss_rgb_alpha, which also gives the alpha gradient)
+    -> OptixTracer.trace (hit lists recorded)  ->  image loss gradient (L1, or L1 + SSIM with losses.image_loss_rgb; with a background,
+       a mask or the linear-to-sRGB post-processing, losses.image_loss_rgb_alpha, which also gives the alpha gradient)
     -> OptixTracer.trace_bwd (hit-list replay) into the exchange buffer  ->  FlatGradientExchange (one all-reduce of 240 B x N)
     -> FusedGaussianAdam.step (+ the opacity and scale regularisers, once per step)  ->  GS / MCMC densification (replica-consistent)
 
@@ -43,11 +43,12 @@ class GaussianTrainStepGRT(TrainStep):
 
     def _image_loss(self, pred, target, lambda_l1, lambda_ssim, background, mask):
         rgb, alpha, zero1 = pred
-        if background is None and mask is None:  # black, unmasked: the rgb loss, no alpha gradient
+        if background is None and mask is None and self.post_processing is None:  # black, unmasked: the rgb loss, no alpha gradient
             loss, _, _, d_rgb = losses.image_loss_rgb(rgb, target, lambda_l1, lambda_ssim)
             return loss, (d_rgb, zero1)
-        # composited onto the background, masked: rgb and alpha gradients (gut_loss.cu)
-        loss, _, _, d_rgb, d_alpha = losses.image_loss_rgb_alpha(rgb, alpha, target, lambda_l1, lambda_ssim, background=background, mask=mask)
+        # composited onto the background, post-processed, masked: rgb and alpha gradients (gut_loss.cu)
+        loss, _, _, d_rgb, d_alpha = losses.image_loss_rgb_alpha(rgb, alpha, target, lambda_l1, lambda_ssim, background=background, mask=mask,
+                                                                 post_processing=self.post_processing)
         return loss, (d_rgb, d_alpha)
 
     def _l1_grads(self, pred, diff):
@@ -79,13 +80,13 @@ class GaussianTrainStepGRT(TrainStep):
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, T_to_world):
-        """Forward only: (rgb [1,H,W,3], alpha [1,H,W,1], dist [1,H,W,2], hits [1,H,W,1], visibility [N,1]).  The build it needs does not
-        advance the step's BVH cadence."""
+        """Forward only: (rgb [1,H,W,3], alpha [1,H,W,1], dist [1,H,W,2], hits [1,H,W,1], visibility [N,1]); rgb encoded under
+        post_processing.  The build it needs does not advance the step's BVH cadence."""
         particles, sph = self.activated()
         self.tracer.tracer_wrapper.build_bvh_packed(particles)
         rgb, alpha, dst, _, hits, vis = self.tracer.tracer_wrapper.trace(self.frame, T_to_world, rays_o, rays_d, particles, sph, 0,
                                                                           self.sph_degree, self.min_transmittance)
-        return rgb, alpha, dst, hits, vis
+        return self._post_process(rgb), alpha, dst, hits, vis
 
     @staticmethod
     def sensor_position(T_to_world) -> np.ndarray:

@@ -7,7 +7,8 @@ the pieces of this repository wired together, with no autograd graph:
     activations  ->  hybrid_rays (the world-space mirror rays and their hit mask, csrc/hybrid.cu)  ->  SplatRaster.trace (primary)
     -> packed LBVH build  ->  OptixTracer.trace of the [1,H,W,3] secondary rays (identity ray-to-world)
     -> hybrid_composite: rgb = primary_rgb + reflectivity (1 - primary alpha) hit secondary_rgb
-    -> image loss (L1; L1 + SSIM; or composited onto the background with the PRIMARY alpha and masked, which gives that alpha a gradient)
+    -> image loss (L1; L1 + SSIM; or composited onto the background with the PRIMARY alpha, encoded to sRGB and masked, which gives that
+       alpha a gradient)
     -> hybrid_composite_bwd -> SplatRaster.trace_bwd into the exchange buffer -> OptixTracer.trace_bwd(accumulate=True) into the same rows
     -> FlatGradientExchange (one all-reduce of 240 B x N)  ->  FusedGaussianAdam  ->  GS / MCMC densification (BVH rebuilt after it)
 
@@ -197,15 +198,15 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, T_to_world):
-        """Forward only: (hybrid rgb [H,W,3], primary rgba [H,W,4], secondary rgb [1,H,W,3], hit [H*W]).  The build it needs does not
-        advance the step's BVH cadence."""
+        """Forward only: (hybrid rgb [H,W,3], primary rgba [H,W,4], secondary rgb [1,H,W,3], hit [H*W]).  Under post_processing the hybrid
+        rgb is encoded, the two passes are returned as traced.  The build it needs does not advance the step's BVH cadence."""
         particles, sph = self.activated()
         _, rgba, _, _, sec, (_, _, hit), rgb = self._forward(rays_o, rays_d, sensor, T_to_world, particles, sph, train=False)
-        return rgb, rgba, sec[0], hit
+        return self._post_process(rgb), rgba, sec[0], hit
 
     def _image_loss(self, pred, target, lambda_l1, lambda_ssim, background, mask):
         rgb, rgba, zero1 = pred
-        alpha = rgba[..., 3:].contiguous() if (background is not None or mask is not None) else None
+        alpha = rgba[..., 3:].contiguous() if (background is not None or mask is not None or self.post_processing is not None) else None
         return GaussianTrainStepGRT._image_loss(self, (rgb, alpha, zero1), target, lambda_l1, lambda_ssim, background, mask)
 
     @torch.no_grad()

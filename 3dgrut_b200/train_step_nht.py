@@ -6,7 +6,7 @@ Replaces Tracer.render -> apply_feature_decoder -> apply_background -> loss -> a
 
     activations  ->  render the [N,48] features (3DGUT: [H,W,25] = 24 features + alpha; 3DGRT: packed BVH build, then [1,H,W,24] + alpha)
     -> FeatureDecoder forward on the world ray directions normalize(R_c2w rays_d)  ->  image loss on the decoded rgb (L1, L1 + SSIM, or
-       composited onto the background / masked, which gives the render's alpha its gradient)
+       composited onto the background / encoded to sRGB / masked, which gives the render's alpha its gradient)
     -> decoder backward: d_features into a per-resolution buffer, d_params straight into the tail of the exchange buffer
     -> render backward into the exchange buffer  ->  FlatGradientExchange ([N,12] + [N,48] + decoder params in ONE all-reduce)
     -> FusedNHTAdam (the Gaussians and the decoder in one launch)  ->  FeatureDecoder.ema_update  ->  GS / MCMC densification
@@ -170,9 +170,9 @@ class GaussianTrainStepNHT(_NHTStep, TrainStep):
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, pose):
-        """Forward only: (decoded rgb [H,W,3], alpha [H,W,1])."""
+        """Forward only: (decoded rgb [H,W,3], encoded under post_processing; alpha [H,W,1])."""
         out = self._forward(rays_o, rays_d, sensor, pose)
-        return out[8], out[6]
+        return self._post_process(out[8]), out[6]
 
     @torch.no_grad()
     def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None, mask=None):
@@ -216,11 +216,12 @@ class GaussianTrainStepGRTNHT(_NHTStep, GaussianTrainStepGRT):
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, T_to_world):
-        """Forward only: (decoded rgb [H,W,3], alpha [H,W,1]).  The build it needs does not advance the step's BVH cadence."""
+        """Forward only: (decoded rgb [H,W,3], encoded under post_processing; alpha [H,W,1]).  The build it needs does not advance the
+        step's BVH cadence."""
         particles, feats = self.activated()
         self.tracer.tracer_wrapper.build_bvh_packed(particles)
         out = self._forward(rays_o, rays_d, T_to_world, particles, feats)
-        return out[8], out[3][0]
+        return self._post_process(out[8]), out[3][0]
 
     @torch.no_grad()
     def step(self, rays_o, rays_d, T_to_world, target_rgb, all_sensor_positions=None, mask=None):

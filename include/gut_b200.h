@@ -21,7 +21,8 @@
  *   out_rgba  [H,W,4], out_dist [H,W], out_hits [H,W], visibility [N] (src/splatRaster.cpp:212-216)
  *   d_particles [N,12], d_sph [N,48]                                  (src/splatRaster.cpp:291-293)
  * Errors: every call returns 0 on success, non-zero on failure; gutb200_last_error() gives the message
- * (the reference logs and drops its Status codes, src/splatRaster.cpp:242,254; we surface them).
+ * (the reference logs and drops its Status codes, src/splatRaster.cpp:242,254; we surface them).  Given NULL, it gives the message of
+ * the last failed call on this thread that takes no context and records one (gutb200_image_loss_postprocessed), else "null context".
  */
 #ifndef GUT_B200_H
 #define GUT_B200_H
@@ -177,6 +178,15 @@ int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const fl
 int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
                                   const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
                                   float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2);
+/* gutb200_image_loss_composited with the reference trainer's post-processing (post_processing.method, threedgrut/utils/
+ * post_processing_linear_to_srgb.py) applied after the background and before the mask: post_processing 0 = none (the composited entry
+ * itself), 1 = linear-to-sRGB: x = s(c) m with c = rgb + bg (1 - alpha), s(c) = 1.055 max(c, 1e-8)^(1/2.4) - 0.055 above c = 0.0031308,
+ * 12.92 c at or below it (no clamp); d rgb = m s'(c) dL/dx, d alpha = -sum_c bg_c m s'(c_c) dL/dx_c.  Any other value returns 1, and
+ * gutb200_last_error(NULL) names it. */
+int gutb200_image_loss_postprocessed(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                                     const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                                     float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2,
+                                     int32_t post_processing);
 
 /* 3DGRUT hybrid (ours; hybrid.py's mirror_rays and render_hybrid as device code for train_step_hybrid): primary rays through 3DGUT, one
  * mirror bounce off a plane through 3DGRT.  No context: one launch each on `stream` of the current device, no synchronisation; 0 on success.
