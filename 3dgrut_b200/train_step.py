@@ -32,9 +32,10 @@ class TrainStep:
     (`_init_renderer`) and its exchange (`_new_exchange`), gives the loss gradient its renderer's layout (`_image_loss`, `_l1_grads`),
     and writes `step` as: activations -> trace -> `_loss` -> backward into `exchange.out()` -> `_update`."""
 
-    def __init__(self, params: dict, lrs: dict, conf=None, sph_degree: int = 3, selective: bool = False, group=None, eps: float = 1e-15,
-                 densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0, background="black",
-                 background_seed: int = 0, lambda_opacity: float = 0.0, lambda_scale: float = 0.0, post_processing=None):
+    def __init__(self, params: dict, lrs: dict | None, conf=None, sph_degree: int | None = None, selective: bool = False, group=None,
+                 eps: float = 1e-15, densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0,
+                 background="black", background_seed: int = 0, lambda_opacity: float = 0.0, lambda_scale: float = 0.0, post_processing=None,
+                 schedule=None):
         """params: raw leaf tensors for optimizers.GROUPS (positions, density, rotation, scale, features_albedo, features_specular).
         conf: a config with a `render:` section, read as the step's renderer reads it.
         densify_conf: a densify.DensifyConfig (GS strategy: clone / split / prune / reset) or densify.MCMCConfig (relocate / add / perturb)
@@ -42,12 +43,25 @@ class TrainStep:
         the loss (model.background.color); "random" draws from a generator seeded background_seed + rank.  lambda_opacity / lambda_scale:
         the regularisers of the loss (loss.lambda_opacity / loss.lambda_scale when use_opacity / use_scale).  post_processing: None or
         "linear-to-srgb" (post_processing.method): the composited render is encoded to sRGB before the mask and the loss, for sRGB targets
-        and linear radiance; "ppisp" raises NotImplementedError.  It has no parameters and adds 0 to the loss."""
+        and linear radiance; "ppisp" raises NotImplementedError.  It has no parameters and adds 0 to the loss.  sph_degree: the SH degree
+        rendered (default 3).  schedule: None (constant `lrs` and `sph_degree`) or a schedule.TrainingSchedule, which sets the initial rates
+        (in place of `lrs`) and degree (refused together with an explicit sph_degree) and updates both after every Adam launch, as the
+        reference trainer's schedulers and progressive SH do."""
         losses.post_processing_code(post_processing)  # refuse what is not built before anything is allocated
         self.post_processing = post_processing
         self.params = {k: params[k] for k in self.GROUPS}  # ONE dict shared with the optimizer and the densifier
         self.device = self.params["positions"].device
-        self.sph_degree = int(sph_degree)
+        self.schedule = schedule
+        if schedule is not None:
+            if sph_degree is not None:
+                raise ValueError("sph_degree and schedule: the schedule sets the SH degree (model.progressive_training); pass one of them")
+            lrs, sph_degree = schedule.initial_lrs(), schedule.initial_sph_degree()
+            missing = set(self.GROUPS) - set(lrs)
+            if missing:
+                raise ValueError(f"schedule: no learning rate for {sorted(missing)}; build it with the feature type this step trains")
+        elif lrs is None:
+            raise ValueError("lrs: the learning rates are required without a schedule")
+        self.sph_degree = 3 if sph_degree is None else int(sph_degree)
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
         self._init_renderer(conf if conf is not None else {"render": {}})
@@ -127,6 +141,11 @@ class TrainStep:
             reg = dict(lambda_opacity=self.lambda_opacity, lambda_scale=self.lambda_scale)
         self._adam(d_particles, d_sph, vis if self.optimizer.selective else None, reg)
         self._mark("adam")
+        if self.schedule is not None:
+            # the reference's scheduler_step(global_step = frame) and progressive SH, after Adam and before the strategy (schedule.py);
+            # host scalars the next step's launches take: no launch, no copy
+            lrs, self.sph_degree = self.schedule.advance(self.frame)
+            self.optimizer.lrs.update(lrs)
         self.frame += 1
         if self.densifier is not None and not frozen and self.densifier.post_optimizer_step(self.frame, self.scene_extent, positions_lr=self.optimizer.lrs["positions"]):
             self._densified()
