@@ -1,4 +1,5 @@
 """Shared helpers of the tests."""
+import dataclasses
 import os
 import re
 
@@ -147,6 +148,48 @@ def ray_sample(height, width, k, seed):
     idx = np.random.default_rng(seed).choice(height * width, size=k, replace=False)
     edge = np.concatenate([(height - 1) * width + np.arange(width), np.arange(height) * width + width - 1])
     return np.unique(np.concatenate([idx, edge]))
+
+
+def tile_sample(ranges, height, width, heaviest=16, k=48, seed=0):
+    """Sorted indices of a sample of the 16x16 tiles of a height x width frame: the `heaviest` longest lists of `ranges` ([T, 2] begin /
+    end of each tile's list), every tile of the last row and last column (partly filled on a ragged frame), and a seeded `k` others."""
+    gx, gy = (width + 15) // 16, (height + 15) // 16
+    lens = ranges[:, 1].astype(np.int64) - ranges[:, 0]
+    heavy = np.argsort(-lens, kind="stable")[:heaviest]
+    edge = np.concatenate([(gy - 1) * gx + np.arange(gx), np.arange(gy) * gx + gx - 1])
+    rest = np.setdiff1d(np.arange(gx * gy), np.concatenate([heavy, edge]))
+    pick = np.random.default_rng(seed).choice(rest, size=min(k, rest.size), replace=False)
+    return np.unique(np.concatenate([heavy, edge, pick]))
+
+
+def restrict_to_tiles(particles, sph, pr, bn, tiles):
+    """The oracle's frame cut down to the tiles `tiles`: a copy of the binning `bn` in which every other tile has an empty list, over
+    the particles those lists name alone.  Returns (rows, particles, sph, pr, bn): `rows` are the sorted indices of the kept particles in
+    the full scene, and the kept lists name them by their position in `rows`.  A pixel reads only its tile's list, so on the sampled
+    pixels the oracle's forward over the cut frame is the full frame's; with the output gradients zero on every other pixel, so is its
+    backward at `rows`, and every other particle's gradient is zero (tests/test_oracle_tile_sample.py pins both).  Dropping the other
+    particles keeps the backward's per-thread float64 accumulators at the size of the sample instead of the scene."""
+    ranges = np.zeros_like(bn.ranges)
+    ranges[tiles] = bn.ranges[tiles]
+    keep = np.zeros(len(bn.sorted_values), bool)
+    for b, e in bn.ranges[tiles]:
+        keep[b:e] = True
+    keep &= bn.sorted_values != 0xFFFFFFFF  # a list ends at its first invalid entry; that one stays as it is
+    rows = np.unique(bn.sorted_values[keep])
+    values = bn.sorted_values.copy()
+    values[keep] = np.searchsorted(rows, bn.sorted_values[keep]).astype(np.uint32)
+    sub_pr = dataclasses.replace(pr, **{f.name: getattr(pr, f.name)[rows] for f in dataclasses.fields(pr)})
+    sub_bn = dataclasses.replace(bn, sorted_values=values, ranges=ranges)
+    return rows, particles[rows], sph[rows], sub_pr, sub_bn
+
+
+def tile_pixels(tiles, height, width):
+    """[H, W] bool: the pixels of the 16x16 tiles `tiles` (row-major tile index, (width + 15) // 16 tiles per row)."""
+    gx = (width + 15) // 16
+    y, x = np.mgrid[0:height, 0:width]
+    mask = np.zeros(((height + 15) // 16) * gx, bool)
+    mask[tiles] = True
+    return mask[(y // 16) * gx + x // 16]
 
 
 def frac_within(a, b, atol):
