@@ -114,6 +114,7 @@ SIGNATURES = {
     "grtb200_build_bvh": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _i32]),
     "grtb200_build_bvh_packed": (_int, [_vp, _vp, _i64, _vp]),
     "grtb200_trace": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp]),
+    "grtb200_trace_normals": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_bwd": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_bwd_accumulate": (_int, _grt_trace + [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "grtb200_trace_nht": (_int, _grt_trace_nht + [_vp, _vp, _vp, _vp, _vp]),
@@ -374,6 +375,14 @@ class GrtContext(_Handle):
               out_dist, out_hits, visibility):
         self._check(self._lib.grtb200_trace(self._h, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d,
                                             r2w_host, out_rgb, out_alpha, out_dist, out_hits, visibility), "grtb200_trace")
+
+    def trace_normals(self, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d, r2w_host, out_rgb, out_alpha,
+                      out_dist, out_hits, visibility, out_normals):
+        """trace that also writes the unnormalised ray normals out_normals [R,3] (grtb200_trace_normals); trace_bwd replays its hit lists
+        as trace's, and the normals get no gradient."""
+        self._check(self._lib.grtb200_trace_normals(self._h, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o,
+                                                    rays_d, r2w_host, out_rgb, out_alpha, out_dist, out_hits, visibility, out_normals),
+                    "grtb200_trace_normals")
 
     def trace_bwd(self, stream, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d, r2w_host, out_rgb, out_alpha,
                   out_dist, d_rgb, d_alpha, d_dist, d_particles, d_sph, accumulate=False):

@@ -18,7 +18,8 @@
 //   replay_bwd_kernel replays those lists in the backward (no traversal, so one instantiation serves both primitives);
 //                     trace_kernel<PRIM,DEG,true> re-traces only overflowed rays.
 // Both kernels share one ray prologue (ray_pixel, world_ray), one k-nearest query loop for the forward and one for the re-trace and one hit adjoint
-// (backward_hit); the feature kind FK (ShRadiance or NhtFeatures, DESIGN.md section 13) supplies only what it accumulates.
+// (backward_hit); the feature kind FK (ShRadiance or NhtFeatures, DESIGN.md section 13; ShRadianceNormals, the SH forward that also sums
+// the rays' normals, section 17) supplies only what it accumulates.
 // Candidate rule (DESIGN.md section 9), primitive_type instances: the ray segment of the query meets the proxy's oriented box and
 // the custom intersection of the reference accepts (intersectInstanceParticle); icosahedron: the ray enters the proxy on the query's
 // (tmin, tmax), keyed by the entry t (front-facing triangle hit).  Subtrees entered beyond the current 16th hit are culled, which is
@@ -53,8 +54,10 @@ constexpr float kInf = 1e20f;     // RayHit::InfiniteDistance
 constexpr uint32_t kNone = 0xFFFFFFFFu;
 constexpr float kEpsT = 1e-9f;
 constexpr int kStack = 64;
-// What a trace integrates: SH radiance (grtb200_trace) or Neural Harmonic Texture features with fp32 / fp16 rows (grtb200_trace_nht).
-constexpr int kFeatSH = 0, kFeatNht = 1, kFeatNhtHalf = 2;
+// What a trace integrates: SH radiance (grtb200_trace) or Neural Harmonic Texture features with fp32 / fp16 rows (grtb200_trace_nht);
+// kFeatShNormals is the SH radiance forward that also accumulates the ray's normal (grtb200_trace_normals, DESIGN.md section 17).  It
+// has no backward of its own: its hit lists and its forward key are those of kFeatSH.
+constexpr int kFeatSH = 0, kFeatNht = 1, kFeatNhtHalf = 2, kFeatShNormals = 3;
 constexpr int kTraceThreads = 128;  // threads per trace / replay CTA: the NHT per-thread shared rows below are [kNhtOut][128]
 #ifndef GRT_BLOCKS_PER_SM
 #define GRT_BLOCKS_PER_SM 6
@@ -353,6 +356,7 @@ struct TraceParams {
     const float* d_rgb; const float* d_alpha; const float* d_dist;
     float* d_particles; float* d_sph;
     unsigned long long* counters;  // debug work counters (grtb200_debug_trace_counters); only the COUNT instantiation touches them
+    float* out_normals;            // [R,3] accumulated normals; only the kFeatShNormals forward touches them
 };
 
 // work counters of one forward trace (lane-level unless noted): 0 rays, 1 k-nearest queries, 2 node visits (one per warp and node in
@@ -581,8 +585,8 @@ struct RayGrad {
 };
 
 // What a trace integrates.  The walk (trace_rays, replay_bwd_kernel) does not depend on it; a kind supplies
-//   forward:  clear() its accumulators; chunk() once per k-nearest query; add() an accepted hit of weight w = alpha T, true when the
-//             hit counts and marks its particle visible; store() the ray's output;
+//   forward:  clear() its accumulators; chunk() once per k-nearest query; add() an accepted hit of particle frame f and weight
+//             w = alpha T, true when the hit counts and marks its particle visible; store() the ray's output;
 //   backward: init() from the forward's output and its gradient; chunk(); adjoint(), its part of the adjoint of an accepted hit, which
 //             fills the particle gradient; scatter() its own gradient row of the particle.
 
@@ -596,7 +600,7 @@ struct ShRadiance {
     __device__ __forceinline__ explicit ShRadiance(float*) {}
     __device__ __forceinline__ void clear() { Cx = Cy = Cz = 0.f; }
     __device__ __forceinline__ void chunk(const TraceParams& P, float dx, float dy, float dz) { sh_basis16(P.sph_degree, dx, dy, dz, basis); }
-    __device__ __forceinline__ bool add(const TraceParams& P, uint32_t pid, const CanonicalHit&, float w) {
+    __device__ __forceinline__ bool add(const TraceParams& P, uint32_t pid, const ParticleFrame&, const CanonicalHit&, float w) {
         const float4* c4 = reinterpret_cast<const float4*>(P.sph + static_cast<size_t>(pid) * 48);
         float cf[48];
 #pragma unroll
@@ -664,6 +668,39 @@ struct ShRadiance {
     }
 };
 
+// SH radiance plus the ray's normal (grtb200_trace_normals): forward only, out_normals = [R,3] unnormalised.  Per accepted hit, as
+// processHit accumulates rayNormal (gaussianParticles.cuh:397-401, referenceOptix.cu:103-186), with gro / grd the canonical ray and
+// grayDist = |grd x gro|^2 of the accept test:
+//   normal += w safe_normalize((gro + grd (dot(grd, -gro) - sqrt(9 - grayDist))) * (R s))
+// `*` element-wise and R s = operator*(float33, float3) of the quaternion matrix and the scale (mathUtils.h:450-455): sum_i s_i row_i.
+// It is not the ellipsoid's geometric normal; it is what the reference's "normals" view shows.  9 - grayDist < 0 needs a response
+// below exp(-4.5), i.e. min_response < 0.0111: there the sqrt is NaN, as in the reference.
+struct ShRadianceNormals : ShRadiance {
+    float Nx, Ny, Nz;
+
+    __device__ __forceinline__ explicit ShRadianceNormals(float* row) : ShRadiance(row) {}
+    __device__ __forceinline__ void clear() {
+        ShRadiance::clear();
+        Nx = Ny = Nz = 0.f;
+    }
+    __device__ __forceinline__ bool add(const TraceParams& P, uint32_t pid, const ParticleFrame& f, const CanonicalHit& h, float w) {
+        ShRadiance::add(P, pid, f, h, w);
+        const float sx = f.r0x * f.sx + f.r1x * f.sy + f.r2x * f.sz;  // particleRotation * particleScale
+        const float sy = f.r0y * f.sx + f.r1y * f.sy + f.r2y * f.sz;
+        const float sz = f.r0z * f.sx + f.r1z * f.sy + f.r2z * f.sz;
+        const float pd = -(h.gdx * h.gox + h.gdy * h.goy + h.gdz * h.goz) - sqrtf(9.0f - h.gray);
+        const float vx = (h.gox + h.gdx * pd) * sx, vy = (h.goy + h.gdy * pd) * sy, vz = (h.goz + h.gdz * pd) * sz;
+        const float l = vx * vx + vy * vy + vz * vz;
+        const float il = l > 0.f ? rsqrtf(l) : 1.f;  // safe_normalize
+        Nx += w * (vx * il); Ny += w * (vy * il); Nz += w * (vz * il);
+        return true;
+    }
+    __device__ __forceinline__ void store(const TraceParams& P, int64_t ray) {
+        ShRadiance::store(P, ray);
+        P.out_normals[ray * 3] = Nx; P.out_normals[ray * 3 + 1] = Ny; P.out_normals[ray * 3 + 2] = Nz;
+    }
+};
+
 // Neural Harmonic Texture features (grtb200_trace_nht, DESIGN.md section 13) with fp32 or fp16 (HALF) rows: sph = the [N,48] feature
 // rows, out_rgb / d_rgb = the [R,24] ray features, d_sph = the [N,48] fp32 feature gradient.  The ray's 24 accumulators (forward) or
 // gradients (backward) live in `feat`, this thread's row of the CTA's lane-interleaved [kNhtOut][kTraceThreads] shared array: they do
@@ -687,7 +724,7 @@ struct NhtFeatures {
         bary_weights(h.gox + h.gdx * pd, h.goy + h.gdy * pd, h.goz + h.gdz * pd, wk);
         blend_global<HALF>(P.sph, pid, wk, b);
     }
-    __device__ __forceinline__ bool add(const TraceParams& P, uint32_t pid, const CanonicalHit& h, float w) {
+    __device__ __forceinline__ bool add(const TraceParams& P, uint32_t pid, const ParticleFrame&, const CanonicalHit& h, float w) {
         // referenceSlangOptix.cu:144-176: features, hit count and visibility only where the hit weight is > 0
         if (!(w > 0.f)) return false;
         float fb[kNhtBase];
@@ -749,12 +786,13 @@ struct NhtFeatures {
 };
 
 template <int FK>
-using Kind = std::conditional_t<FK == kFeatSH, ShRadiance, NhtFeatures<FK == kFeatNhtHalf>>;
+using Kind = std::conditional_t<FK == kFeatSH, ShRadiance,
+                                std::conditional_t<FK == kFeatShNormals, ShRadianceNormals, NhtFeatures<FK == kFeatNhtHalf>>>;
 
 // this thread's feature row (NhtFeatures); nullptr for SH radiance, which keeps its accumulators in registers
 template <int FK>
 __device__ __forceinline__ float* feature_row() {
-    if constexpr (FK == kFeatSH) {
+    if constexpr (FK == kFeatSH || FK == kFeatShNormals) {
         return nullptr;
     } else {
         __shared__ float s_feat[kNhtOut][kTraceThreads];  // lane-interleaved ([channel][thread]: conflict-free), 12 KB per CTA
@@ -828,7 +866,7 @@ __device__ __forceinline__ void trace_rays(const TraceParams& P, const TraceRay&
                 }
                 if (h.accept) {
                     const float w = h.alpha * T;
-                    if (kind.add(P, pid, h, w)) {
+                    if (kind.add(P, pid, f, h, w)) {
                         hits += 1.f;
                         P.visibility[pid] = __int_as_float(1);  // benign race, same value (referenceOptix.cu:158-161)
                     }
@@ -1272,16 +1310,19 @@ int grtb200_scene_aabb(grtb200_ctx* c, float* aabb6) {
 }
 
 // Forward of either feature kind: fk = kFeatSH (sph [N,48] SH coefficients, out_rgb [R,3]) or an NHT kind (sph = the [N,48] feature
-// rows, out_rgb = the [R,24] ray features).
+// rows, out_rgb = the [R,24] ray features).  out_normals (SH only, else nullptr): the kFeatShNormals forward also writes the [R,3]
+// normals; it records the same hit lists under the same key as the plain SH forward, so the SH backward replays them.
 static int trace_fwd(grtb200_ctx* c, int fk, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
                      float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o, const float* rays_d,
-                     const float* ray_to_world_host, float* out_rgb, float* out_alpha, float* out_dist, float* out_hits, float* visibility) {
+                     const float* ray_to_world_host, float* out_rgb, float* out_alpha, float* out_dist, float* out_hits, float* visibility,
+                     float* out_normals = nullptr) {
     if (!c) return 1;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     GRT_CUDA(c, cudaSetDevice(c->device));
     TraceParams P;
     if (int rc = fill_params(c, P, n, particles, sph, sph_degree, min_transmittance, batch, height, width, rays_o, rays_d, ray_to_world_host, s)) return rc;
     P.out_rgb = out_rgb; P.out_alpha = out_alpha; P.out_dist = out_dist; P.out_hits = out_hits; P.visibility = visibility;
+    P.out_normals = out_normals;
     if (n > 0) GRT_CUDA(c, cudaMemsetAsync(visibility, 0, static_cast<size_t>(n) * 4, s));
     // hit-list cache for the backward of this forward (grow-only; GRTB200_HITCAP=0 turns it off, the backward then re-traces)
     c->fwd_key.valid = false;
@@ -1319,10 +1360,23 @@ static int trace_fwd(grtb200_ctx* c, int fk, void* stream, int64_t n, const floa
         c->fwd_key.feature_kind = fk;
         c->hit_cap_used = cap;
     }
-    with_kind(fk, [&](auto k) { launch_trace<false, false, decltype(k)::value>(c->cfg, P, s); });
+    if (out_normals)
+        launch_trace<false, false, kFeatShNormals>(c->cfg, P, s);
+    else
+        with_kind(fk, [&](auto k) { launch_trace<false, false, decltype(k)::value>(c->cfg, P, s); });
     c->launches++;
     GRT_CUDA(c, cudaGetLastError());
     return 0;
+}
+
+int grtb200_trace_normals(grtb200_ctx* c, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
+                          float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o, const float* rays_d,
+                          const float* ray_to_world_host, float* out_rgb, float* out_alpha, float* out_dist, float* out_hits, float* visibility,
+                          float* out_normals) {
+    if (!c) return 1;
+    if (!out_normals) return fail(c, "out_normals is null (grtb200_trace writes no normals)");
+    return trace_fwd(c, kFeatSH, stream, n, particles, sph, sph_degree, min_transmittance, batch, height, width, rays_o, rays_d,
+                     ray_to_world_host, out_rgb, out_alpha, out_dist, out_hits, visibility, out_normals);
 }
 
 int grtb200_trace(grtb200_ctx* c, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,

@@ -23,14 +23,14 @@ NHT_PIPELINES = ("referenceSlang", "referenceSlangBwd")
 
 def _check_pipelines(pipeline, backward_pipeline, nht: bool, enable_normals: bool):
     """Refuse, with NotImplementedError naming the key, every pairing this tracer does not build: SH radiance goes with the reference /
-    referenceBwd pipelines, NHT features with referenceSlang / referenceSlangBwd; no normals.  Needs no GPU."""
+    referenceBwd pipelines, NHT features with referenceSlang / referenceSlangBwd; normals with SH radiance only.  Needs no GPU."""
     want, kind = (NHT_PIPELINES, "NHT features (model.feature_type: nht)") if nht else (SH_PIPELINES, "SH radiance (model.feature_type: sh)")
     if str(pipeline) != want[0]:
         raise NotImplementedError(f"render.pipeline_type={pipeline!r}: {kind} are traced through {want[0]!r} only")
     if str(backward_pipeline) != want[1]:
         raise NotImplementedError(f"render.backward_pipeline_type={backward_pipeline!r}: {kind} are differentiated through {want[1]!r} only")
-    if enable_normals:
-        raise NotImplementedError("render.enable_normals=True: normals output is not built")
+    if enable_normals and nht:
+        raise NotImplementedError("render.enable_normals=True: normals are built for SH radiance (reference pipeline) only")
 
 
 def _nht_config(conf):
@@ -57,6 +57,7 @@ class OptixTracer:
         if nht is None and int(particle_radiance_sph_degree) != 3:
             raise NotImplementedError("this build stores 16 SH coefficients per particle")
         self._nht = nht
+        self._normals = bool(enable_normals)
         # kind-dependent parts of trace / trace_bwd, resolved once: ray-feature channels, how the per-particle features are handed to the
         # kernels, and the native forward / backward with the arguments that select the kind (SH degree, or the NHT row layout)
         if nht is None:
@@ -115,9 +116,12 @@ class OptixTracer:
             raise RuntimeError(f"trace: NHT features must be a [N,{NHT_FEATURE_DIM}] CUDA tensor, got {tuple(features.shape)}")
         return features.detach().to(torch.float16 if self._nht["half"] else torch.float32).contiguous()
 
-    def trace(self, frame_id, ray_to_world, ray_ori, ray_dir, particle_density, particle_features, render_opts, sph_degree, min_transmittance):
+    def trace(self, frame_id, ray_to_world, ray_ori, ray_dir, particle_density, particle_features, render_opts, sph_degree, min_transmittance,
+              normals=None):
         """optixTracer.cpp:893-960 -> (feat [B,H,W,3], alpha [B,H,W,1], hit [B,H,W,2], normals [B,H,W,3], hits [B,H,W,1], vis [N,1]);
-        with NHT features feat is [B,H,W,24] and particle_features the [N,48] features."""
+        with NHT features feat is [B,H,W,24] and particle_features the [N,48] features.  normals (ours): None follows enable_normals;
+        False skips them for one call (a training step whose loss never reads them).  With normals the [B,H,W,3] tensor holds each ray's
+        unnormalised normal sum (grtb200_trace_normals), otherwise zeros; every other output is the same either way."""
         dev = ray_ori.device
         b, h, w = (int(v) for v in ray_ori.shape[:3])
         n = int(particle_density.shape[0])
@@ -126,13 +130,17 @@ class OptixTracer:
         opts = dict(dtype=torch.float32, device=dev)
         feat, alpha = torch.empty((b, h, w, self._out_channels), **opts), torch.empty((b, h, w, 1), **opts)
         hit, hits = torch.empty((b, h, w, 2), **opts), torch.empty((b, h, w, 1), **opts)
-        nrm = torch.zeros((b, h, w, 3), **opts)
+        with_normals = self._normals if normals is None else bool(normals) and self._normals
+        nrm = (torch.empty if with_normals else torch.zeros)((b, h, w, 3), **opts)  # the normals forward writes every ray
         vis = torch.empty((max(n, 1), 1), **opts)
         r2w = self._r2w(ray_to_world)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        self._native_trace(self._context(dev), stream, n, ptr(particle_density), ptr(particle_features), *self._kind_args(sph_degree),
-                           float(min_transmittance), b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(feat), ptr(alpha), ptr(hit),
-                           ptr(hits), ptr(vis))
+        args = (self._context(dev), stream, n, ptr(particle_density), ptr(particle_features), *self._kind_args(sph_degree), float(min_transmittance),
+                b, h, w, ptr(ray_ori), ptr(ray_dir), r2w.ctypes.data, ptr(feat), ptr(alpha), ptr(hit), ptr(hits), ptr(vis))
+        if with_normals:
+            native.GrtContext.trace_normals(*args, ptr(nrm))
+        else:
+            self._native_trace(*args)
         return feat, alpha, hit, nrm, hits, vis[:n]
 
     def set_replay(self, enable, device):
@@ -163,7 +171,9 @@ class OptixTracer:
         (SH radiance, with `out`): this trace's gradients are added to what `out` holds instead (grtb200_trace_bwd_accumulate), so that
         two passes can write one buffer.  With NHT features dFeatures is the fp32 [N,48] feature gradient, and `out` is taken the same way.
         The reference's Slang backward reads the forward's features rounded to fp16 under render.feature_output_half; this one reads
-        them as the forward wrote them, in fp32 (feature_output_half is not applied, DESIGN.md section 13)."""
+        them as the forward wrote them, in fp32 (feature_output_half is not applied, DESIGN.md section 13).  ray_normals and
+        ray_normals_grd are accepted and ignored: the normals get no gradient, as in the reference, whose backward (referenceBwdOptix.cu)
+        never reads them (DESIGN.md section 17); a forward with normals is replayed as one without."""
         if accumulate and (out is None or self._nht is not None):
             raise NotImplementedError("trace_bwd(accumulate=True) adds SH radiance gradients into a given `out` pair")
         dev = ray_ori.device

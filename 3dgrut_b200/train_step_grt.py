@@ -85,7 +85,7 @@ class GaussianTrainStepGRT(TrainStep):
         particles, sph = self.activated()
         self.tracer.tracer_wrapper.build_bvh_packed(particles)
         rgb, alpha, dst, _, hits, vis = self.tracer.tracer_wrapper.trace(self.frame, T_to_world, rays_o, rays_d, particles, sph, 0,
-                                                                          self.sph_degree, self.min_transmittance)
+                                                                          self.sph_degree, self.min_transmittance, normals=False)
         return self._post_process(rgb), alpha, dst, hits, vis
 
     @staticmethod
@@ -108,7 +108,7 @@ class GaussianTrainStepGRT(TrainStep):
         self._build(particles)
         self._mark("build")
         rgb, alpha, dst, nrm, hits, vis = ot.trace(self.frame, T_to_world, rays_o, rays_d, particles, sph, 0, self.sph_degree,
-                                                   self.min_transmittance)
+                                                   self.min_transmittance, normals=False)  # render.enable_normals: the loss reads none
         self._mark("trace")
         zero1, zero3 = self._zero_grads(H, W)
         loss, (d_rgb, d_alpha) = self._loss((rgb, alpha, zero1), rgb[0], target_rgb.reshape(H, W, 3), H, W, mask)

@@ -191,7 +191,8 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         else:
             self.tracer.tracer_wrapper.build_bvh_packed(particles)
         self._mark("build")
-        sec = self.tracer.tracer_wrapper.trace(self.frame, self._identity, sec_o, sec_d, particles, sph, 0, self.sph_degree, self.min_transmittance)
+        sec = self.tracer.tracer_wrapper.trace(self.frame, self._identity, sec_o, sec_d, particles, sph, 0, self.sph_degree, self.min_transmittance,
+                                               normals=False)
         self._mark("secondary")
         rgb = hybrid_composite(rgba, sec[0], hit, self.reflectivity, out=buf["rgb"])
         return pose, rgba, dst, vis_p, sec, (sec_o, sec_d, hit), rgb

@@ -9,6 +9,7 @@
  *   grtb200_build_bvh          <- OptixTracer::buildBVH                           (src/optixTracer.cpp:616-890)
  *   grtb200_build_bvh_packed   the same build from the [N,12] particle record (ours: the no-autograd training step)
  *   grtb200_trace              <- OptixTracer::trace   -> __raygen__rg            (src/optixTracer.cpp:893-960, src/kernels/cuda/referenceOptix.cu:103-186)
+ *   grtb200_trace_normals      grtb200_trace that also sums the rays' normals (render.enable_normals)
  *   grtb200_trace_bwd          <- OptixTracer::traceBwd -> bwd __raygen__rg        (src/optixTracer.cpp:962-1031, src/kernels/cuda/referenceBwdOptix.cu:103-170)
  *   grtb200_trace_nht / grtb200_trace_bwd_nht  the same with NHT features         (src/kernels/cuda/referenceSlangOptix.cu, referenceSlangBwdOptix.cu)
  *
@@ -70,6 +71,18 @@ int grtb200_trace(grtb200_ctx* ctx, void* stream, int64_t n, const float* partic
                   float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
                   const float* rays_d, const float* ray_to_world_host, float* out_rgb, float* out_alpha, float* out_dist,
                   float* out_hits, float* visibility);
+
+/* grtb200_trace that also writes the rays' normals (render.enable_normals; <- the `normal` accumulator of processHit,
+ * include/3dgrt/kernels/cuda/gaussianParticles.cuh:397-401): out_normals [R,3] = sum over the accepted hits of
+ * weight * safe_normalize((gro + grd (dot(grd, -gro) - sqrt(9 - grayDist))) * (R s)), unnormalised, written for every ray (zero where
+ * no hit is accepted).  Every other output is bit-identical to grtb200_trace's, and the hit lists it records are replayed by
+ * grtb200_trace_bwd / grtb200_trace_bwd_accumulate exactly as grtb200_trace's are.  There is no gradient of the normals (the reference's
+ * backward has none).  A particle_kernel_min_response below exp(-4.5) = 0.0111 makes sqrt(9 - grayDist) NaN for some hits, as in the
+ * reference.  out_normals must not be null. */
+int grtb200_trace_normals(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
+                          float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                          const float* rays_d, const float* ray_to_world_host, float* out_rgb, float* out_alpha, float* out_dist,
+                          float* out_hits, float* visibility, float* out_normals);
 
 int grtb200_trace_bwd(grtb200_ctx* ctx, void* stream, int64_t n, const float* particles, const float* sph, int32_t sph_degree,
                       float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
