@@ -10,9 +10,10 @@
 //                  heaviest-first tile order, total I and the capacity check on the device
 //   expand_place   every (particle, tile) pair is dropped into its tile's slice at an atomically claimed slot as the 64-bit key
 //                  (depth bits << 32 | particle index)                                      (gut_project.cu)
-//   tile_sort      one CTA per tile sorts its slice by that key: a stable LSD radix sort over the depth bits (8 bits a pass, passes
-//                  with a single digit skipped; a slice of up to 4096 keys is sorted in shared memory, a longer one ping-pongs
-//                  through the L2) + a fix-up of equal-depth runs by particle index
+//   tile_sort      one CTA per tile sorts its slice by that key: a slice of up to 4096 keys in shared memory by one counting pass
+//                  over depth buckets and a rank inside each bucket; a longer slice (or one with an over-full bucket) by a stable LSD
+//                  radix sort over the depth bits (8 bits a pass, single-digit passes skipped) + a fix-up of equal-depth runs by
+//                  particle index
 //                  (a first version used a bitonic network: 125 M compare-exchanges at C2 cost 0.13 ms, 2.0 ms at C3 -- replaced)
 // The keys are unique inside a tile (a particle enters a tile once), so the result is exactly the reference's order whatever order
 // the atomics claimed the slots in; only sorted artefacts are observable and they stay bit-identical (tests/test_gut_parity_gpu.py).
@@ -187,10 +188,11 @@ __global__ void __launch_bounds__(kScanTiles) tile_scan_write_kernel(int num_til
 // cloned Gaussians; the slots were claimed in arbitrary order, so the sort cannot rely on stability for them.
 
 //
-// A slice of at most kStageKeys keys (every tile of C2) is sorted in shared memory instead: it is loaded once, each pass reads the warp's
-// segment into registers, ranks it and scatters it back into the same shared buffer (the reads of a pass end at the barriers before its
-// scatter, so one buffer suffices), the fix-up runs there, and the values are written once.  Longer slices (C3: 6-30 k keys) keep the
-// L2 ping-pong.  The CTA picks its path from n, so the choice is uniform across it.
+// A slice of at most kStageKeys keys (every tile of C2) is sorted in shared memory instead, by the bucket pass below; only if one of its
+// depth buckets is over-full does it take the radix passes in shared memory: each pass reads the warp's segment into registers, ranks it
+// and scatters it back into the same shared buffer (the reads of a pass end at the barriers before its scatter, so one buffer suffices),
+// the fix-up runs there, and the values are written once.  Longer slices (C3: 6-30 k keys) keep the L2 ping-pong.  The CTA picks its
+// path from n and from a CTA-wide vote, so the choice is uniform across it.
 
 constexpr int kSortThreads = 512, kSortWarps = kSortThreads / 32;   // 16 warps per tile: the long lists (6-30 k keys at C3) are latency-bound
 constexpr int kSortUnroll = 4;                                      // keys in flight per lane in the count / scatter loops
@@ -275,12 +277,100 @@ __device__ __forceinline__ void fix_equal_depth_runs(unsigned long long* a, uint
     }
 }
 
+// Bucket pass for a staged slice (n <= kStageKeys): one counting sort on the depth bits, then the keys of each bucket are ranked by the
+// full 64-bit key.  The depth bits are those of a non-negative float (a distance, or a view-space z >= 0.2 under global_z_order: the
+// projection drops every particle in front of that plane), so their unsigned order is the depth order -- and it is the order the radix
+// passes and the reference sort by either way.
+//   1. min / max of the depth bits over the CTA; `shift` maps (max - min) to fewer than kBuckets buckets of equal width
+//   2. each key is counted into bucket (d - min) >> shift
+//   3. one exclusive scan over the bucket counters (4 per thread); any bucket above kBucketMax keys sends the tile to the radix passes
+//   4. the keys are scattered into their buckets in s_keys at slots claimed from the offsets, which end as the buckets' ends
+//   5. a key's rank inside its bucket is the number of smaller keys there: every key lands on its final slot in one step, so no
+//      equal-depth fix-up is needed (the keys are unique)
+// Five barriers, against about four per radix pass plus the fix-up.  The bucket counters alias the radix digit counters.
+constexpr int kBucketBits = 11, kBuckets = 1 << kBucketBits;        // 2048: the fullest bucket of a C2 tile holds 4 keys (median) to 30
+constexpr int kBucketsPerThread = kBuckets / kSortThreads;         // one 16-byte load / store per thread
+constexpr uint32_t kBucketMax = 64;  // a fuller bucket (equal depths, clones, tight clusters) costs more to rank than the radix passes
+static_assert(kBucketsPerThread == 4 && kBuckets <= kSortWarps * 256, "bucket counters are one uint4 per thread inside s_cnt");
+
+// Returns false once `out` holds the slice's sorted values; true (uniformly) if a bucket was over-full -- s_keys then holds the slice.
+// Only the depth bits stay in registers across the barriers: the scatter reads the keys again (an L1 / L2 hit), the ranking reads them
+// from s_keys, so the radix passes that share the kernel keep their register budget.
+__device__ __forceinline__ bool bucket_pass(const unsigned long long* __restrict__ src, uint32_t n, uint32_t (*s_cnt)[256],
+                                            uint32_t (*s_wminmax)[kSortWarps], unsigned long long* s_keys, uint32_t* __restrict__ out) {
+    uint32_t* cnt = &s_cnt[0][0];
+    uint4* cnt4 = reinterpret_cast<uint4*>(cnt);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    cnt4[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u);
+    uint32_t d[kStagePerLane];
+    uint32_t lo = 0xFFFFFFFFu, hi = 0u;
+#pragma unroll
+    for (int u = 0; u < kStagePerLane; ++u) {
+        const uint32_t i = threadIdx.x + u * kSortThreads;
+        d[u] = i < n ? static_cast<uint32_t>(src[i] >> 32) : 0u;
+        if (i < n) {
+            lo = min(lo, d[u]);
+            hi = max(hi, d[u]);
+        }
+    }
+    lo = __reduce_min_sync(kFullMask, lo);
+    hi = __reduce_max_sync(kFullMask, hi);
+    if (lane == 0) {
+        s_wminmax[0][warp] = lo;
+        s_wminmax[1][warp] = hi;
+    }
+    __syncthreads();   // (1) counters zeroed, per-warp min / max published
+#pragma unroll
+    for (int w = 0; w < kSortWarps; ++w) {
+        lo = min(lo, s_wminmax[0][w]);
+        hi = max(hi, s_wminmax[1][w]);
+    }
+    const int shift = max(0, (32 - __clz(static_cast<int>(hi - lo))) - kBucketBits);   // (hi - lo) >> shift < kBuckets
+#pragma unroll
+    for (int u = 0; u < kStagePerLane; ++u)
+        if (threadIdx.x + u * kSortThreads < n) atomicAdd(&cnt[(d[u] - lo) >> shift], 1u);
+    __syncthreads();   // (2) counts complete
+    const uint4 c = cnt4[threadIdx.x];
+    const uint32_t sum = (c.x + c.y) + (c.z + c.w);
+    uint32_t incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t v = __shfl_up_sync(kFullMask, incl, o);
+        if (lane >= o) incl += v;
+    }
+    if (lane == 31) s_wminmax[0][warp] = incl;   // the min / max were read before barrier (2)
+    if (__syncthreads_or(max(max(c.x, c.y), max(c.z, c.w)) > kBucketMax)) {   // (3) uniform
+        for (uint32_t i = threadIdx.x; i < n; i += kSortThreads) s_keys[i] = src[i];
+        return true;   // the radix passes start by zeroing s_cnt: every read of it above precedes barrier (3)
+    }
+    uint32_t run = incl - sum;
+    for (int w = 0; w < warp; ++w) run += s_wminmax[0][w];
+    cnt4[threadIdx.x] = make_uint4(run, run + c.x, run + c.x + c.y, run + c.x + c.y + c.z);
+    __syncthreads();   // (4) bucket offsets
+#pragma unroll
+    for (int u = 0; u < kStagePerLane; ++u) {   // the offsets advance to the ends of the buckets
+        const uint32_t i = threadIdx.x + u * kSortThreads;
+        if (i < n) s_keys[atomicAdd(&cnt[(d[u] - lo) >> shift], 1u)] = src[i];
+    }
+    __syncthreads();   // (5) every bucket filled
+    for (uint32_t i = threadIdx.x; i < n; i += kSortThreads) {
+        const unsigned long long k = s_keys[i];
+        const uint32_t b = (static_cast<uint32_t>(k >> 32) - lo) >> shift;
+        const uint32_t first = b > 0u ? cnt[b - 1] : 0u, end = cnt[b];
+        uint32_t rank = first;
+        for (uint32_t j = first; j < end; ++j) rank += s_keys[j] < k ? 1u : 0u;
+        out[rank] = static_cast<uint32_t>(k);
+    }
+    return false;
+}
+
 template <bool BALLOT>
 __global__ void __launch_bounds__(kSortThreads) tile_sort_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ ranges,
                                                                  const uint32_t* __restrict__ totals, unsigned long long* keys,
                                                                  unsigned long long* keys_alt, uint32_t* __restrict__ sorted_values) {
     __shared__ uint32_t s_cnt[kSortWarps][256];   // per-warp digit counts -> running slot of (warp, digit)
     __shared__ uint32_t s_tot[8];
+    __shared__ uint32_t s_wminmax[2][kSortWarps];
     __shared__ int s_flag;
     extern __shared__ unsigned long long s_keys[];  // kStageKeys entries: the staged slice
     if (totals[1] != 0u) return;  // capacity exceeded: the host grows the buffers and launches again
@@ -298,7 +388,8 @@ __global__ void __launch_bounds__(kSortThreads) tile_sort_kernel(const uint32_t*
     const uint32_t w0 = min(n, warp * seg), w1 = min(n, w0 + seg);
 
     if (n <= static_cast<uint32_t>(kStageKeys)) {
-        for (uint32_t i = threadIdx.x; i < n; i += kSortThreads) s_keys[i] = src[i];
+        if (!bucket_pass(src, n, s_cnt, s_wminmax, s_keys, sorted_values + begin)) return;
+        // an over-full bucket: s_keys holds the slice (in bucket order), the radix passes sort it from there
         for (int shift = 32; shift < 64; shift += 8) {
             for (int i = threadIdx.x; i < aw * 256; i += kSortThreads) (&s_cnt[0][0])[i] = 0u;
             if (threadIdx.x == 0) s_flag = 0;

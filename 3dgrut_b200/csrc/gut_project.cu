@@ -17,7 +17,7 @@ namespace gutb200 {
 namespace {
 
 constexpr int kProjThreads = 256;
-constexpr int kSmallBox = 8;  // footprints above this many tiles are walked by the whole warp
+constexpr int kSmallBox = 8;  // project_kernel: footprints above this many tiles are counted by the whole warp
 
 struct TileBox {
     int x0, y0, x1, y1;
@@ -505,48 +505,45 @@ __global__ void __launch_bounds__(256) expand_place_kernel(FrameCamera cam, Fram
     float maxpow = 0.f;
     int cells = 0;
     unsigned long long key = 0ull;
-    auto place = [&](int tile, unsigned long long k) {   // sub-bucket = low bits of the particle index (low word of the key)
-        const size_t at = static_cast<size_t>(tile) * kTileSubs + (static_cast<uint32_t>(k) & (kTileSubs - 1));
-        const uint32_t slot = atomicAdd(&fill[at], 1u);
-        const uint32_t pos = sub_base[at] + slot;
-        if (slot < tile_hist[at] && pos < capacity) keys[pos] = k;
-    };
     if (active) {
         key = (static_cast<unsigned long long>(__float_as_uint(depth[i])) << 32) | static_cast<unsigned long long>(static_cast<uint32_t>(i));
         bb = tile_box(cam.grid_x, cam.grid_y, pr.cx, pr.cy, pr.ex, pr.ey);
-        cells = (bb.x1 - bb.x0) * (bb.y1 - bb.y0);
-        if (!cfg.tile_culling) {
-            for (int y = bb.y0; y < bb.y1; ++y)
-                for (int x = bb.x0; x < bb.x1; ++x) place(y * cam.grid_x + x, key);
-            cells = 0;
-        } else {
-            maxpow = logf(pr.op / cfg.min_alpha);
-            if (cells <= kSmallBox) {
-                for (int y = bb.y0; y < bb.y1; ++y)
-                    for (int x = bb.x0; x < bb.x1; ++x)
-                        if (tile_min_power(static_cast<float>(x), static_cast<float>(y), pr.ca, pr.cb, pr.cc, pr.cx, pr.cy) < maxpow)
-                            place(y * cam.grid_x + x, key);
-                cells = 0;
-            }
-        }
+        cells = max(0, (bb.x1 - bb.x0) * (bb.y1 - bb.y0));
+        if (cfg.tile_culling) maxpow = logf(pr.op / cfg.min_alpha);
     }
-    const unsigned lane = threadIdx.x & 31;
-    unsigned big = __ballot_sync(0xFFFFFFFFu, cells > kSmallBox);
-    while (big) {
-        const int src = __ffs(big) - 1;
-        big &= big - 1;
+    // The warp's footprints are one list of cells (an exclusive scan of the cell counts), walked 32 cells a step: every lane tests a
+    // cell whatever the sizes of the footprints, instead of each lane walking its own particle's box.  A lane's cell belongs to the last
+    // lane whose first cell is not after it (lanes with no cells share their successor's start and are skipped by the search).
+    const int lane = static_cast<int>(threadIdx.x & 31);
+    int first = cells;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xFFFFFFFFu, first, o);
+        if (lane >= o) first += v;
+    }
+    const int total = __shfl_sync(0xFFFFFFFFu, first, 31);
+    first -= cells;
+    for (int c0 = 0; c0 < total; c0 += 32) {
+        const int c = c0 + lane;
+        int src = 0;
+#pragma unroll
+        for (int step = 16; step > 0; step >>= 1)
+            if (__shfl_sync(0xFFFFFFFFu, first, src + step) <= c) src += step;
+        const int at0 = c - __shfl_sync(0xFFFFFFFFu, first, src);
         const int bx0 = __shfl_sync(0xFFFFFFFFu, bb.x0, src), by0 = __shfl_sync(0xFFFFFFFFu, bb.y0, src);
-        const int bw = __shfl_sync(0xFFFFFFFFu, bb.x1, src) - bx0, nc = __shfl_sync(0xFFFFFFFFu, cells, src);
+        const int bw = __shfl_sync(0xFFFFFFFFu, bb.x1, src) - bx0;
         const float qa = __shfl_sync(0xFFFFFFFFu, pr.ca, src), qb = __shfl_sync(0xFFFFFFFFu, pr.cb, src), qc = __shfl_sync(0xFFFFFFFFu, pr.cc, src);
         const float qx = __shfl_sync(0xFFFFFFFFu, pr.cx, src), qy = __shfl_sync(0xFFFFFFFFu, pr.cy, src), qp = __shfl_sync(0xFFFFFFFFu, maxpow, src);
         const unsigned long long qk = __shfl_sync(0xFFFFFFFFu, key, src);
-        for (int c0 = 0; c0 < nc; c0 += 32) {
-            const int c = c0 + static_cast<int>(lane);
-            if (c < nc) {
-                const int y = by0 + c / bw, x = bx0 + c % bw;
-                if (tile_min_power(static_cast<float>(x), static_cast<float>(y), qa, qb, qc, qx, qy) < qp) place(y * cam.grid_x + x, qk);
-            }
-        }
+        if (c >= total) continue;
+        const int y = by0 + at0 / bw, x = bx0 + at0 % bw;
+        // the culling test is project_kernel's expression on the same operands: the pairs claimed per (tile, sub-counter) are exactly
+        // the tile_hist counts, which bound the claims below
+        if (cfg.tile_culling && !(tile_min_power(static_cast<float>(x), static_cast<float>(y), qa, qb, qc, qx, qy) < qp)) continue;
+        const size_t at = static_cast<size_t>(y * cam.grid_x + x) * kTileSubs + (static_cast<uint32_t>(qk) & (kTileSubs - 1));  // sub-bucket: particle & 15
+        const uint32_t slot = atomicAdd(&fill[at], 1u);
+        const uint32_t pos = sub_base[at] + slot;
+        if (slot < tile_hist[at] && pos < capacity) keys[pos] = qk;
     }
 }
 
