@@ -45,6 +45,14 @@ def check_step_condition(step: int, start: int, end: int, freq: int) -> bool:  #
     return bool((start >= 0 and step > start) and (step < end or end == -1) and step % freq == 0)
 
 
+def load_generator(generator: torch.Generator, state, seed: int) -> None:
+    """Restore a generator from get_state()'s byte tensor (on any device), or seed it `seed` when there is none."""
+    if state is None:
+        generator.manual_seed(int(seed))
+    else:
+        generator.set_state(state.detach().to("cpu", torch.uint8))
+
+
 def quaternion_to_so3(q: torch.Tensor) -> torch.Tensor:
     """utils/misc.py quaternion_to_so3: rotation matrices of (unnormalised) w,x,y,z quaternions, normalised first."""
     q = torch.nn.functional.normalize(q, dim=1)
@@ -62,6 +70,8 @@ class GSDensifier:
     Every mutating call replaces the tensors inside those dicts in place of the old ones (the dict objects stay the same, so an optimizer
     holding them sees the new tensors)."""
 
+    METHOD = "gs"  # strategy.method
+
     def __init__(self, params: dict, moments: list, conf: DensifyConfig | None = None, group=None):
         self.params, self.moments, self.conf, self.group = params, moments, conf or DensifyConfig(), group
         dev = params["positions"].device
@@ -70,6 +80,26 @@ class GSDensifier:
         self.grad_norm_denom = torch.zeros((n, 1), dtype=torch.int32, device=dev)
         self.generator = torch.Generator(device=dev)
         self.generator.manual_seed(int(self.conf.seed))
+
+    def state_dict(self) -> dict:
+        """The gradient statistics (gs.py:42-57) and the split generator's state; the tensors are the densifier's own."""
+        return {"grad_norm_accum": self.grad_norm_accum, "grad_norm_denom": self.grad_norm_denom, "generator": self.generator.get_state()}
+
+    def load_state_dict(self, state: dict | None) -> None:
+        """Copies of the state's buffers for the current N (load the parameters first).  A missing buffer is zeroed and a missing
+        generator state re-seeded, as the constructor does (a reference checkpoint carries no generator)."""
+        state = state or {}
+        dev, n = self.params["positions"].device, self.n
+        accum, denom = state.get("grad_norm_accum"), state.get("grad_norm_denom")
+        if accum is None or denom is None:
+            self._reset_buffers()
+        else:
+            for name, t in (("grad_norm_accum", accum), ("grad_norm_denom", denom)):
+                if tuple(t.shape) != (n, 1):
+                    raise ValueError(f"densifier {name}: expected shape {(n, 1)}, got {tuple(t.shape)}")
+            self.grad_norm_accum = accum.detach().to(device=dev, dtype=torch.float32, copy=True).contiguous()
+            self.grad_norm_denom = denom.detach().to(device=dev, dtype=torch.int32, copy=True).contiguous()
+        load_generator(self.generator, state.get("generator"), self.conf.seed)
 
     # ---- activations of the reference model (model.py:102-118)
     def scale(self):
@@ -238,6 +268,8 @@ def compute_relocation(opacities: torch.Tensor, scales: torch.Tensor, ratios: to
 class MCMCDensifier:
     """Same contract as GSDensifier: operates on the raw parameter dict and the optimizer's moment dicts."""
 
+    METHOD = "mcmc"  # strategy.method
+
     def __init__(self, params: dict, moments: list, conf: MCMCConfig | None = None, group=None):
         import math
 
@@ -247,6 +279,14 @@ class MCMCDensifier:
         self.binoms = torch.tensor([[math.comb(n, k) if k <= n else 0 for k in range(n_max)] for n in range(n_max)], dtype=torch.float32, device=dev)
         self.generator = torch.Generator(device=dev)
         self.generator.manual_seed(int(self.conf.seed))
+
+    def state_dict(self) -> dict:
+        """The generator's state: all the strategy carries between calls (the binomial table follows from the config)."""
+        return {"generator": self.generator.get_state()}
+
+    def load_state_dict(self, state: dict | None) -> None:
+        """A missing generator state is re-seeded as the constructor does."""
+        load_generator(self.generator, (state or {}).get("generator"), self.conf.seed)
 
     @property
     def n(self) -> int:

@@ -203,11 +203,12 @@ class Background:
         self.random = self.color is None
         self.black = self.color == (0.0, 0.0, 0.0)
         self.device = device
+        self.seed = int(seed)
         self.generator = None
         self.image = None  # the latest random draw [H,W,3]
         if self.random:
             self.generator = torch.Generator(device=device)
-            self.generator.manual_seed(int(seed))
+            self.generator.manual_seed(self.seed)
 
     def draw(self, H: int, W: int):
         """None for black, the colour, or this step's random image [H,W,3] (drawn into a buffer that the next draw overwrites)."""

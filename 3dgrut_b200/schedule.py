@@ -181,6 +181,16 @@ class TrainingSchedule:
         self.step = step + 1
         return dict(self.lrs), self.sph_degree
 
+    def advance_to(self, step: int) -> "TrainingSchedule":
+        """Advance step by step up to (not including) `step`: a schedule fresh from `from_config` then holds what it holds after the
+        reference's iteration step - 1, bit for bit (a checkpoint with no schedule state resumes so).  Returns self."""
+        step = int(step)
+        if step < self.step:
+            raise ValueError(f"schedule: cannot go back from step {self.step} to step {step}")
+        for s in range(self.step, step):
+            self.advance(s)
+        return self
+
     def state_dict(self) -> dict:
         """What a resumed run needs to continue bit for bit: the step index, the SH degree, the decoder's epoch and the current rates."""
         return {"step": self.step, "sph_degree": self.sph_degree, "decoder_epoch": self.decoder_epoch, "lrs": dict(self.lrs)}

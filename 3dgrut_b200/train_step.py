@@ -21,6 +21,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+import checkpoint
 import losses
 import optimizers
 import view_parallel
@@ -169,6 +170,113 @@ class TrainStep:
         grows by itself."""
         if self.exchange.n != self.n:
             self.exchange = self._new_exchange()
+
+    # ---- checkpoints (checkpoint.py writes and reads these states in the reference's ckpt_*.pt layout)
+
+    FEATURE_TYPE = "sh"  # model.feature_type of the parameters the step trains
+    WIDTHS = optimizers.WIDTHS
+
+    def _settings(self) -> dict:
+        """The constructor arguments that are settings rather than state, as plain data.  A state records them, and load_state_dict
+        refuses a state trained with other values."""
+        bg, opt = self.background, self.optimizer
+        return {"selective": bool(opt.selective), "eps": float(opt.eps), "lambda_l1": self.lambda_l1, "lambda_ssim": self.lambda_ssim,
+                "lambda_opacity": self.lambda_opacity, "lambda_scale": self.lambda_scale,
+                "background": "random" if bg.random else [float(c) for c in bg.color], "post_processing": self.post_processing,
+                "strategy": None if self.densifier is None else self.densifier.METHOD}
+
+    def _adam_steps(self) -> dict:
+        return {k: int(self.optimizer.steps) for k in self.GROUPS}
+
+    def _load_adam_steps(self, steps: dict):
+        self.optimizer.steps = int(steps[self.GROUPS[0]])
+
+    def state_dict(self) -> dict:
+        """Everything a later `step` reads: the raw parameters, both Adam moments and the step count, frame, SH degree, scene extent and
+        rates, the densifier's buffers and generator, this rank's background generator and the schedule's state, with the settings the
+        step was built with.  The tensors are the step's own, not copies (as nn.Module.state_dict's); checkpoint.save writes them."""
+        opt, sched = self.optimizer, self.schedule
+        return {"feature_type": self.FEATURE_TYPE, "settings": self._settings(), "frame": int(self.frame), "sph_degree": int(self.sph_degree),
+                "scene_extent": float(self.scene_extent), "lrs": dict(opt.lrs),
+                "progression": None if sched is None or sched.progression is None else [int(v) for v in sched.progression],
+                "params": dict(self.params), "exp_avg": {k: opt.exp_avg[k] for k in self.GROUPS},
+                "exp_avg_sq": {k: opt.exp_avg_sq[k] for k in self.GROUPS}, "adam_steps": self._adam_steps(),
+                "densifier": None if self.densifier is None else self.densifier.state_dict(),
+                "background_generator": None if self.background.generator is None else self.background.generator.get_state(),
+                "schedule": None if sched is None else sched.state_dict()}
+
+    def _check_state(self, state: dict):
+        """Refuse (ValueError naming the key) a state this step cannot continue, before anything is changed."""
+        if state.get("feature_type", "sh") != self.FEATURE_TYPE:
+            raise ValueError(f"feature_type: the state holds {state.get('feature_type')!r} parameters, this step trains {self.FEATURE_TYPE!r}")
+        mine = self._settings()
+        for key, theirs in (state.get("settings") or {}).items():
+            if key in mine and _plain(theirs) != _plain(mine[key]):
+                raise ValueError(f"{key}: the state was trained with {theirs!r}, this step is built with {mine[key]!r} (a constructor "
+                                 f"setting, not state: build the step as the run was built)")
+        n = int(state["params"]["positions"].shape[0])
+        for k, w in zip(self.GROUPS, self.WIDTHS):
+            for what in ("params", "exp_avg", "exp_avg_sq"):
+                if tuple(state[what][k].shape) != (n, w):
+                    raise ValueError(f"{what}.{k}: expected shape {(n, w)}, got {tuple(state[what][k].shape)}")
+        checkpoint.check_step_counts(self.FEATURE_TYPE, state["adam_steps"])
+        missing = set(self.optimizer.lrs) - set(state["lrs"])
+        if missing:
+            raise ValueError(f"lrs: the state has no rate for {sorted(missing)}")
+        if self.schedule is not None and state.get("schedule") is None and self.schedule.step > int(state["frame"]):
+            raise ValueError(f"schedule: the state has no schedule and this step's is past its frame {int(state['frame'])}")
+
+    def _load_extra(self, state: dict, take):
+        """What a subclass holds beyond TrainStep's state; called after the parameters are in place."""
+
+    @torch.no_grad()
+    def load_state_dict(self, state: dict, assign: bool = False):
+        """Continue from `state` (state_dict()'s, or checkpoint.from_reference_layout's), which may hold a different N: the tensors inside
+        the shared parameter and moment dicts are replaced, as densification replaces them, and the exchange is re-capacitied.
+        assign=False copies the state's tensors; assign=True takes them as the step's own where they already are float32 on the step's
+        device (as nn.Module.load_state_dict(assign=True)), so a state read onto the device is not copied again.  A state without generator
+        states re-seeds them as the constructor does; without a schedule state, the step's schedule (fresh from from_config) is replayed to
+        the state's frame."""
+        self._check_state(state)
+
+        def take(t):
+            out = t.detach().to(device=self.device, dtype=torch.float32)
+            if not assign and out.data_ptr() == t.data_ptr():
+                out = out.clone()
+            return out.contiguous()
+
+        opt = self.optimizer
+        for k in self.GROUPS:  # the same dict objects: the optimizer and the densifier see the new tensors
+            self.params[k], opt.exp_avg[k], opt.exp_avg_sq[k] = take(state["params"][k]), take(state["exp_avg"][k]), take(state["exp_avg_sq"][k])
+        self._load_adam_steps(state["adam_steps"])
+        opt.lrs.update({k: float(state["lrs"][k]) for k in opt.lrs})
+        self.frame, self.scene_extent = int(state["frame"]), float(state["scene_extent"])
+        if self.densifier is not None:
+            self.densifier.load_state_dict(state.get("densifier"))
+        if self.background.generator is not None:
+            import densify
+
+            densify.load_generator(self.background.generator, state.get("background_generator"), self.background.seed)
+        if self.schedule is not None:
+            if state.get("schedule") is not None:
+                self.schedule.load_state_dict(state["schedule"])
+            else:
+                self.schedule.advance_to(self.frame)
+        if state.get("sph_degree") is not None:
+            self.sph_degree = int(state["sph_degree"])
+        elif self.schedule is not None:
+            self.sph_degree = self.schedule.sph_degree
+        self._load_extra(state, take)
+        self._densified()
+
+
+def _plain(v):
+    """Settings as compared: tuples as lists."""
+    if isinstance(v, (list, tuple)):
+        return [_plain(x) for x in v]
+    if isinstance(v, dict):
+        return {k: _plain(x) for k, x in v.items()}
+    return v
 
 
 class GaussianTrainStep(TrainStep):

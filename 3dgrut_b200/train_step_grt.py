@@ -62,6 +62,14 @@ class GaussianTrainStepGRT(TrainStep):
     def num_update_bvh(self) -> int:
         return self.tracer.num_update_bvh
 
+    def state_dict(self) -> dict:
+        return {**super().state_dict(), "num_update_bvh": int(self.tracer.num_update_bvh)}
+
+    def _load_extra(self, state: dict, take):
+        """The BVH cadence counter; the next build is a rebuild (_densified sets _rebuild), as after the reference's build_acc on resume."""
+        super()._load_extra(state, take)
+        self.tracer.num_update_bvh = int(state.get("num_update_bvh") or 0)
+
     def _build(self, particles):
         """Tracer.build_acc's cadence: with density clamping every build is a rebuild, otherwise the update path is taken until
         max_consecutive_bvh_update.  The native build is a full rebuild either way; num_update_bvh counts what the reference would do."""

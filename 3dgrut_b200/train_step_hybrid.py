@@ -154,6 +154,10 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         self.plane_point, self.plane_normal, self.reflectivity = m["plane_point"], m["plane_normal"], m["reflectivity"]
         super().__init__(params, lrs, conf=hybrid_render_conf(conf if conf is not None else {"render": {}}), **kw)
 
+    def _settings(self) -> dict:
+        return {**super()._settings(), "mirror": {"plane_point": [float(v) for v in self.plane_point],
+                                                  "plane_normal": [float(v) for v in self.plane_normal], "reflectivity": self.reflectivity}}
+
     def _init_renderer(self, conf):
         super()._init_renderer(conf)  # the 3DGRT tracer of the secondary rays
         self.raster = SplatRaster(conf)

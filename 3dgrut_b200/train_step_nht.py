@@ -127,6 +127,64 @@ class _NHTStep:
                             **reg)
         self.decoder.ema_update(self.frame)
 
+    # ---- checkpoints: the decoder's parameters, moments, EMA shadow, architecture and scheduler on top of TrainStep's state
+
+    FEATURE_TYPE = "nht"
+    WIDTHS = optimizers.NHT_WIDTHS
+
+    def _settings(self) -> dict:
+        return {**super()._settings(), "decoder_weight_decay": self.decoder_weight_decay, "color_refine_start": self.color_refine_start}
+
+    def _adam_steps(self) -> dict:
+        return {k: int(v) for k, v in self.optimizer.steps.items()}  # per group: colour refinement freezes the geometry's count
+
+    def _load_adam_steps(self, steps: dict):
+        missing = set(self.optimizer.GROUPS) - set(steps)
+        if missing:
+            raise ValueError(f"adam_steps: no step count for {sorted(missing)}")
+        self.optimizer.steps = {k: int(steps[k]) for k in self.optimizer.GROUPS}
+
+    def _decoder_arch(self) -> dict:
+        """Trainer.save_checkpoint's feature_decoder.arch (trainer.py:1059-1066)."""
+        d = self.decoder
+        return {"ray_feature_dim": d.ray_feature_dim, "hidden_dim": d.hidden_dim, "num_layers": d.num_layers, "sh_scale": d.sh_scale,
+                "output_activation": d.output_activation, "unpremultiply_alpha": d.unpremultiply_alpha}
+
+    def state_dict(self) -> dict:
+        state = super().state_dict()
+        opt, dec = self.optimizer, self.schedule.decoder if self.schedule is not None else None
+        if dec is None:  # a constant rate: an exponential decay by 1
+            sched = {"type": "exponential", "base_lr": float(opt.lrs["decoder"]), "gamma": 1.0}
+        elif dec.kind == "cosine":
+            sched = {"type": "cosine", "base_lr": dec.base_lr, "max_steps": dec.max_steps, "eta_min": dec.eta_min}
+        else:
+            sched = {"type": "exponential", "base_lr": dec.base_lr, "gamma": dec.gamma}
+        state["decoder"] = {"params": self.decoder.network.params.detach(), "exp_avg": opt.decoder_exp_avg, "exp_avg_sq": opt.decoder_exp_avg_sq,
+                            "ema": self.decoder.ema_state_dict(), "arch": self._decoder_arch(), "scheduler": sched}
+        return state
+
+    def _check_state(self, state: dict):
+        super()._check_state(state)
+        dec = state.get("decoder")
+        if dec is None:
+            raise ValueError("decoder: an NHT state carries the feature decoder's")
+        mine = self._decoder_arch()
+        for key, theirs in dec["arch"].items():
+            if key in mine and theirs != mine[key]:
+                raise ValueError(f"feature_decoder.arch.{key}: the state's decoder has {theirs!r}, this step's {mine[key]!r}")
+        n = self.decoder.network.params.numel()
+        for what in ("params", "exp_avg", "exp_avg_sq"):
+            if tuple(dec[what].shape) != (n,):
+                raise ValueError(f"decoder.{what}: expected the flat vector of {n} parameters, got {tuple(dec[what].shape)}")
+
+    def _load_extra(self, state: dict, take):
+        super()._load_extra(state, take)
+        dec, opt = state["decoder"], self.optimizer
+        self.decoder.network.params.data.copy_(dec["params"])  # the Parameter object stays the one the optimizer holds
+        opt.decoder_exp_avg, opt.decoder_exp_avg_sq = take(dec["exp_avg"]), take(dec["exp_avg_sq"])
+        if dec["ema"]:
+            self.decoder.load_ema_state_dict({k: v.to(self.device) for k, v in dec["ema"].items()})
+
     def _decode(self, features, dirs):
         """rgb [H*W,3] of the [H*W,24] composited features."""
         return fd.decode(features, dirs, self.decoder.network.params.data, self.decoder.config)
