@@ -96,6 +96,8 @@ SIGNATURES = {
     "gutb200_hybrid_rays": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_hybrid_composite": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp]),
     "gutb200_hybrid_composite_bwd": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),
+    "gutb200_knn_workspace_bytes": (_sz, [_i64]),
+    "gutb200_knn": (_int, [_vp, _i64, _vp, _i64, _vp, _i32, _vp, _sz, _vp, _vp]),
     "gutb200_forward_host": (_int, [_vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_backward_host": (_int, [_vp, _cam, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_last_stats": (_int, [_vp, _i64p, _i64p, _i64p, _i64p]),

@@ -37,6 +37,7 @@
 
 #include "../../include/grt_b200.h"
 #include "hit_math.cuh"
+#include "lbvh.cuh"
 #include "nht_features.cuh"
 
 namespace gutb200 {
@@ -73,22 +74,7 @@ struct __align__(16) LeafProxy {  // proxy in leaf (sorted) order: 64 B, the par
     float4 a0, a1, a2;
     uint32_t pid, pad0, pad1, pad2;
 };
-struct __align__(16) BvhNode {
-    float4 b0;    // lmin.xyz, lmax.x
-    float4 b1;    // lmax.yz, rmin.xy
-    float4 b2;    // rmin.z, rmax.xyz
-    float4 meta;  // left, right (int bits: >=0 internal, <0 leaf ~leaf index), left slack, right slack
-};
-struct __align__(16) Box {
-    float4 lo;  // min.xyz, slack (largest proxy half-diagonal below)
-    float4 hi;  // max.xyz, unused
-};
-
-__device__ __forceinline__ int float_order(float f) {  // monotone float -> int map for atomicMin/Max
-    const int i = __float_as_int(f);
-    return i >= 0 ? i : i ^ 0x7FFFFFFF;
-}
-__device__ __forceinline__ float order_float(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
+// BvhNode, Box, the scene-box reduction, Morton codes, hierarchy_kernel and refit_kernel: lbvh.cuh (shared with gut_knn.cu)
 
 // kernelScale (particlePrimitives.cu:27-51), generalized Gaussian branch
 __device__ __forceinline__ float kernel_scale(float density, float min_response, int clamping, float degree) {
@@ -171,16 +157,7 @@ __global__ void __launch_bounds__(256) proxy_kernel(int n, const float* __restri
     b.lo = make_float4(px - hx, py - hy, pz - hz, radius);
     b.hi = make_float4(px + hx, py + hy, pz + hz, 0.f);
     boxes[i] = b;
-    atomicMin(scene + 0, float_order(b.lo.x)); atomicMin(scene + 1, float_order(b.lo.y)); atomicMin(scene + 2, float_order(b.lo.z));
-    atomicMax(scene + 3, float_order(b.hi.x)); atomicMax(scene + 4, float_order(b.hi.y)); atomicMax(scene + 5, float_order(b.hi.z));
-}
-
-__device__ __forceinline__ uint32_t expand_bits(uint32_t v) {
-    v = (v * 0x00010001u) & 0xFF0000FFu;
-    v = (v * 0x00000101u) & 0x0F00F00Fu;
-    v = (v * 0x00000011u) & 0xC30C30C3u;
-    v = (v * 0x00000005u) & 0x49249249u;
-    return v;
+    scene_box_extend(scene, b.lo.x, b.lo.y, b.lo.z, b.hi.x, b.hi.y, b.hi.z);
 }
 
 // size_levels > 0: the two top bits of the key are a size class of the proxy (radius relative to the scene diagonal), so the LBVH
@@ -191,20 +168,15 @@ __global__ void __launch_bounds__(256) morton_kernel(int n, const Proxy* __restr
                                                      uint32_t* __restrict__ codes, uint32_t* __restrict__ ids) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float lx = order_float(scene[0]), ly = order_float(scene[1]), lz = order_float(scene[2]);
-    const float ex = fmaxf(order_float(scene[3]) - lx, 1e-20f), ey = fmaxf(order_float(scene[4]) - ly, 1e-20f),
-                ez = fmaxf(order_float(scene[5]) - lz, 1e-20f);
+    const SceneBox sb = scene_box(scene);
     const Proxy p = proxies[i];
-    const float ux = fminf(fmaxf((p.a0.w - lx) / ex * 1024.f, 0.f), 1023.f);
-    const float uy = fminf(fmaxf((p.a1.w - ly) / ey * 1024.f, 0.f), 1023.f);
-    const float uz = fminf(fmaxf((p.a2.w - lz) / ez * 1024.f, 0.f), 1023.f);
     uint32_t cls = 0;
     if (size_levels > 0) {
-        const float diag = sqrtf(ex * ex + ey * ey + ez * ez);
+        const float diag = sqrtf(sb.ex * sb.ex + sb.ey * sb.ey + sb.ez * sb.ez);
         const float rel = boxes[i].lo.w / diag;   // proxy radius / scene diagonal
         cls = rel < t0 ? 0u : (rel < t1 ? 1u : (rel < t2 ? 2u : 3u));
     }
-    codes[i] = (cls << 30) | (expand_bits(static_cast<uint32_t>(ux)) * 4 + expand_bits(static_cast<uint32_t>(uy)) * 2 + expand_bits(static_cast<uint32_t>(uz)));
+    codes[i] = (cls << 30) | morton30(sb, p.a0.w, p.a1.w, p.a2.w);
     ids[i] = static_cast<uint32_t>(i);
 }
 
@@ -237,82 +209,6 @@ __global__ void __launch_bounds__(256) leaf_kernel(int n, int leaf, const uint32
     leaf_codes[g] = codes_sorted[first];
     leaf_ids[g] = static_cast<uint32_t>(g);
     leaf_boxes[g] = u;
-}
-
-// common-prefix length of sorted keys i and j (index as tie breaker); -1 outside the range
-__device__ __forceinline__ int delta(const uint32_t* __restrict__ codes, int n, int i, int j) {
-    if (j < 0 || j >= n) return -1;
-    const uint32_t a = codes[i], b = codes[j];
-    if (a == b) return 32 + __clz(static_cast<uint32_t>(i) ^ static_cast<uint32_t>(j));
-    return __clz(a ^ b);
-}
-
-// Karras 2012: one thread per internal node; children are (internal index) or ~(particle id) for leaves
-__global__ void __launch_bounds__(256) hierarchy_kernel(int n, const uint32_t* __restrict__ codes, const uint32_t* __restrict__ ids,
-                                                        int2* __restrict__ children, int* __restrict__ parent,
-                                                        int* __restrict__ leaf_parent) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n - 1) return;
-    const int d = (delta(codes, n, i, i + 1) - delta(codes, n, i, i - 1)) >= 0 ? 1 : -1;
-    const int dmin = delta(codes, n, i, i - d);
-    int lmax = 2;
-    while (delta(codes, n, i, i + lmax * d) > dmin) lmax *= 2;
-    int l = 0;
-    for (int t = lmax / 2; t >= 1; t /= 2)
-        if (delta(codes, n, i, i + (l + t) * d) > dmin) l += t;
-    const int j = i + l * d;
-    const int dnode = delta(codes, n, i, j);
-    int s = 0, t = l;
-    do {
-        t = (t + 1) >> 1;
-        if (delta(codes, n, i, i + (s + t) * d) > dnode) s += t;
-    } while (t > 1);
-    const int gamma = i + s * d + min(d, 0);
-    const int lo = min(i, j), hi = max(i, j);
-    int left, right;
-    if (lo == gamma) {
-        left = ~static_cast<int>(ids[gamma]);
-        leaf_parent[gamma] = i;
-    } else {
-        left = gamma;
-        parent[gamma] = i;
-    }
-    if (hi == gamma + 1) {
-        right = ~static_cast<int>(ids[gamma + 1]);
-        leaf_parent[gamma + 1] = i;
-    } else {
-        right = gamma + 1;
-        parent[gamma + 1] = i;
-    }
-    children[i] = make_int2(left, right);
-    if (i == 0) parent[0] = -1;
-}
-
-__global__ void __launch_bounds__(256) refit_kernel(int n, const int2* __restrict__ children, const int* __restrict__ parent,
-                                                    const int* __restrict__ leaf_parent, const Box* __restrict__ leaf_boxes,
-                                                    Box* __restrict__ node_boxes, int* __restrict__ flags, BvhNode* __restrict__ nodes) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int cur = leaf_parent[i];
-    while (cur >= 0) {
-        __threadfence();
-        if (atomicAdd(flags + cur, 1) == 0) return;  // first arrival: the sibling subtree is not finished yet
-        __threadfence();
-        const int2 ch = children[cur];
-        const Box l = ch.x < 0 ? leaf_boxes[~ch.x] : node_boxes[ch.x];
-        const Box r = ch.y < 0 ? leaf_boxes[~ch.y] : node_boxes[ch.y];
-        BvhNode nd;
-        nd.b0 = make_float4(l.lo.x, l.lo.y, l.lo.z, l.hi.x);
-        nd.b1 = make_float4(l.hi.y, l.hi.z, r.lo.x, r.lo.y);
-        nd.b2 = make_float4(r.lo.z, r.hi.x, r.hi.y, r.hi.z);
-        nd.meta = make_float4(__int_as_float(ch.x), __int_as_float(ch.y), l.lo.w, r.lo.w);
-        nodes[cur] = nd;
-        Box u;
-        u.lo = make_float4(fminf(l.lo.x, r.lo.x), fminf(l.lo.y, r.lo.y), fminf(l.lo.z, r.lo.z), fmaxf(l.lo.w, r.lo.w));
-        u.hi = make_float4(fmaxf(l.hi.x, r.hi.x), fmaxf(l.hi.y, r.hi.y), fmaxf(l.hi.z, r.hi.z), 0.f);
-        node_boxes[cur] = u;
-        cur = parent[cur];
-    }
 }
 
 // one leaf: a root whose left child is the only leaf and whose right child is the point (3e38, 3e38, 3e38), which no ray segment
@@ -1220,9 +1116,7 @@ static int build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos, 
     }
     const int ni = static_cast<int>(n);
     const unsigned blocks = (ni + 255) / 256;
-    const int init[6] = {0x7F7FFFFF, 0x7F7FFFFF, 0x7F7FFFFF, static_cast<int>(0xFF7FFFFF ^ 0x7FFFFFFF), static_cast<int>(0xFF7FFFFF ^ 0x7FFFFFFF),
-                         static_cast<int>(0xFF7FFFFF ^ 0x7FFFFFFF)};  // +FLT_MAX / ordered(-FLT_MAX)
-    GRT_CUDA(c, cudaMemcpyAsync(c->scene, init, sizeof(init), cudaMemcpyHostToDevice, s));
+    GRT_CUDA(c, cudaMemcpyAsync(c->scene, kSceneBoxInit, sizeof(kSceneBoxInit), cudaMemcpyHostToDevice, s));
     if (packed)
         proxy_kernel<12, 12, 12, 12><<<blocks, 256, 0, s>>>(ni, pos, rot, scl, dns, c->cfg.min_response, c->cfg.density_clamping,
                                                             static_cast<float>(c->cfg.kernel_degree), c->cfg.primitive,

@@ -205,6 +205,18 @@ int gutb200_hybrid_composite(void* stream, int64_t pixels, const float* primary_
 int gutb200_hybrid_composite_bwd(void* stream, int64_t pixels, const float* primary_rgba, const float* secondary_rgb, const float* hit,
                                  float reflectivity, const float* d_rgb, const float* d_alpha, float* d_primary_rgba, float* d_secondary_rgb);
 
+/* Exact k nearest neighbours (ours; the initial Gaussian scales of initialization.py, DESIGN.md section 19).  targets [n_targets,3] and
+ * queries [n_queries,3] float32 device arrays; queries NULL: the targets query themselves (n_queries must equal n_targets) and query i
+ * excludes target i, and only it (duplicates are neighbours at distance 0).  Row q of out_idx [n_queries,k] int32 holds the k targets with
+ * the smallest float32 squared distance (qx-px)^2 + (qy-py)^2 + (qz-pz)^2, ascending, ties broken by the lower target index; out_dist
+ * [n_queries,k] (NULL: not written) those squared distances.  Exact and deterministic: the same inputs give the same bits on every run.
+ * No context: launches on `stream` of the current device, no synchronisation.  workspace: gutb200_knn_workspace_bytes(n_targets) device
+ * bytes (0 for n_targets outside 1..INT32_MAX).  Returns 1, with the message in gutb200_last_error(NULL), for k outside 1..4, fewer
+ * than k + 1 targets with self-exclusion or k without, sizes above INT32_MAX, a NULL array or a workspace that is too small. */
+size_t gutb200_knn_workspace_bytes(int64_t n_targets);
+int gutb200_knn(void* stream, int64_t n_targets, const float* targets, int64_t n_queries, const float* queries, int32_t k, void* workspace,
+                size_t workspace_bytes, int32_t* out_idx, float* out_dist);
+
 int gutb200_forward_host(gutb200_ctx* ctx, const gutb200_camera* cam, int64_t n, const float* particles,
                          const float* sph, int32_t sph_degree, const float* rays_o, const float* rays_d,
                          float* out_rgba, float* out_dist, float* out_hits, float* visibility);
