@@ -89,10 +89,7 @@ SIGNATURES = {
     "gutb200_nht_adam_step": (_int, [_vp, _i64, _i64, _vpp, _vpp, _vpp, _f32p, _i64p, _f32, _f32, _f32, _i32, _f32, _f32, _f32, _f32, _i32,
                                      _vp, _vp, _vp, _vp, _f32, _f32]),
     "gutb200_image_loss_scratch_bytes": (_sz, [_i32, _i32]),
-    "gutb200_image_loss": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
-    "gutb200_image_loss_rgb": (_int, [_vp, _i32, _i32, _vp, _vp, _f32, _f32, _vp, _vp, _vp]),
-    "gutb200_image_loss_composited": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp]),
-    "gutb200_image_loss_postprocessed": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp, _i32]),
+    "gutb200_image_loss": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp, _i32]),
     "gutb200_hybrid_rays": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_hybrid_composite": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp]),
     "gutb200_hybrid_composite_bwd": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),

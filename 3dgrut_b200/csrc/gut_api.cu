@@ -325,7 +325,7 @@ void drain_timers(gutb200_ctx* c) {
 
 namespace gutb200 {
 
-// The message of the last failed call that takes no context (gutb200_image_loss_postprocessed), per host thread.
+// The message of the last failed call that takes no context (gutb200_image_loss), per host thread.
 static thread_local std::string g_context_free_error;
 
 void set_context_free_error(const std::string& msg) { g_context_free_error = msg; }

@@ -12,25 +12,29 @@
 //                       d loss / d map (stored [H,W,9])
 //   loss_grad_kernel    convolves those maps and assembles d loss / d x, written as [H,W,4] with a zero alpha gradient -- directly the
 //                       d_rgba argument of gutb200_backward.
-// Both are templated on the pixel strides of the prediction and the gradient, so that gutb200_image_loss_rgb runs the same arithmetic on
-// the 3DGRT layout (rgb [H,W,3] in, d_rgb [H,W,3] out, directly the d_rgb argument of grtb200_trace_bwd).
+// Both are templated on the pixel strides of the prediction and the gradient, so that layout 3 of gutb200_image_loss runs the same
+// arithmetic on the 3DGRT layout (rgb [H,W,3] in, d_rgb [H,W,3] out, directly the d_rgb argument of grtb200_trace_bwd).
 //
-// gutb200_image_loss_composited adds the two image-side parts of the training loss (threedgrut/model/background.py:80-93,
+// A background and a mask add the two image-side parts of the training loss (threedgrut/model/background.py:80-93,
 // trainer.py:691-694) where the kernels load x and y, and their chain rule where loss_grad_kernel writes:
 //     x = (rgb + bg (1 - alpha)) m,  y = target m          bg: constant colour or [H,W,3] image; m: optional [H,W] mask
 //     d rgb_c = m dL/dx_c,  d alpha = -sum_c bg_c m dL/dx_c
 // The background mode (BG) and the mask (MASK) are template parameters beside the strides; BG = 0 (black) with no mask is the plain loss.
 //
-// gutb200_image_loss_postprocessed adds the reference's `post_processing.method: linear-to-srgb` (threedgrut/utils/
+// post_processing = 1 adds the reference's `post_processing.method: linear-to-srgb` (threedgrut/utils/
 // post_processing_linear_to_srgb.py, applied after the background and before the loss, trainer.py:1165-1172) as a third template
 // parameter, POST (0 none, 1 linear-to-sRGB), between the composite and the mask:
 //     x = s(c) m,  c = rgb + bg (1 - alpha),   s(c) = 1.055 max(c, 1e-8)^(1/2.4) - 0.055 if c > 0.0031308, else 12.92 c   (no clamp: HDR)
 //     d rgb_c = m s'(c_c) dL/dx_c,  d alpha = -sum_c bg_c m s'(c_c) dL/dx_c
 // POST = 0 compiles every existing instantiation to the code it had without this parameter.
+//
+// The one C entry point, gutb200_image_loss, turns (layout, background mode, mask, post-processing) into those template arguments in one
+// dispatch: 2 x 3 x 2 x 2 instantiations of each kernel.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <string>
+#include <type_traits>
 
 #include "../../include/gut_b200.h"
 
@@ -49,7 +53,7 @@ struct Window {
     float w[11];
 };
 
-// Extra inputs and outputs of the composited loss; unused (all null) by the plain entries.
+// Extra inputs and outputs of the composited loss; unread by the plain kernels.
 struct Composite {
     const float* alpha;     // [H,W]: the prediction's alpha when it is not channel 3 of the prediction (PS == 3)
     const float* bg_image;  // [H,W,3] background (BG == 2)
@@ -192,7 +196,7 @@ __global__ void __launch_bounds__(kT * kT) ssim_stats_kernel(int H, int W, const
 }
 
 // GS: floats per pixel of the gradient (4: d_rgba, one 16-byte store, its alpha gradient zero unless BG != 0; 3: d_rgb, plus cp.d_alpha
-// in the composited entry).
+// in the composited instantiations).
 template <int PS, int GS, int BG = 0, bool MASK = false, int POST = 0>
 __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const float* __restrict__ pred_rgba, const float* __restrict__ target,
                                                             Composite cp, Window win, float l1_scale /* lambda_l1 / (H W 3) */,
@@ -276,9 +280,9 @@ __global__ void __launch_bounds__(kT * kT) loss_grad_kernel(int H, int W, const 
     }
 }
 
-template <int PS, int GS, int BG = 0, bool MASK = false, int POST = 0>
-int image_loss(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1, float lambda_ssim,
-               void* scratch, float* d_pred, float* sums2, Composite cp = Composite{}) {
+template <int PS, int GS, int BG, bool MASK, int POST>
+cudaError_t image_loss(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1,
+                       float lambda_ssim, void* scratch, float* d_pred, float* sums2, Composite cp) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     Window win;
     double g[11], total = 0.0;
@@ -291,55 +295,34 @@ int image_loss(void* stream, int32_t height, int32_t width, const float* pred, c
     const double count = (height > 10 && width > 10) ? static_cast<double>(height - 10) * (width - 10) * 3.0 : 1.0;
     const dim3 block(kT, kT), grid((width + kT - 1) / kT, (height + kT - 1) / kT);
     float* dmaps = static_cast<float*>(scratch);
+    cudaError_t e;
     if constexpr (BG != 0 || MASK || POST != 0) {
         // the composited kernels keep their two sums in fp64 at the head of the scratch (its 16 spare bytes), the maps after them
         cp.acc = static_cast<double*>(scratch);
         cp.sums = sums2;
         dmaps = reinterpret_cast<float*>(static_cast<char*>(scratch) + 16);
-        if (cudaMemsetAsync(cp.acc, 0, 2 * sizeof(double), s) != cudaSuccess) return 2;
+        e = cudaMemsetAsync(cp.acc, 0, 2 * sizeof(double), s);
     } else {
-        if (cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s) != cudaSuccess) return 2;
+        e = cudaMemsetAsync(sums2, 0, 2 * sizeof(float), s);
+        // the plain kernels write no alpha gradient: on the split layout it is zero
+        if (e == cudaSuccess && GS == 3 && cp.d_alpha) e = cudaMemsetAsync(cp.d_alpha, 0, static_cast<size_t>(height) * width * sizeof(float), s);
     }
+    if (e != cudaSuccess) return e;
     ssim_stats_kernel<PS, BG, MASK, POST><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win,
                                                                  static_cast<float>(-lambda_ssim / count), dmaps, sums2);
     loss_grad_kernel<PS, GS, BG, MASK, POST><<<grid, block, 0, s>>>(height, width, pred, target_rgb, cp, win,
                                                                     static_cast<float>(lambda_l1 / (static_cast<double>(height) * width * 3.0)),
                                                                     dmaps, d_pred);
-    return cudaGetLastError() == cudaSuccess ? 0 : 2;
+    return cudaGetLastError();
 }
 
-template <int L>
-int image_loss_composited(void* stream, int32_t height, int32_t width, const float* pred, const float* target_rgb, float lambda_l1,
-                          float lambda_ssim, void* scratch, float* d_pred, float* sums2, const Composite& cp, int bg_mode, bool mask,
-                          int post = 0) {
-    if (post == 1) {
-        // every background and mask goes through the post-processed kernels (a black, unmasked one too: the encode is not the identity)
-#define GUT_LOSS_POST_CASE(BG_, M_) \
-    if (bg_mode == BG_ && mask == M_) return image_loss<L, L, BG_, M_, 1>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp);
-        GUT_LOSS_POST_CASE(0, false)
-        GUT_LOSS_POST_CASE(0, true)
-        GUT_LOSS_POST_CASE(1, false)
-        GUT_LOSS_POST_CASE(1, true)
-        GUT_LOSS_POST_CASE(2, false)
-        GUT_LOSS_POST_CASE(2, true)
-#undef GUT_LOSS_POST_CASE
-        return 1;
-    }
-    if (bg_mode == 0 && !mask) {
-        // black, no mask: the plain loss; the split layout's alpha gradient is zero
-        if (L == 3 && cudaMemsetAsync(cp.d_alpha, 0, static_cast<size_t>(height) * width * sizeof(float), static_cast<cudaStream_t>(stream)) != cudaSuccess)
-            return 2;
-        return image_loss<L, L>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2);
-    }
-#define GUT_LOSS_CASE(BG_, M_) \
-    if (bg_mode == BG_ && mask == M_) return image_loss<L, L, BG_, M_>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp);
-    GUT_LOSS_CASE(0, true)
-    GUT_LOSS_CASE(1, false)
-    GUT_LOSS_CASE(1, true)
-    GUT_LOSS_CASE(2, false)
-    GUT_LOSS_CASE(2, true)
-#undef GUT_LOSS_CASE
-    return 1;
+// The runtime value v in [0, N) as a template argument: f(std::integral_constant<int, v>()), as grt.cu's with_kind does.
+template <int N, class F>
+cudaError_t with_value(int v, F&& f) {
+    if constexpr (N == 1)
+        return f(std::integral_constant<int, 0>());
+    else
+        return v == N - 1 ? f(std::integral_constant<int, N - 1>()) : with_value<N - 1>(v, f);
 }
 
 }  // namespace
@@ -352,37 +335,23 @@ size_t gutb200_image_loss_scratch_bytes(int32_t height, int32_t width) {
     return static_cast<size_t>(height) * static_cast<size_t>(width) * 9 * sizeof(float) + 16;
 }
 
-int gutb200_image_loss(void* stream, int32_t height, int32_t width, const float* pred_rgba, const float* target_rgb, float lambda_l1,
-                       float lambda_ssim, void* scratch, float* d_rgba, float* sums2) {
-    if (height <= 0 || width <= 0 || !pred_rgba || !target_rgb || !scratch || !d_rgba || !sums2) return 1;
-    if ((reinterpret_cast<uintptr_t>(d_rgba) & 15) != 0) return 3;
-    return gutb200::image_loss<4, 4>(stream, height, width, pred_rgba, target_rgb, lambda_l1, lambda_ssim, scratch, d_rgba, sums2);
-}
-
-// The same loss on the 3DGRT layout: prediction rgb [H,W,3] (alpha is a separate output there and takes no part), gradient d_rgb [H,W,3].
-int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const float* pred_rgb, const float* target_rgb, float lambda_l1,
-                           float lambda_ssim, void* scratch, float* d_rgb, float* sums2) {
-    if (height <= 0 || width <= 0 || !pred_rgb || !target_rgb || !scratch || !d_rgb || !sums2) return 1;
-    return gutb200::image_loss<3, 3>(stream, height, width, pred_rgb, target_rgb, lambda_l1, lambda_ssim, scratch, d_rgb, sums2);
-}
-
-// The loss on the composited, masked prediction (see the top of this file), for either layout:
-//   layout 4: pred [H,W,4] rgba, d_pred [H,W,4] = d_rgba with its alpha gradient (16-byte aligned); pred_alpha / d_alpha unused
-//   layout 3: pred [H,W,3] rgb + pred_alpha [H,W], d_pred [H,W,3] = d_rgb + d_alpha [H,W]
-// background_rgb: 3 host floats, or NULL (black); background_image: [H,W,3] device image (takes precedence), or NULL.  A black background
-// is skipped entirely: no alpha gradient.  mask: [H,W] device floats, or NULL.
-static int image_loss_entry(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
-                            const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
-                            float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2, int post) {
-    if (height <= 0 || width <= 0 || !pred || !target_rgb || !scratch || !d_pred || !sums2) return 1;
-    if (layout != 3 && layout != 4) return 1;
-    if (layout == 3 && (!pred_alpha || !d_alpha)) return 1;
-    if (layout == 4 && (reinterpret_cast<uintptr_t>(d_pred) & 15) != 0) return 3;
+int gutb200_image_loss(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                       const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                       float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2, int32_t post_processing) {
+    const auto fail = [](int rc, const std::string& why) {
+        gutb200::set_context_free_error("gutb200_image_loss: " + why);
+        return rc;
+    };
+    if (height <= 0 || width <= 0 || !pred || !target_rgb || !scratch || !d_pred || !sums2)
+        return fail(1, "needs a positive height and width and non-null pred, target_rgb, scratch, d_pred and sums2");
+    if (layout != 3 && layout != 4) return fail(1, "layout=" + std::to_string(layout) + " (3 = rgb + alpha, 4 = rgba)");
+    if (post_processing != 0 && post_processing != 1)
+        return fail(1, "post_processing=" + std::to_string(post_processing) + " is not built (0 = none, 1 = linear-to-sRGB)");
     gutb200::Composite cp{};
     cp.alpha = pred_alpha;
     cp.d_alpha = d_alpha;
     cp.mask = mask;
-    int bg_mode = 0;
+    int bg_mode = 0;  // a black background is skipped entirely: no alpha gradient
     if (background_image) {
         cp.bg_image = background_image;
         bg_mode = 2;
@@ -390,34 +359,22 @@ static int image_loss_entry(void* stream, int32_t height, int32_t width, int32_t
         for (int c = 0; c < 3; ++c) cp.bg[c] = background_rgb[c];
         bg_mode = 1;
     }
-    if (layout == 4)
-        return gutb200::image_loss_composited<4>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp,
-                                                 bg_mode, mask != nullptr, post);
-    return gutb200::image_loss_composited<3>(stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp, bg_mode,
-                                             mask != nullptr, post);
-}
-
-int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
-                                  const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
-                                  float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2) {
-    return image_loss_entry(stream, height, width, layout, pred, pred_alpha, target_rgb, background_rgb, background_image, mask, lambda_l1,
-                            lambda_ssim, scratch, d_pred, d_alpha, sums2, 0);
-}
-
-// The composited loss with the post-processing of the reference trainer applied after the background and before the mask:
-// post_processing 0 = none (gutb200_image_loss_composited itself), 1 = linear-to-sRGB.  Any other value returns 1 and names itself in
-// gutb200_last_error(NULL).
-int gutb200_image_loss_postprocessed(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
-                                     const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
-                                     float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2,
-                                     int32_t post_processing) {
-    if (post_processing != 0 && post_processing != 1) {
-        gutb200::set_context_free_error("gutb200_image_loss_postprocessed: post_processing=" + std::to_string(post_processing) +
-                                        " is not built (0 = none, 1 = linear-to-sRGB)");
-        return 1;
-    }
-    return image_loss_entry(stream, height, width, layout, pred, pred_alpha, target_rgb, background_rgb, background_image, mask, lambda_l1,
-                            lambda_ssim, scratch, d_pred, d_alpha, sums2, post_processing);
+    if (layout == 3 && bg_mode != 0 && !pred_alpha) return fail(1, "layout 3 with a background needs pred_alpha");
+    if (layout == 3 && (bg_mode != 0 || mask || post_processing != 0) && !d_alpha)
+        return fail(1, "layout 3 with a background, a mask or post-processing needs d_alpha");
+    if (layout == 4 && (reinterpret_cast<uintptr_t>(d_pred) & 15) != 0) return fail(3, "layout 4 stores d_pred 16 bytes at a time: align it");
+    const cudaError_t e = gutb200::with_value<2>(layout == 4, [&](auto wide) {
+        return gutb200::with_value<3>(bg_mode, [&](auto bg) {
+            return gutb200::with_value<2>(mask != nullptr, [&](auto masked) {
+                return gutb200::with_value<2>(post_processing, [&](auto post) {
+                    constexpr int L = decltype(wide)::value ? 4 : 3;
+                    return gutb200::image_loss<L, L, decltype(bg)::value, decltype(masked)::value != 0, decltype(post)::value>(
+                        stream, height, width, pred, target_rgb, lambda_l1, lambda_ssim, scratch, d_pred, sums2, cp);
+                });
+            });
+        });
+    });
+    return e == cudaSuccess ? 0 : fail(2, cudaGetErrorString(e));
 }
 
 }  // extern "C"

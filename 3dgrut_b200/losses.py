@@ -1,17 +1,18 @@
 """Image loss of the training step on the GPU (SURVEY.md section 8f row 3): lambda_l1 * L1 + lambda_ssim * (1 - SSIM) and its gradient
-w.r.t. the rendered image in two launches (csrc/gut_loss.cu), replacing l1_loss + fused_ssim + their autograd
-(threedgrut/model/losses.py:20-33, trainer.py:698-739).  The gradient comes out as [H,W,4] with a zero alpha gradient, i.e. directly the
-`ray_radiance_density_grd` / d_rgba argument of SplatRaster.trace_bwd; image_loss_rgb takes and returns the 3DGRT layout (rgb [H,W,3]).
+w.r.t. the rendered image in two launches of one C entry point (gutb200_image_loss, csrc/gut_loss.cu), replacing l1_loss + fused_ssim +
+their autograd (threedgrut/model/losses.py:20-33, trainer.py:698-739).  The gradient comes out as [H,W,4] with a zero alpha gradient, i.e.
+directly the `ray_radiance_density_grd` / d_rgba argument of SplatRaster.trace_bwd; image_loss_rgb takes and returns the 3DGRT layout (rgb
+[H,W,3]).
 
 With `background=` and / or `mask=`, the loss is taken on the prediction composited onto the background and multiplied by the mask, as the
-reference trainer does (model/background.py:80-93, trainer.py:691-694), in the same two launches (gutb200_image_loss_composited): the
-gradient then has a live alpha part.  image_loss_rgb_alpha is that loss on the 3DGRT layout (rgb and alpha as separate tensors).
+reference trainer does (model/background.py:80-93, trainer.py:691-694), in the same two launches: the gradient then has a live alpha part.
+image_loss_rgb_alpha is that loss on the 3DGRT layout (rgb and alpha as separate tensors).
 `Background` and `mask_hw` resolve the training steps' `background=` / `mask=` arguments.
 
 With `post_processing="linear-to-srgb"` (the reference's post_processing.method, configs/base_gs.yaml:188-197), the composited prediction is
 encoded to sRGB before the mask and the loss (threedgrut/utils/post_processing_linear_to_srgb.py, trainer.py:1165-1172), still in the same
-two launches (gutb200_image_loss_postprocessed): use it when the ground-truth images are display-referred sRGB and the renderer outputs
-linear radiance.  `linear_to_srgb` is that encode for rendered images outside the loss.  No CPU fallback."""
+two launches: use it when the ground-truth images are display-referred sRGB and the renderer outputs linear radiance.  `linear_to_srgb` is
+that encode for rendered images outside the loss.  No CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -22,7 +23,7 @@ import b200_native as native
 
 _scratch = {}
 
-POST_PROCESSING = {None: 0, "linear-to-srgb": 1}  # post_processing.method -> the post_processing code of gutb200_image_loss_postprocessed
+POST_PROCESSING = {None: 0, "linear-to-srgb": 1}  # post_processing.method -> the post_processing code of gutb200_image_loss
 
 
 def post_processing_code(method) -> int:
@@ -60,30 +61,11 @@ def _scalars(sums, H, W, lambda_l1, lambda_ssim):
     return loss, l1, ssim
 
 
-def _run(entry, pred, tgt, ch_pred, lambda_l1, lambda_ssim, d_pred, name):
-    for t, w, ch in ((pred, name, ch_pred), (tgt, "target_rgb", 3)):
-        _check_image(t, w, ch)
-    H, W = int(pred.shape[0]), int(pred.shape[1])
-    if tuple(tgt.shape[:2]) != (H, W):
-        raise RuntimeError("prediction and target resolutions differ")
-    dev = pred.device
-    lib = native.load()
-    scratch = _scratch_for(lib, dev, H, W)
-    if d_pred is None:
-        d_pred = torch.empty((H, W, ch_pred), dtype=torch.float32, device=dev)
-    sums = torch.empty(2, dtype=torch.float32, device=dev)
-    stream = torch.cuda.current_stream(dev).cuda_stream
-    with torch.cuda.device(dev):
-        rc = getattr(lib, entry)(stream, H, W, pred.data_ptr(), tgt.data_ptr(), float(lambda_l1), float(lambda_ssim), scratch.data_ptr(),
-                                 d_pred.data_ptr(), sums.data_ptr())
-    if rc != 0:
-        raise RuntimeError(f"{entry} failed ({rc})")
-    return (*_scalars(sums, H, W, lambda_l1, lambda_ssim), d_pred)
-
-
-def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background, mask, d_pred, d_alpha, post=0):
-    """gutb200_image_loss_composited, or gutb200_image_loss_postprocessed with post != 0.  background: None (black), 3 floats, or a float32
-    CUDA image [H,W,3]; mask: None or [H,W]."""
+def _run(layout, pred, tgt, lambda_l1, lambda_ssim, d_pred, alpha=None, d_alpha=None, background=None, mask=None, post=0):
+    """One call of gutb200_image_loss.  layout 4: pred [H,W,4]; layout 3: pred [H,W,3] and alpha [H,W,1] or None (image_loss_rgb: black and
+    unmasked, the alpha is never read).  background: None (black), 3 floats, or a float32 CUDA image [H,W,3]; mask: None or as mask_hw.
+    Returns (loss, l1, ssim, d_pred, d_alpha); layout 3 allocates d_alpha [H,W,1] when it is None and alpha is given (it is returned) or the
+    post-processing writes it."""
     _check_image(pred, "pred_rgba" if layout == 4 else "pred_rgb", layout)
     _check_image(tgt, "target_rgb", 3)
     H, W = int(pred.shape[0]), int(pred.shape[1])
@@ -96,6 +78,7 @@ def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background
         _check_image(bg_img, "background", 3)
         if tuple(bg_img.shape[:2]) != (H, W) or bg_img.device != dev:
             raise RuntimeError("background image: expected [H,W,3] on the prediction's device")
+        bg_img = bg_img.data_ptr()
     elif background is not None:
         rgb = [float(v) for v in background]
         if len(rgb) != 3:
@@ -109,18 +92,16 @@ def _run_composited(layout, pred, alpha, tgt, lambda_l1, lambda_ssim, background
     scratch = _scratch_for(lib, dev, H, W)
     if d_pred is None:
         d_pred = torch.empty((H, W, layout), dtype=torch.float32, device=dev)
-    if layout == 3 and d_alpha is None:
+    if layout == 3 and d_alpha is None and (alpha is not None or post):
         d_alpha = torch.empty((H, W, 1), dtype=torch.float32, device=dev)
     sums = torch.empty(2, dtype=torch.float32, device=dev)
     stream = torch.cuda.current_stream(dev).cuda_stream
-    ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-    args = (stream, H, W, layout, pred.data_ptr(), ptr(alpha), tgt.data_ptr(), bg_rgb, ptr(bg_img), ptr(mask), float(lambda_l1),
-            float(lambda_ssim), scratch.data_ptr(), d_pred.data_ptr(), ptr(d_alpha), sums.data_ptr())
-    entry = "gutb200_image_loss_postprocessed" if post else "gutb200_image_loss_composited"
     with torch.cuda.device(dev):
-        rc = lib.gutb200_image_loss_postprocessed(*args, post) if post else lib.gutb200_image_loss_composited(*args)
+        rc = lib.gutb200_image_loss(stream, H, W, layout, pred.data_ptr(), None if alpha is None else alpha.data_ptr(), tgt.data_ptr(), bg_rgb,
+                                    bg_img, None if mask is None else mask.data_ptr(), float(lambda_l1), float(lambda_ssim), scratch.data_ptr(),
+                                    d_pred.data_ptr(), None if d_alpha is None else d_alpha.data_ptr(), sums.data_ptr(), post)
     if rc != 0:
-        raise RuntimeError(f"{entry} failed ({rc})")
+        raise RuntimeError(f"gutb200_image_loss failed ({rc}): {lib.gutb200_last_error(None).decode()}")
     return (*_scalars(sums, H, W, lambda_l1, lambda_ssim), d_pred, d_alpha)
 
 
@@ -134,11 +115,7 @@ def image_loss(pred_rgba: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: flo
     post = post_processing_code(post_processing)
     pred = pred_rgba.reshape(pred_rgba.shape[-3:])
     tgt = target_rgb.reshape(target_rgb.shape[-3:])
-    if post:
-        return _run_composited(4, pred, None, tgt, lambda_l1, lambda_ssim, background, mask, d_rgba, None, post)[:4]
-    if background is None and mask is None:
-        return _run("gutb200_image_loss", pred, tgt, 4, lambda_l1, lambda_ssim, d_rgba, "pred_rgba")
-    return _run_composited(4, pred, None, tgt, lambda_l1, lambda_ssim, background, mask, d_rgba, None)[:4]
+    return _run(4, pred, tgt, lambda_l1, lambda_ssim, d_rgba, background=background, mask=mask, post=post)[:4]
 
 
 def image_loss_rgb(pred_rgb: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: float = 0.8, lambda_ssim: float = 0.2, d_rgb: torch.Tensor | None = None,
@@ -149,12 +126,7 @@ def image_loss_rgb(pred_rgb: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: 
     post = post_processing_code(post_processing)
     pred = pred_rgb.reshape(pred_rgb.shape[-3:])
     tgt = target_rgb.reshape(target_rgb.shape[-3:])
-    if post:
-        # black and unmasked: the alpha is never read and its gradient is zero, but the split layout takes both
-        H, W = int(pred.shape[0]), int(pred.shape[1])
-        alpha = torch.zeros((H, W, 1), dtype=torch.float32, device=pred.device)
-        return _run_composited(3, pred, alpha, tgt, lambda_l1, lambda_ssim, None, None, d_rgb, None, post)[:4]
-    return _run("gutb200_image_loss_rgb", pred, tgt, 3, lambda_l1, lambda_ssim, d_rgb, "pred_rgb")
+    return _run(3, pred, tgt, lambda_l1, lambda_ssim, d_rgb, post=post)[:4]
 
 
 def image_loss_rgb_alpha(pred_rgb: torch.Tensor, pred_alpha: torch.Tensor, target_rgb: torch.Tensor, lambda_l1: float = 0.8,
@@ -171,7 +143,7 @@ def image_loss_rgb_alpha(pred_rgb: torch.Tensor, pred_alpha: torch.Tensor, targe
     if not (isinstance(pred_alpha, torch.Tensor) and pred_alpha.is_cuda and pred_alpha.dtype == torch.float32 and pred_alpha.is_contiguous()
             and pred_alpha.numel() == H * W and pred_alpha.shape[-1] == 1):
         raise RuntimeError("pred_alpha: expected a contiguous float32 CUDA tensor [H,W,1] (there is no CPU fallback)")
-    return _run_composited(3, pred, pred_alpha, tgt, lambda_l1, lambda_ssim, background, mask, d_rgb, d_alpha, post)
+    return _run(3, pred, tgt, lambda_l1, lambda_ssim, d_rgb, alpha=pred_alpha, d_alpha=d_alpha, background=background, mask=mask, post=post)
 
 
 def mask_hw(mask: torch.Tensor, H: int, W: int) -> torch.Tensor:

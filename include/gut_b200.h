@@ -22,7 +22,7 @@
  *   d_particles [N,12], d_sph [N,48]                                  (src/splatRaster.cpp:291-293)
  * Errors: every call returns 0 on success, non-zero on failure; gutb200_last_error() gives the message
  * (the reference logs and drops its Status codes, src/splatRaster.cpp:242,254; we surface them).  Given NULL, it gives the message of
- * the last failed call on this thread that takes no context and records one (gutb200_image_loss_postprocessed), else "null context".
+ * the last failed call on this thread that takes no context and records one (gutb200_image_loss), else "null context".
  */
 #ifndef GUT_B200_H
 #define GUT_B200_H
@@ -157,36 +157,25 @@ int gutb200_nht_adam_step(void* stream, int64_t n, int64_t n_decoder, float* con
                           float reg_scale);
 
 /* Image loss of the training step and its gradient (SURVEY.md 8f row 3): loss = lambda_l1 mean|x - y| + lambda_ssim (1 - SSIM(x, y))
- * (threedgrut/trainer.py:698-739, model/losses.py:20-33 -> fused_ssim(..., padding="valid"), third-party fused-ssim @ 1272e21).
- * pred_rgba [H,W,4] (the renderer's output, channels 0..2 are used), target_rgb [H,W,3], d_rgba [H,W,4] = d loss / d pred with a zero
- * alpha gradient (directly the d_rgba of gutb200_backward), sums2 [2] device floats = (sum |x - y|, sum of the SSIM map over the valid
- * region): l1 = sums2[0] / (3 H W), ssim = sums2[1] / (3 (H-10) (W-10)).  scratch: gutb200_image_loss_scratch_bytes(H, W) device bytes. */
+ * (threedgrut/trainer.py:698-739, model/losses.py:20-33 -> fused_ssim(..., padding="valid"), third-party fused-ssim @ 1272e21), on the
+ * prediction composited onto a background, post-processed and multiplied by a mask (model/background.py:80-93, trainer.py:691-694,
+ * 1165-1172): x = s(c) m, c = rgb + bg (1 - alpha), y = target m; d rgb = m s'(c) dL/dx, d alpha = -sum_c bg_c m s'(c_c) dL/dx_c.
+ * layout 4: pred [H,W,4] rgba (the renderer's output) and d_pred [H,W,4] = d_rgba, 16-byte aligned (directly the d_rgba of
+ * gutb200_backward); pred_alpha / d_alpha unused.  layout 3: pred [H,W,3] rgb + pred_alpha [H,W] and d_pred [H,W,3] = d_rgb + d_alpha
+ * [H,W] (grtb200_trace's out_rgb / out_alpha and the d_rgb / d_alpha of grtb200_trace_bwd); pred_alpha is needed only with a background,
+ * d_alpha only with a background, a mask or post-processing (otherwise it is zeroed when given).  background_rgb: 3 host floats or NULL
+ * (black); background_image: [H,W,3] device floats or NULL (used instead of background_rgb).  mask: [H,W] device floats or NULL.
+ * post_processing (post_processing.method, threedgrut/utils/post_processing_linear_to_srgb.py): 0 = none (s = identity), 1 =
+ * linear-to-sRGB, s(c) = 1.055 max(c, 1e-8)^(1/2.4) - 0.055 above c = 0.0031308, 12.92 c at or below it (no clamp).
+ * A black background with no mask and no post-processing is the plain loss: zero alpha gradient, and layout 3's rgb gradient is
+ * bit-identical to layout 4's on the [H,W,4] concatenation of rgb and alpha.
+ * sums2 [2] device floats = (sum |x - y|, sum of the SSIM map over the valid region): l1 = sums2[0] / (3 H W), ssim = sums2[1] / (3 (H-10)
+ * (W-10)).  scratch: gutb200_image_loss_scratch_bytes(H, W) device bytes.  Two launches on `stream`; returns 0, 1 for bad arguments, 3 for
+ * a misaligned d_pred (layout 4), 2 for a launch error, and gutb200_last_error(NULL) then names the cause. */
 size_t gutb200_image_loss_scratch_bytes(int32_t height, int32_t width);
-int gutb200_image_loss(void* stream, int32_t height, int32_t width, const float* pred_rgba, const float* target_rgb, float lambda_l1,
-                       float lambda_ssim, void* scratch, float* d_rgba, float* sums2);
-/* The same loss on the 3DGRT layout: pred_rgb [H,W,3] (grtb200_trace's out_rgb; alpha takes no part), d_rgb [H,W,3] (directly the d_rgb
- * of grtb200_trace_bwd).  sums2, the rgb gradient and the scratch contents are bit-identical to gutb200_image_loss on the [H,W,4]
- * concatenation of rgb and alpha. */
-int gutb200_image_loss_rgb(void* stream, int32_t height, int32_t width, const float* pred_rgb, const float* target_rgb, float lambda_l1,
-                           float lambda_ssim, void* scratch, float* d_rgb, float* sums2);
-/* The loss on the prediction composited onto a background and multiplied by a mask (threedgrut/model/background.py:80-93,
- * trainer.py:691-694): x = (rgb + bg (1 - alpha)) m, y = target m.  layout 4: pred [H,W,4] rgba and d_pred [H,W,4] = d_rgba with a live
- * alpha gradient (16-byte aligned; pred_alpha / d_alpha unused); layout 3: pred [H,W,3] rgb + pred_alpha [H,W] and d_pred [H,W,3] = d_rgb
- * + d_alpha [H,W] (the d_rgb / d_alpha of grtb200_trace_bwd).  background_rgb: 3 host floats or NULL (black); background_image: [H,W,3]
- * device floats or NULL (used instead of background_rgb when given); black is skipped (zero alpha gradient).  mask: [H,W] or NULL.
- * d rgb = m dL/dx, d alpha = -sum_c bg_c m dL/dx_c.  Black with no mask runs gutb200_image_loss / _rgb's kernels. */
-int gutb200_image_loss_composited(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
-                                  const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
-                                  float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2);
-/* gutb200_image_loss_composited with the reference trainer's post-processing (post_processing.method, threedgrut/utils/
- * post_processing_linear_to_srgb.py) applied after the background and before the mask: post_processing 0 = none (the composited entry
- * itself), 1 = linear-to-sRGB: x = s(c) m with c = rgb + bg (1 - alpha), s(c) = 1.055 max(c, 1e-8)^(1/2.4) - 0.055 above c = 0.0031308,
- * 12.92 c at or below it (no clamp); d rgb = m s'(c) dL/dx, d alpha = -sum_c bg_c m s'(c_c) dL/dx_c.  Any other value returns 1, and
- * gutb200_last_error(NULL) names it. */
-int gutb200_image_loss_postprocessed(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
-                                     const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
-                                     float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2,
-                                     int32_t post_processing);
+int gutb200_image_loss(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                       const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
+                       float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2, int32_t post_processing);
 
 /* 3DGRUT hybrid (ours; hybrid.py's mirror_rays and render_hybrid as device code for train_step_hybrid): primary rays through 3DGUT, one
  * mirror bounce off a plane through 3DGRT.  No context: one launch each on `stream` of the current device, no synchronisation; 0 on success.

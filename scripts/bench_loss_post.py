@@ -1,8 +1,8 @@
 """Device time of the image loss with and without the linear-to-sRGB post-processing (post_processing.method: linear-to-srgb), alternating
 in one process, at 800x800 and 1237x822 (0.8 L1 + 0.2 (1 - SSIM), white background + a 0/1 mask), per layout:
 
-    rgba    gutb200_image_loss_composited   vs  gutb200_image_loss_postprocessed(linear-to-sRGB)
-    split   gutb200_image_loss_composited   vs  gutb200_image_loss_postprocessed(linear-to-sRGB)    (d_rgb + d_alpha)
+    rgba    gutb200_image_loss, layout 4, post_processing 0   vs  post_processing 1 (linear-to-sRGB)
+    split   gutb200_image_loss, layout 3, post_processing 0   vs  post_processing 1 (linear-to-sRGB)    (d_rgb + d_alpha)
 
     python scripts/bench_loss_post.py [--reps 200] [--rounds 5]
 

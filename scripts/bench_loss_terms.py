@@ -1,9 +1,9 @@
 """Device time of the per-step launches the rest of the reference loss adds, against the launches they replace, alternating in one process:
 
   - image loss at 800x800 (0.8 L1 + 0.2 (1 - SSIM)), per layout:
-      rgba    gutb200_image_loss (plain)            vs gutb200_image_loss_composited, white background + a 0/1 mask
-      split   gutb200_image_loss_rgb (plain)        vs gutb200_image_loss_composited, white background + a 0/1 mask (d_rgb + d_alpha)
-              and, for the random background, the composited entry on a [H,W,3] background image
+      rgba    gutb200_image_loss, layout 4, plain   vs  composited: white background + a 0/1 mask
+      split   gutb200_image_loss, layout 3, plain   vs  composited: white background + a 0/1 mask (d_rgb + d_alpha)
+              and, for the random background, the composited loss on a [H,W,3] background image
   - fused Adam at 300k Gaussians: gutb200_gaussian_adam_step vs gutb200_gaussian_adam_step_reg (lambda_opacity = lambda_scale = 0.01)
 
     python scripts/bench_loss_terms.py [--reps 200] [--rounds 5]
@@ -73,9 +73,9 @@ def main():
     ds = torch.from_numpy(rng.normal(size=(n, 48)).astype(np.float32) * 1e-4).to(dev)
 
     variants = {
-        "loss rgba  plain (gutb200_image_loss)": lambda: losses.image_loss(rgba, tgt, 0.8, 0.2, d_rgba=d4),
+        "loss rgba  plain (gutb200_image_loss, layout 4)": lambda: losses.image_loss(rgba, tgt, 0.8, 0.2, d_rgba=d4),
         "loss rgba  white + mask (composited)": lambda: losses.image_loss(rgba, tgt, 0.8, 0.2, d_rgba=d4, background=white, mask=mask),
-        "loss split plain (gutb200_image_loss_rgb)": lambda: losses.image_loss_rgb(rgb, tgt, 0.8, 0.2, d_rgb=d3),
+        "loss split plain (gutb200_image_loss, layout 3)": lambda: losses.image_loss_rgb(rgb, tgt, 0.8, 0.2, d_rgb=d3),
         "loss split white + mask (composited)": lambda: losses.image_loss_rgb_alpha(rgb, alpha, tgt, 0.8, 0.2, background=white, mask=mask,
                                                                                    d_rgb=d3, d_alpha=da),
         "loss split random image + mask (composited)": lambda: losses.image_loss_rgb_alpha(rgb, alpha, tgt, 0.8, 0.2, background=bg_img,

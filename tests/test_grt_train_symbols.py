@@ -7,9 +7,10 @@ def test_training_step_entry_points_are_exported():
 
     lib = nat.load()
     assert "grtb200_build_bvh_packed" in declared("grt_b200.h") and "grtb200_build_bvh_packed" in nat.GRT_EXPORTS
-    assert "gutb200_image_loss_rgb" in declared("gut_b200.h") and "gutb200_image_loss_rgb" in nat.EXPORTS
-    for name in ("grtb200_build_bvh_packed", "gutb200_image_loss_rgb", "grtb200_build_bvh", "gutb200_image_loss"):
+    assert "gutb200_image_loss" in declared("gut_b200.h") and "gutb200_image_loss" in nat.EXPORTS  # the rgb layout is its layout 3
+    for name in ("grtb200_build_bvh_packed", "grtb200_build_bvh", "gutb200_image_loss"):
         assert hasattr(lib, name), name
+    assert "gutb200_image_loss_rgb" not in declared("gut_b200.h") and not hasattr(lib, "gutb200_image_loss_rgb")
     assert hasattr(nat.GrtContext, "build_bvh_packed")
 
 

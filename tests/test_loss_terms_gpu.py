@@ -1,4 +1,4 @@
-"""GPU parity of the composited / masked image loss (gutb200_image_loss_composited) and of the fused Adam step with the opacity and scale
+"""GPU parity of the composited / masked image loss (gutb200_image_loss) and of the fused Adam step with the opacity and scale
 regularisers (gutb200_gaussian_adam_step_reg) against tests/loss_terms_oracle.py.
 Bars as in test_loss_gpu.py / test_adam_gpu.py: loss terms 1e-6 absolute; gradient |diff| <= 2e-6 * max|grad| + 1e-10; Adam 2e-6 relative."""
 import numpy as np
@@ -129,19 +129,29 @@ def test_composited_loss_rejects_bad_arguments():
     stream = torch.cuda.current_stream(dev).cuda_stream
     bg = (ctypes.c_float * 3)(1.0, 1.0, 1.0)
     rgba = torch.cat([rgb, alpha], -1).contiguous()
-    call = lib.gutb200_image_loss_composited
-    assert call(stream, 16, 16, 4, rgba.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr() + 4, None,
-                sums.data_ptr()) == 3  # the 4-wide gradient is stored 16 bytes at a time
-    assert call(stream, 16, 16, 3, rgb.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), d.data_ptr(),
-                sums.data_ptr()) == 1  # split layout without its alpha
-    assert call(stream, 16, 16, 3, rgb.data_ptr(), alpha.data_ptr(), tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(),
-                None, sums.data_ptr()) == 1  # ... or without d_alpha
-    assert call(stream, 16, 16, 5, rgba.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None,
-                sums.data_ptr()) == 1
-    assert call(stream, 0, 16, 4, rgba.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None,
-                sums.data_ptr()) == 1
-    assert call(stream, 16, 16, 4, rgba.data_ptr(), None, None, bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None,
-                sums.data_ptr()) == 1
+
+    def call(*args):  # the entry without post-processing; a refusal names its reason in gutb200_last_error(NULL)
+        rc = lib.gutb200_image_loss(*args, 0)
+        return rc, lib.gutb200_last_error(None).decode()
+
+    rc, why = call(stream, 16, 16, 4, rgba.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr() + 4,
+                   None, sums.data_ptr())
+    assert rc == 3 and "align" in why  # the 4-wide gradient is stored 16 bytes at a time
+    rc, why = call(stream, 16, 16, 3, rgb.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(),
+                   d.data_ptr(), sums.data_ptr())
+    assert rc == 1 and "pred_alpha" in why  # split layout without its alpha
+    rc, why = call(stream, 16, 16, 3, rgb.data_ptr(), alpha.data_ptr(), tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(),
+                   d.data_ptr(), None, sums.data_ptr())
+    assert rc == 1 and "needs d_alpha" in why  # ... or without d_alpha
+    rc, why = call(stream, 16, 16, 5, rgba.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None,
+                   sums.data_ptr())
+    assert rc == 1 and "layout=5" in why
+    rc, why = call(stream, 0, 16, 4, rgba.data_ptr(), None, tgt.data_ptr(), bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None,
+                   sums.data_ptr())
+    assert rc == 1 and "height" in why
+    rc, why = call(stream, 16, 16, 4, rgba.data_ptr(), None, None, bg, None, None, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None,
+                   sums.data_ptr())
+    assert rc == 1 and "target_rgb" in why
 
 
 @pytest.mark.parametrize("selective", [False, True])

@@ -4,7 +4,8 @@ import inspect
 
 from helpers import declared
 
-NEW = ("gutb200_image_loss_composited", "gutb200_gaussian_adam_step_reg")
+NEW = ("gutb200_image_loss", "gutb200_gaussian_adam_step_reg")
+REMOVED = ("gutb200_image_loss_rgb", "gutb200_image_loss_composited", "gutb200_image_loss_postprocessed")  # one loss entry takes every case
 
 
 def test_loss_terms_entry_points_are_exported():
@@ -14,8 +15,10 @@ def test_loss_terms_entry_points_are_exported():
     for name in NEW:
         assert name in declared("gut_b200.h") and name in nat.EXPORTS, name
         assert hasattr(lib, name), name
-    assert lib.gutb200_image_loss_composited.argtypes is not None
+    assert len(lib.gutb200_image_loss.argtypes) == 17  # layout, background, mask and post-processing included
     assert lib.gutb200_gaussian_adam_step_reg.argtypes is not None
+    for name in REMOVED:
+        assert name not in declared("gut_b200.h") and name not in nat.SIGNATURES and not hasattr(lib, name), name
 
 
 def test_new_arguments_without_a_gpu():

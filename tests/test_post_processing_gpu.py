@@ -88,31 +88,30 @@ def test_none_is_bit_identical_to_the_existing_entries():
             a = losses.image_loss(rgba, t_y, 0.8, 0.2, background=t_bg, mask=t_m)
             b = losses.image_loss(rgba, t_y, 0.8, 0.2, background=t_bg, mask=t_m, post_processing=None)
             assert torch.equal(a[3], b[3]) and abs(float(a[0]) - float(b[0])) <= 1e-6
+            want = {4: b}
             a = losses.image_loss_rgb_alpha(t_rgb, t_alpha, t_y, 0.8, 0.2, background=t_bg, mask=t_m)
             b = losses.image_loss_rgb_alpha(t_rgb, t_alpha, t_y, 0.8, 0.2, background=t_bg, mask=t_m, post_processing=None)
             assert torch.equal(a[3], b[3]) and torch.equal(a[4], b[4]) and abs(float(a[0]) - float(b[0])) <= 1e-6
-            # the C entry with post_processing 0 against gutb200_image_loss_composited, both layouts
+            want[3] = b
+            # the C entry called directly with post_processing 0 against what losses.* returned above, both layouts
             bg_rgb = (ctypes.c_float * 3)(*bg) if isinstance(bg, tuple) else None
             bg_img = t_bg.data_ptr() if isinstance(t_bg, torch.Tensor) else None
             mask = None if t_m is None else t_m.data_ptr()
             for layout, pred in ((4, rgba), (3, t_rgb)):
-                outs = []
-                for entry in ("composited", "postprocessed"):
-                    scratch = torch.empty(int(lib.gutb200_image_loss_scratch_bytes(h, w)) // 4 + 1, device=dev)
-                    d = torch.empty((h, w, layout), device=dev)
-                    d_alpha = torch.empty((h, w), device=dev)
-                    sums = torch.empty(2, device=dev)
-                    args = (stream, h, w, layout, pred.data_ptr(), None if layout == 4 else t_alpha.data_ptr(), t_y.data_ptr(), bg_rgb, bg_img, mask,
-                            0.8, 0.2, scratch.data_ptr(), d.data_ptr(), None if layout == 4 else d_alpha.data_ptr(), sums.data_ptr())
-                    rc = lib.gutb200_image_loss_composited(*args) if entry == "composited" else lib.gutb200_image_loss_postprocessed(*args, 0)
-                    assert rc == 0
-                    outs.append((d, d_alpha if layout == 3 else None, sums))
-                (d0, a0, s0), (d1, a1, s1) = outs
-                assert torch.equal(d0, d1), (background, masked, layout)
+                scratch = torch.empty(int(lib.gutb200_image_loss_scratch_bytes(h, w)) // 4 + 1, device=dev)
+                d = torch.empty((h, w, layout), device=dev)
+                d_alpha = torch.empty((h, w, 1), device=dev)
+                sums = torch.empty(2, device=dev)
+                rc = lib.gutb200_image_loss(stream, h, w, layout, pred.data_ptr(), None if layout == 4 else t_alpha.data_ptr(), t_y.data_ptr(),
+                                            bg_rgb, bg_img, mask, 0.8, 0.2, scratch.data_ptr(), d.data_ptr(),
+                                            None if layout == 4 else d_alpha.data_ptr(), sums.data_ptr(), 0)
+                assert rc == 0
+                assert torch.equal(d, want[layout][3]), (background, masked, layout)
                 means = torch.tensor([3.0 * h * w, 3.0 * (h - 10) * (w - 10)], device=dev)   # l1 and ssim of the sums
-                assert float(((s0 - s1) / means).abs().max()) <= 1e-6, (background, masked, layout)
+                l1_ssim = torch.stack([want[layout][1], want[layout][2]]).to(torch.float32)
+                assert float((sums / means - l1_ssim).abs().max()) <= 1e-6, (background, masked, layout)
                 if layout == 3:
-                    assert torch.equal(a0, a1), (background, masked, layout)
+                    assert torch.equal(d_alpha, want[layout][4]), (background, masked, layout)
 
 
 def test_rgb_entry_and_refusals():
@@ -138,8 +137,8 @@ def test_rgb_entry_and_refusals():
     d_alpha = torch.empty((40, 56), device=dev)
     sums = torch.empty(2, device=dev)
     stream = torch.cuda.current_stream(dev).cuda_stream
-    rc = lib.gutb200_image_loss_postprocessed(stream, 40, 56, 3, t_rgb.data_ptr(), t_alpha.data_ptr(), t_y.data_ptr(), None, None, None, 0.8,
-                                              0.2, scratch.data_ptr(), d.data_ptr(), d_alpha.data_ptr(), sums.data_ptr(), 7)
+    rc = lib.gutb200_image_loss(stream, 40, 56, 3, t_rgb.data_ptr(), t_alpha.data_ptr(), t_y.data_ptr(), None, None, None, 0.8, 0.2,
+                                scratch.data_ptr(), d.data_ptr(), d_alpha.data_ptr(), sums.data_ptr(), 7)
     assert rc == 1 and "post_processing=7" in lib.gutb200_last_error(None).decode()
 
 
