@@ -90,6 +90,8 @@ SIGNATURES = {
                                      _vp, _vp, _vp, _vp, _f32, _f32]),
     "gutb200_image_loss_scratch_bytes": (_sz, [_i32, _i32]),
     "gutb200_image_loss": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _vp, _vp, _i32]),
+    "gutb200_image_metrics_scratch_bytes": (_sz, [_i32, _i32]),
+    "gutb200_image_metrics": (_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_hybrid_rays": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gutb200_hybrid_composite": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp]),
     "gutb200_hybrid_composite_bwd": (_int, [_vp, _i64, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),

@@ -30,6 +30,9 @@ UNITS = {
     # optimizer step: plain IEEE arithmetic (the reference plugin is built without fast-math, setup_optimizers.py)
     "gut_optim.cu": [],
     "gut_loss.cu": [],
+    # evaluation metrics: no contraction, so that the composite rounds as its torch expression does (the PNG bytes and the LPIPS input
+    # agree); IEEE division for the colour correction
+    "gut_metrics.cu": ["-fmad=false"],
     "gut_debug.cu": [],
     # NHT feature decoder: fp16 tensor-core MLP, IEEE fp32 encoding and epilogues
     "nht_decoder.cu": [],

@@ -306,6 +306,14 @@ class GaussianTrainStep(TrainStep):
         return rgba, dist_, hits, vis
 
     @torch.no_grad()
+    def metrics_inputs(self, rays_o, rays_d, sensor, pose):
+        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": rgba [H,W,4] before background and
+        post-processing (the loss's layout 4), "alpha": None (channel 3), "hits": [H,W,1]}.  Arguments as render's."""
+        particles, sph = self.activated()
+        rgba, _, hits, _ = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
+        return {"pred": rgba, "alpha": None, "hits": hits}
+
+    @torch.no_grad()
     def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view.  target_rgb: [H,W,3].  all_sensor_positions: [world,3] sensor positions of every
         rank's view of this step in rank order (omit on a single GPU).  mask: optional [H,W] ([H,W,1], [1,H,W,1]) float CUDA tensor that

@@ -96,6 +96,16 @@ class GaussianTrainStepGRT(TrainStep):
                                                                           self.sph_degree, self.min_transmittance, normals=False)
         return self._post_process(rgb), alpha, dst, hits, vis
 
+    @torch.no_grad()
+    def metrics_inputs(self, rays_o, rays_d, T_to_world):
+        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": rgb [H,W,3] before background and
+        post-processing, "alpha": [H,W,1] (the loss's layout 3), "hits": [H,W,1]}.  Arguments as render's; no BVH cadence is advanced."""
+        particles, sph = self.activated()
+        self.tracer.tracer_wrapper.build_bvh_packed(particles)
+        rgb, alpha, _, _, hits, _ = self.tracer.tracer_wrapper.trace(self.frame, T_to_world, rays_o, rays_d, particles, sph, 0,
+                                                                      self.sph_degree, self.min_transmittance, normals=False)
+        return {"pred": rgb[0], "alpha": alpha[0], "hits": hits[0]}
+
     @staticmethod
     def sensor_position(T_to_world) -> np.ndarray:
         """World position of the view's sensor: the translation of T_to_world (float32 [3])."""

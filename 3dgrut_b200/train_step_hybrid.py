@@ -188,7 +188,7 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         sec_o, sec_d, hit = hybrid_rays(rays_o, rays_d, T_to_world, self.plane_point, self.plane_normal, out=buf["rays"])
         self._mark("rays")
         pose = self.pose_from_c2w(T_to_world)
-        rgba, dst, _, vis_p = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
+        rgba, dst, hits, vis_p = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
         self._mark("primary")
         if train:
             self._build(particles)
@@ -199,15 +199,24 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
                                                normals=False)
         self._mark("secondary")
         rgb = hybrid_composite(rgba, sec[0], hit, self.reflectivity, out=buf["rgb"])
-        return pose, rgba, dst, vis_p, sec, (sec_o, sec_d, hit), rgb
+        return pose, rgba, dst, vis_p, sec, (sec_o, sec_d, hit), rgb, hits
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, T_to_world):
         """Forward only: (hybrid rgb [H,W,3], primary rgba [H,W,4], secondary rgb [1,H,W,3], hit [H*W]).  Under post_processing the hybrid
         rgb is encoded, the two passes are returned as traced.  The build it needs does not advance the step's BVH cadence."""
         particles, sph = self.activated()
-        _, rgba, _, _, sec, (_, _, hit), rgb = self._forward(rays_o, rays_d, sensor, T_to_world, particles, sph, train=False)
+        _, rgba, _, _, sec, (_, _, hit), rgb, _ = self._forward(rays_o, rays_d, sensor, T_to_world, particles, sph, train=False)
         return self._post_process(rgb), rgba, sec[0], hit
+
+    @torch.no_grad()
+    def metrics_inputs(self, rays_o, rays_d, sensor, T_to_world):
+        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": the hybrid composite rgb [H,W,3] before background
+        and post-processing, "alpha": the primary pass's alpha [H,W,1] (as the loss composites), "hits": the primary pass's [H,W,1]}.
+        Arguments as render's; no BVH cadence is advanced."""
+        particles, sph = self.activated()
+        _, rgba, _, _, _, _, rgb, hits = self._forward(rays_o, rays_d, sensor, T_to_world, particles, sph, train=False)
+        return {"pred": rgb, "alpha": rgba[..., 3:].contiguous(), "hits": hits}
 
     def _image_loss(self, pred, target, lambda_l1, lambda_ssim, background, mask):
         rgb, rgba, zero1 = pred
@@ -225,7 +234,7 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         if mask is not None:
             mask = losses.mask_hw(mask, H, W)
         particles, sph = self.activated()
-        pose, rgba, dst, vis_p, (srgb, salpha, sdst, snrm, _, vis_s), (sec_o, sec_d, hit), rgb = self._forward(
+        pose, rgba, dst, vis_p, (srgb, salpha, sdst, snrm, _, vis_s), (sec_o, sec_d, hit), rgb, _ = self._forward(
             rays_o, rays_d, sensor, T_to_world, particles, sph, train=True)
         buf = self._scratch(H, W)
         zero1, zero3 = self._zero_grads(H, W)

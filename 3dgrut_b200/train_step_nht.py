@@ -224,7 +224,7 @@ class GaussianTrainStepNHT(_NHTStep, TrainStep):
         dirs = world_ray_directions(c2w_rotation_from_pose7(pose), rays_d)
         rgb = self._decode(features, dirs).view(H, W, 3)
         self._mark("decode")
-        return particles, feats, out, dst, vis, features, alpha, dirs, rgb
+        return particles, feats, out, dst, vis, features, alpha, dirs, rgb, hits
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, pose):
@@ -233,13 +233,20 @@ class GaussianTrainStepNHT(_NHTStep, TrainStep):
         return self._post_process(out[8]), out[6]
 
     @torch.no_grad()
+    def metrics_inputs(self, rays_o, rays_d, sensor, pose):
+        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": decoded rgb [H,W,3] before background and
+        post-processing, "alpha": [H,W,1], "hits": [H,W,1]}.  Arguments as render's; decoded with the decoder's current weights."""
+        out = self._forward(rays_o, rays_d, sensor, pose)
+        return {"pred": out[8], "alpha": out[6], "hits": out[9]}
+
+    @torch.no_grad()
     def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view; arguments as GaussianTrainStep.step.  Returns this view's loss (a device scalar), the
         regularisers included while they apply."""
         H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
         if mask is not None:
             mask = losses.mask_hw(mask, H, W)
-        particles, feats, out, dst, vis, features, alpha, dirs, rgb = self._forward(rays_o, rays_d, sensor, pose)
+        particles, feats, out, dst, vis, features, alpha, dirs, rgb, _ = self._forward(rays_o, rays_d, sensor, pose)
         zero1 = self._zero(H, W)
         loss, (d_rgb, d_alpha) = self._loss((rgb, alpha, zero1), rgb, target_rgb.reshape(H, W, 3), H, W, mask)
         self._mark("loss")
@@ -270,7 +277,7 @@ class GaussianTrainStepGRTNHT(_NHTStep, GaussianTrainStepGRT):
         dirs = world_ray_directions(c2w_rotation_from_T(T_to_world), rays_d)
         rgb = self._decode(features, dirs).view(H, W, 3)
         self._mark("decode")
-        return particles, feats, feat, alpha, dst, nrm, vis, dirs, rgb
+        return particles, feats, feat, alpha, dst, nrm, vis, dirs, rgb, hits
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, T_to_world):
@@ -282,6 +289,15 @@ class GaussianTrainStepGRTNHT(_NHTStep, GaussianTrainStepGRT):
         return self._post_process(out[8]), out[3][0]
 
     @torch.no_grad()
+    def metrics_inputs(self, rays_o, rays_d, T_to_world):
+        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": decoded rgb [H,W,3] before background and
+        post-processing, "alpha": [H,W,1], "hits": [H,W,1]}.  Arguments as render's; no BVH cadence is advanced."""
+        particles, feats = self.activated()
+        self.tracer.tracer_wrapper.build_bvh_packed(particles)
+        out = self._forward(rays_o, rays_d, T_to_world, particles, feats)
+        return {"pred": out[8], "alpha": out[3][0], "hits": out[9][0]}
+
+    @torch.no_grad()
     def step(self, rays_o, rays_d, T_to_world, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view; arguments as GaussianTrainStepGRT.step."""
         H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
@@ -290,7 +306,7 @@ class GaussianTrainStepGRTNHT(_NHTStep, GaussianTrainStepGRT):
         particles, feats = self.activated()
         self._build(particles)
         self._mark("build")
-        _, _, feat, alpha, dst, nrm, vis, dirs, rgb = self._forward(rays_o, rays_d, T_to_world, particles, feats)
+        _, _, feat, alpha, dst, nrm, vis, dirs, rgb, _ = self._forward(rays_o, rays_d, T_to_world, particles, feats)
         zero1, zero3 = self._zero_grads(H, W)
         loss, (d_rgb, d_alpha) = self._loss((rgb, alpha, zero1), rgb, target_rgb.reshape(H, W, 3), H, W, mask)
         self._mark("loss")

@@ -177,6 +177,40 @@ int gutb200_image_loss(void* stream, int32_t height, int32_t width, int32_t layo
                        const float* target_rgb, const float* background_rgb, const float* background_image, const float* mask,
                        float lambda_l1, float lambda_ssim, void* scratch, float* d_pred, float* d_alpha, float* sums2, int32_t post_processing);
 
+/* Test-set metrics of one rendered frame as the reference evaluator computes them (threedgrut/render.py:294-369, trainer.py:641-657,
+ * 1350-1364), with the pixel loads of gutb200_image_loss and no mask: x = s(rgb + bg (1 - alpha)) against the target y [H,W,3].
+ *   psnr = 10 log10(1 / mean (x - y)^2) over 3HW (x unclipped; +inf when x == y).  ssim: the 11-tap Gaussian window (sigma 1.5), C1 =
+ *   0.01^2, C2 = 0.03^2, both variances clamped at 0, mean over the (H-10)(W-10) 3 interior (torchmetrics' SSIM with data_range 1:
+ *   reflect pad 5, crop 5).  a, b per channel (threedgrut/utils/color_correct.py:96-145) from fp64 moments over all HW pixels: var =
+ *   max(E[y^2] - E[y]^2, 1e-8), a = (E[xy] - E[x] E[y]) / var, b = E[x] - a E[y], then a = 1 where |a| < 1e-8; cc_psnr / cc_ssim are psnr
+ *   / ssim of x_cc = clip((x - b) / a, 0, 1) (fp32, IEEE division) against y.  l1 = mean |x - y|.  hits [H,W] int32 or NULL: mean,
+ *   unbiased std, min, max (NaN without hits).
+ * layout, pred, pred_alpha, background_rgb and post_processing as in gutb200_image_loss (a background image is not taken: evaluation
+ * composites a constant colour, and a random training background evaluates as black).  pred_u8 / target_u8: [H,W,3] device bytes or
+ * NULL, x and y quantised as torchvision.utils.save_image does: trunc(clamp(fl(fl(v 255) + 0.5), 0, 255)).
+ * out: GUTB200_METRICS_K device doubles in the order of the enum below.  scratch: gutb200_image_metrics_scratch_bytes(H, W) device bytes,
+ * 8-byte aligned.  Four launches on `stream` (pass, finalise, colour-corrected pass, finalise), no synchronisation, no atomics: the same
+ * inputs give the same bits.  Returns 0, 1 for bad arguments (H or W below 11 among them), 2 for a launch error; gutb200_last_error(NULL)
+ * then names the cause. */
+enum {
+    GUTB200_METRIC_PSNR = 0,
+    GUTB200_METRIC_SSIM = 1,
+    GUTB200_METRIC_CC_PSNR = 2,
+    GUTB200_METRIC_CC_SSIM = 3,
+    GUTB200_METRIC_L1 = 4,
+    GUTB200_METRIC_HITS_MEAN = 5,
+    GUTB200_METRIC_HITS_STD = 6,
+    GUTB200_METRIC_HITS_MIN = 7,
+    GUTB200_METRIC_HITS_MAX = 8,
+    GUTB200_METRIC_A = 9,  /* a[3] */
+    GUTB200_METRIC_B = 12, /* b[3] */
+    GUTB200_METRICS_K = 15
+};
+size_t gutb200_image_metrics_scratch_bytes(int32_t height, int32_t width);
+int gutb200_image_metrics(void* stream, int32_t height, int32_t width, int32_t layout, const float* pred, const float* pred_alpha,
+                          const float* target_rgb, const float* background_rgb, int32_t post_processing, const int32_t* hits, void* scratch,
+                          double* out, uint8_t* pred_u8, uint8_t* target_u8);
+
 /* 3DGRUT hybrid (ours; hybrid.py's mirror_rays and render_hybrid as device code for train_step_hybrid): primary rays through 3DGUT, one
  * mirror bounce off a plane through 3DGRT.  No context: one launch each on `stream` of the current device, no synchronisation; 0 on success.
  * gutb200_hybrid_rays: rays_o / rays_d [pixels,3] in camera space, T_to_world_host the 12 floats of the camera-to-world [R | t] (row-major

@@ -151,7 +151,7 @@ def main():
     def fwd_bwd(v):
         with torch.no_grad():
             particles, sph = st.activated()
-            pose, rgba, dst, _, sec, (so, sd, hit), _ = st._forward(rays_o, rays_d, sensor, poses[v], particles, sph, train=True)
+            pose, rgba, dst, _, sec, (so, sd, hit), _, _ = st._forward(rays_o, rays_d, sensor, poses[v], particles, sph, train=True)
             d_rgba, d_sec = th.hybrid_composite_bwd(rgba, sec[0], hit, st.reflectivity, d_img)
             z1, z3 = st._zero_grads(H, W)
             st.raster.trace_bwd(st.frame, st.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst,
