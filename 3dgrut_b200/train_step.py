@@ -13,9 +13,11 @@ Every rank holds a replica of the parameters and renders its own camera of the s
 batch (number of ranks), so the replicas stay identical.  The trainer, datasets, densification and logging of the reference stay out
 of scope; this class exists so that the path can be run -- and tested -- as the training loop uses it.
 
-`TrainStep` holds what this step and the 3DGRT one (train_step_grt.GaussianTrainStepGRT) share: the parameters, the optimizer, the
-background, the densifier, the loss dispatch and everything after the backward."""
+`TrainStep` holds what every training step shares: the parameters, the optimizer, the background, the densifier, the order of a step,
+the loss dispatch and everything after the backward.  A renderer's step supplies its forward (a `Frame`) and its backward."""
 from __future__ import annotations
+
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -28,10 +30,24 @@ import view_parallel
 from threedgut_tracer.tracer import SplatRaster
 
 
+class Frame(NamedTuple):
+    """What a step reads after its renderer's forward."""
+    pred: torch.Tensor    # the render the loss takes, before background and post-processing
+    layout: int           # 4: pred is the 3DGUT rgba [H,W,4]; 3: pred is rgb [H,W,3] and `alpha` is separate
+    rgb: torch.Tensor     # the colour channels [H,W,3]
+    alpha: torch.Tensor | None  # [H,W,1] (any strides), or None where it is channel 3 of pred
+    hits: torch.Tensor    # [H,W,1]
+    vis: torch.Tensor     # the visibility the optimizer's selective update reads
+    saved: tuple          # the renderer's own: what its `_backward` reads
+
+
 class TrainStep:
     """The part of a view-parallel training step that does not depend on the renderer.  A subclass creates its renderer
-    (`_init_renderer`) and its exchange (`_new_exchange`), gives the loss gradient its renderer's layout (`_image_loss`, `_l1_grads`),
-    and writes `step` as: activations -> trace -> `_loss` -> backward into `exchange.out()` -> `_update`."""
+    (`_init_renderer`) and its exchange (`_new_exchange`), renders a view into a `Frame` (`_forward`), writes the view's gradients into
+    `exchange.out()` (`_backward`) and gives this view's sensor position (`_sensor_position`); its public `step`, `render` and
+    `metrics_inputs` take the view's arguments and `_step` runs: activations -> `_forward` -> `_loss` -> `_backward` -> `_update`."""
+
+    PHASES = ("exchange", "adam", "densify")  # the phases `phase_events` records; a subclass lists its own
 
     def __init__(self, params: dict, lrs: dict | None, conf=None, sph_degree: int | None = None, selective: bool = False, group=None,
                  eps: float = 1e-15, densify_conf=None, scene_extent: float = 1.0, lambda_l1: float = 1.0, lambda_ssim: float = 0.0,
@@ -49,6 +65,7 @@ class TrainStep:
         (in place of `lrs`) and degree (refused together with an explicit sph_degree) and updates both after every Adam launch, as the
         reference trainer's schedulers and progressive SH do."""
         losses.post_processing_code(post_processing)  # refuse what is not built before anything is allocated
+        self._buffers = {}  # name -> (resolution, buffers): see _scratch
         self.post_processing = post_processing
         self.params = {k: params[k] for k in self.GROUPS}  # ONE dict shared with the optimizer and the densifier
         self.device = self.params["positions"].device
@@ -84,6 +101,9 @@ class TrainStep:
 
     GROUPS = optimizers.GROUPS  # the raw parameter tensors the step trains
 
+    def bytes_on_wire(self) -> int:
+        return self.exchange.bytes_on_wire()
+
     def _new_optimizer(self, lrs, eps, selective):
         return optimizers.FusedGaussianAdam(self.params, lrs, eps=eps, selective=selective)
 
@@ -99,23 +119,70 @@ class TrainStep:
         return particle_record(p), torch.cat([p["features_albedo"], p["features_specular"]], dim=1).contiguous()
 
     def _mark(self, phase):
-        if self.phase_events is not None:
+        if self.phase_events is not None and phase in self.PHASES:
             ev = torch.cuda.Event(enable_timing=True)
             ev.record()
             self.phase_events.append((phase, ev))
 
-    def _loss(self, pred, rgb, target, H, W, mask):
-        """This view's loss and its gradient in the renderer's layout.  pred: the render as `_image_loss` / `_l1_grads` take it; rgb: its
-        colour channels [H,W,3]; target: [H,W,3].  The gradient carries the global-batch normalisation (1 / world); the loss returned
-        does not."""
-        if not self.background.black or mask is not None or self.lambda_ssim != 0.0 or self.post_processing is not None:
-            # composited onto the background, post-processed and masked (then with an alpha gradient), or lambda_l1 L1 + lambda_ssim
-            # (1 - SSIM): two launches (gut_loss.cu).  The L1 shortcut below does not apply in encoded space.
-            loss, grads = self._image_loss(pred, target.contiguous(), self.lambda_l1 / self.world, self.lambda_ssim / self.world,
-                                           self.background.draw(H, W), mask)
-            return loss * self.world, grads
-        diff = rgb - target
-        return self.lambda_l1 * diff.abs().mean(), self._l1_grads(pred, diff)
+    def _scratch(self, name, key, make):
+        """The buffers `name` of resolution `key`: make() on the first step at it, and again (dropping the old ones) when it changes."""
+        held = self._buffers.get(name)
+        if held is None or held[0] != key:
+            held = self._buffers[name] = (key, make())
+        return held[1]
+
+    def _zeros(self, H, W, channels):
+        """A zero [1,H,W,channels] gradient for the renderer inputs the loss does not differentiate; never written."""
+        return self._scratch(("zeros", channels), (H, W), lambda: torch.zeros((1, H, W, channels), dtype=torch.float32, device=self.device))
+
+    def _step(self, view, target_rgb, all_sensor_positions, mask):
+        """The body of every `step`.  view: the arguments of the subclass's `render`, rays_o [1,H,W,3] first."""
+        H, W = int(view[0].shape[1]), int(view[0].shape[2])
+        if mask is not None:
+            mask = losses.mask_hw(mask, H, W)
+        particles, features = self.activated()
+        frame = self._forward(view, particles, features, train=True)
+        loss, d_pred, d_alpha = self._loss(frame, target_rgb.reshape(H, W, 3), H, W, mask)
+        self._mark("loss")
+        exchange_args = self._backward(frame, d_pred, d_alpha)
+        my_position = self._sensor_position(frame) if self.densifier is not None or exchange_args else None
+        if exchange_args:  # the compact exchange rebuilds the SH gradient from the sensor position of every view of the step
+            positions = my_position[None] if all_sensor_positions is None else all_sensor_positions
+            exchange_args = (*exchange_args, np.asarray(positions, np.float32))
+        return self._update(loss, particles, frame.vis, all_sensor_positions, my_position, exchange_args)
+
+    @torch.no_grad()
+    def metrics_inputs(self, *view):
+        """Forward only, what the test-set metrics read (metrics.image_metrics); arguments as `render`'s.  {"pred": the render before
+        background and post-processing in the loss's layout (rgba [H,W,4], or rgb [H,W,3] for the split layout), "alpha": [H,W,1], or None
+        where it is channel 3 of pred, "hits": [H,W,1]}.  No BVH cadence is advanced; the NHT steps decode with the current weights."""
+        f = self._forward(view, *self.activated(), train=False)
+        return {"pred": f.pred, "alpha": None if f.alpha is None else f.alpha.contiguous(), "hits": f.hits}
+
+    def _loss(self, frame, target, H, W, mask):
+        """This view's loss and its gradients (d_pred in frame.pred's layout, d_alpha [H,W,1] or None where the loss gives the separate
+        alpha none).  target: [H,W,3].  The gradients carry the global-batch normalisation (1 / world); the loss returned does not."""
+        if self.background.black and mask is None and self.lambda_ssim == 0.0 and self.post_processing is None:
+            diff = frame.rgb - target
+            loss = self.lambda_l1 * diff.abs().mean()
+            if frame.layout == 3:
+                return loss, self._d_l1(diff), None
+            d_rgba = torch.zeros_like(frame.pred)
+            d_rgba[..., :3] = self._d_l1(diff)
+            return loss, d_rgba, None
+        # composited onto the background, post-processed and masked (then with an alpha gradient), or lambda_l1 L1 + lambda_ssim
+        # (1 - SSIM): two launches (gut_loss.cu).  The L1 shortcut above does not apply in encoded space.
+        target, l1, ssim = target.contiguous(), self.lambda_l1 / self.world, self.lambda_ssim / self.world
+        background, post = self.background.draw(H, W), self.post_processing
+        d_alpha = None
+        if frame.layout == 4:  # d_rgba carries the alpha gradient when composited
+            loss, _, _, d_pred = losses.image_loss(frame.pred, target, l1, ssim, background=background, mask=mask, post_processing=post)
+        elif background is None and mask is None and post is None:  # black, unmasked: the rgb loss, no alpha gradient
+            loss, _, _, d_pred = losses.image_loss_rgb(frame.pred, target, l1, ssim)
+        else:
+            loss, _, _, d_pred, d_alpha = losses.image_loss_rgb_alpha(frame.pred, frame.alpha.contiguous(), target, l1, ssim,
+                                                                      background=background, mask=mask, post_processing=post)
+        return loss * self.world, d_pred, d_alpha
 
     def _d_l1(self, diff):
         """d lambda_l1 mean|diff| / d rgb with the global-batch normalisation"""
@@ -286,51 +353,35 @@ class GaussianTrainStep(TrainStep):
     def _new_exchange(self):
         return view_parallel.CompactGradientExchange(self.raster, self.n, self.device, group=self.group)
 
-    def _image_loss(self, rgba, target, lambda_l1, lambda_ssim, background, mask):
-        loss, _, _, d_rgba = losses.image_loss(rgba, target, lambda_l1, lambda_ssim, background=background, mask=mask,
-                                               post_processing=self.post_processing)
-        return loss, d_rgba  # d_rgba carries the alpha gradient when composited (gut_loss.cu)
+    def _forward(self, view, particles, sph, train):
+        rays_o, rays_d, sensor, pose = view
+        rgba, dst, hits, vis = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
+        return Frame(rgba, 4, rgba[..., :3], None, hits, vis, (view, particles, sph, dst))
 
-    def _l1_grads(self, rgba, diff):
-        d_rgba = torch.zeros_like(rgba)
-        d_rgba[..., :3] = self._d_l1(diff)
-        return d_rgba
+    def _backward(self, frame, d_rgba, d_alpha):
+        (rays_o, rays_d, sensor, pose), particles, sph, dst = frame.saved
+        d_dist = torch.zeros_like(dst)
+        self.raster.trace_bwd_compact(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, frame.pred,
+                                      d_rgba, dst, d_dist, out=self.exchange.out())
+        return self.sph_degree, particles
+
+    def _sensor_position(self, frame):
+        _, _, sensor, pose = frame.saved[0]
+        return self.raster.sensor_position(sensor, pose, pose, frame.rgb.shape[1], frame.rgb.shape[0])
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, pose):
         """Forward only: (rgba [H,W,4], dist, hits, visibility); under post_processing the rgb channels are encoded, alpha is not."""
-        particles, sph = self.activated()
-        rgba, dist_, hits, vis = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
-        if self.post_processing is not None:
-            rgba = torch.cat([self._post_process(rgba[..., :3]), rgba[..., 3:]], -1)
-        return rgba, dist_, hits, vis
-
-    @torch.no_grad()
-    def metrics_inputs(self, rays_o, rays_d, sensor, pose):
-        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": rgba [H,W,4] before background and
-        post-processing (the loss's layout 4), "alpha": None (channel 3), "hits": [H,W,1]}.  Arguments as render's."""
-        particles, sph = self.activated()
-        rgba, _, hits, _ = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
-        return {"pred": rgba, "alpha": None, "hits": hits}
+        f = self._forward((rays_o, rays_d, sensor, pose), *self.activated(), train=False)
+        rgba = f.pred if self.post_processing is None else torch.cat([self._post_process(f.rgb), f.pred[..., 3:]], -1)
+        return rgba, f.saved[3], f.hits, f.vis
 
     @torch.no_grad()
     def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view.  target_rgb: [H,W,3].  all_sensor_positions: [world,3] sensor positions of every
         rank's view of this step in rank order (omit on a single GPU).  mask: optional [H,W] ([H,W,1], [1,H,W,1]) float CUDA tensor that
         multiplies prediction and target before the loss.  Returns this view's loss (a device scalar), the regularisers included."""
-        H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
-        if mask is not None:
-            mask = losses.mask_hw(mask, H, W)
-        particles, sph = self.activated()
-        rgba, dst, hits, vis = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
-        loss, d_rgba = self._loss(rgba, rgba[..., :3], target_rgb, H, W, mask)
-        d_dist = torch.zeros_like(dst)
-        self.raster.trace_bwd_compact(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba,
-                                      dst, d_dist, out=self.exchange.out())
-        my_position = self.raster.sensor_position(sensor, pose, pose, W, H)
-        positions = my_position[None] if all_sensor_positions is None else all_sensor_positions
-        return self._update(loss, particles, vis, all_sensor_positions, my_position,
-                            (self.sph_degree, particles, np.asarray(positions, np.float32)))
+        return self._step((rays_o, rays_d, sensor, pose), target_rgb, all_sensor_positions, mask)
 
 
 def particle_record(p: dict) -> torch.Tensor:

@@ -22,9 +22,9 @@ import numpy as np
 import torch
 
 import b200_native as native
-import losses
 from b200_native import cfg_get, ptr
 from threedgut_tracer.tracer import ShutterType, SplatRaster, Tracer as GutTracer
+from train_step import Frame
 from train_step_grt import GaussianTrainStepGRT
 
 PHASES = ("rays", "primary", "build", "secondary", "loss", "backward_primary", "backward_secondary", "exchange", "adam", "densify")
@@ -158,20 +158,15 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         return {**super()._settings(), "mirror": {"plane_point": [float(v) for v in self.plane_point],
                                                   "plane_normal": [float(v) for v in self.plane_normal], "reflectivity": self.reflectivity}}
 
+    PHASES = PHASES
+
     def _init_renderer(self, conf):
         super()._init_renderer(conf)  # the 3DGRT tracer of the secondary rays
         self.raster = SplatRaster(conf)
         self._identity = torch.eye(4, dtype=torch.float32)[None]  # the secondary rays are in world space (host: no read-back per trace)
-        self._buffers = {}
 
-    def _scratch(self, H, W):
-        """Per-resolution buffers: the secondary rays and hit mask, the composite and its gradients."""
-        key = (H, W)
-        if key not in self._buffers:
-            e = lambda *s: torch.empty(s, dtype=torch.float32, device=self.device)  # noqa: E731
-            self._buffers = {key: dict(rays=(e(1, H, W, 3), e(1, H, W, 3), e(H * W)), rgb=e(H, W, 3), grads=(e(H, W, 4), e(1, H, W, 3)),
-                                       zero_dist=torch.zeros((H, W, 1), dtype=torch.float32, device=self.device))}
-        return self._buffers[key]
+    def _empty(self, *shape):
+        return torch.empty(shape, dtype=torch.float32, device=self.device)
 
     @staticmethod
     def pose_from_c2w(T_to_world) -> np.ndarray:
@@ -179,49 +174,53 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         t = T_to_world.detach().cpu() if torch.is_tensor(T_to_world) else np.asarray(T_to_world)
         return GutTracer._pose_from_c2w(t.reshape(-1, 4, 4)[0])
 
-    def _forward(self, rays_o, rays_d, sensor, T_to_world, particles, sph, train):
-        """Rays, primary trace, build, secondary trace, composite.  train: the step's BVH cadence and buffers (True), or a plain rebuild
-        and new tensors (render)."""
+    def _forward(self, view, particles, sph, train):
+        """Rays, primary trace, build, secondary trace, composite.  train: the step's BVH cadence and per-resolution buffers, or a build
+        that does not advance the cadence and new tensors (render, metrics_inputs)."""
+        rays_o, rays_d, sensor, T_to_world = view
         check_sensor(sensor)
         H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
-        buf = self._scratch(H, W) if train else {"rays": None, "rgb": None}
-        sec_o, sec_d, hit = hybrid_rays(rays_o, rays_d, T_to_world, self.plane_point, self.plane_normal, out=buf["rays"])
+        rays = self._scratch("rays", (H, W), lambda: (self._empty(1, H, W, 3), self._empty(1, H, W, 3), self._empty(H * W))) if train else None
+        sec_o, sec_d, hit = hybrid_rays(rays_o, rays_d, T_to_world, self.plane_point, self.plane_normal, out=rays)
         self._mark("rays")
         pose = self.pose_from_c2w(T_to_world)
-        rgba, dst, hits, vis_p = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
+        rgba, dst, hits, vis = self.raster.trace(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
         self._mark("primary")
-        if train:
-            self._build(particles)
-        else:
-            self.tracer.tracer_wrapper.build_bvh_packed(particles)
-        self._mark("build")
+        self._build(particles, train)
         sec = self.tracer.tracer_wrapper.trace(self.frame, self._identity, sec_o, sec_d, particles, sph, 0, self.sph_degree, self.min_transmittance,
                                                normals=False)
         self._mark("secondary")
-        rgb = hybrid_composite(rgba, sec[0], hit, self.reflectivity, out=buf["rgb"])
-        return pose, rgba, dst, vis_p, sec, (sec_o, sec_d, hit), rgb, hits
+        rgb = hybrid_composite(rgba, sec[0], hit, self.reflectivity, out=self._scratch("rgb", (H, W), lambda: self._empty(H, W, 3)) if train else None)
+        if train and self.optimizer.selective:
+            vis = torch.maximum(vis, sec[5])  # visible in either pass
+        # the loss composites the hybrid rgb with the PRIMARY pass's alpha
+        return Frame(rgb, 3, rgb, rgba[..., 3:], hits, vis, (view, particles, sph, pose, rgba, dst, sec, (sec_o, sec_d, hit)))
+
+    def _backward(self, frame, d_rgb, d_alpha):
+        (rays_o, rays_d, sensor, _), particles, sph, pose, rgba, dst, (srgb, salpha, sdst, snrm, _, _), (sec_o, sec_d, hit) = frame.saved
+        H, W = frame.rgb.shape[:2]
+        grads = self._scratch("grads", (H, W), lambda: (self._empty(H, W, 4), self._empty(1, H, W, 3)))
+        d_rgba, d_sec = hybrid_composite_bwd(rgba, srgb, hit, self.reflectivity, d_rgb, d_alpha, out=grads)
+        zero1, zero3 = self._zeros(H, W, 1), self._zeros(H, W, 3)
+        self.raster.trace_bwd(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst,
+                              zero1[0], out=self.exchange.out())
+        self._mark("backward_primary")
+        self.tracer.tracer_wrapper.trace_bwd(self.frame, self._identity, sec_o, sec_d, srgb, salpha, sdst, snrm, particles, sph, d_sec, zero1,
+                                             zero1, zero3, 0, self.sph_degree, self.min_transmittance, out=self.exchange.out(), accumulate=True)
+        self._mark("backward_secondary")
+        return ()
+
+    def _sensor_position(self, frame):
+        _, _, sensor, _ = frame.saved[0]
+        return self.raster.sensor_position(sensor, frame.saved[3], frame.saved[3], frame.rgb.shape[1], frame.rgb.shape[0])
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, T_to_world):
         """Forward only: (hybrid rgb [H,W,3], primary rgba [H,W,4], secondary rgb [1,H,W,3], hit [H*W]).  Under post_processing the hybrid
         rgb is encoded, the two passes are returned as traced.  The build it needs does not advance the step's BVH cadence."""
-        particles, sph = self.activated()
-        _, rgba, _, _, sec, (_, _, hit), rgb, _ = self._forward(rays_o, rays_d, sensor, T_to_world, particles, sph, train=False)
-        return self._post_process(rgb), rgba, sec[0], hit
-
-    @torch.no_grad()
-    def metrics_inputs(self, rays_o, rays_d, sensor, T_to_world):
-        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": the hybrid composite rgb [H,W,3] before background
-        and post-processing, "alpha": the primary pass's alpha [H,W,1] (as the loss composites), "hits": the primary pass's [H,W,1]}.
-        Arguments as render's; no BVH cadence is advanced."""
-        particles, sph = self.activated()
-        _, rgba, _, _, _, _, rgb, hits = self._forward(rays_o, rays_d, sensor, T_to_world, particles, sph, train=False)
-        return {"pred": rgb, "alpha": rgba[..., 3:].contiguous(), "hits": hits}
-
-    def _image_loss(self, pred, target, lambda_l1, lambda_ssim, background, mask):
-        rgb, rgba, zero1 = pred
-        alpha = rgba[..., 3:].contiguous() if (background is not None or mask is not None or self.post_processing is not None) else None
-        return GaussianTrainStepGRT._image_loss(self, (rgb, alpha, zero1), target, lambda_l1, lambda_ssim, background, mask)
+        f = self._forward((rays_o, rays_d, sensor, T_to_world), *self.activated(), train=False)
+        _, _, _, _, rgba, _, sec, (_, _, hit) = f.saved
+        return self._post_process(f.rgb), rgba, sec[0], hit
 
     @torch.no_grad()
     def step(self, rays_o, rays_d, sensor, T_to_world, target_rgb, all_sensor_positions=None, mask=None):
@@ -230,23 +229,4 @@ class GaussianTrainStepHybrid(GaussianTrainStepGRT):
         view of this step in rank order (omit on a single GPU; only the densifier reads this rank's own).  mask: optional [H,W] ([H,W,1],
         [1,H,W,1]) float CUDA tensor that multiplies prediction and target before the loss.  Returns this view's loss (a device scalar), the
         regularisers included."""
-        H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
-        if mask is not None:
-            mask = losses.mask_hw(mask, H, W)
-        particles, sph = self.activated()
-        pose, rgba, dst, vis_p, (srgb, salpha, sdst, snrm, _, vis_s), (sec_o, sec_d, hit), rgb, _ = self._forward(
-            rays_o, rays_d, sensor, T_to_world, particles, sph, train=True)
-        buf = self._scratch(H, W)
-        zero1, zero3 = self._zero_grads(H, W)
-        loss, (d_rgb, d_alpha) = self._loss((rgb, rgba, zero1), rgb, target_rgb.reshape(H, W, 3), H, W, mask)
-        self._mark("loss")
-        d_rgba, d_sec = hybrid_composite_bwd(rgba, srgb, hit, self.reflectivity, d_rgb, None if d_alpha is zero1 else d_alpha, out=buf["grads"])
-        self.raster.trace_bwd(self.frame, self.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst,
-                              buf["zero_dist"], out=self.exchange.out())
-        self._mark("backward_primary")
-        self.tracer.tracer_wrapper.trace_bwd(self.frame, self._identity, sec_o, sec_d, srgb, salpha, sdst, snrm, particles, sph, d_sec, zero1,
-                                             zero1, zero3, 0, self.sph_degree, self.min_transmittance, out=self.exchange.out(), accumulate=True)
-        self._mark("backward_secondary")
-        vis = torch.maximum(vis_p, vis_s) if self.optimizer.selective else vis_p
-        my_position = self.raster.sensor_position(sensor, pose, pose, W, H) if self.densifier is not None else None
-        return self._update(loss, particles, vis, all_sensor_positions, my_position)
+        return self._step((rays_o, rays_d, sensor, T_to_world), target_rgb, all_sensor_positions, mask)

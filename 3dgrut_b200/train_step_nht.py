@@ -1,5 +1,5 @@
 """View-parallel training steps for the Neural Harmonic Texture (NHT) model (model.feature_type: nht) on both renderers:
-GaussianTrainStepNHT (3DGUT) and GaussianTrainStepGRTNHT (3DGRT), on the TrainStep core of train_step.py.
+GaussianTrainStepNHT (3DGUT) and GaussianTrainStepGRTNHT (3DGRT), each the SH step of its renderer with the NHT forward and backward.
 
 Replaces Tracer.render -> apply_feature_decoder -> apply_background -> loss -> autograd -> two torch.optim.Adam of the reference trainer
 (threedgrut/trainer.py:1119-1263, utils/render.py:54-92) with no autograd graph:
@@ -20,12 +20,10 @@ import numpy as np
 import torch
 
 import feature_decoder as fd
-import losses
 import optimizers
 import view_parallel
 from b200_native import NHT_FEATURE_DIM, cfg_get, nht_feature_config
-from threedgut_tracer.tracer import SplatRaster
-from train_step import TrainStep, particle_record
+from train_step import Frame, GaussianTrainStep, particle_record
 from train_step_grt import GaussianTrainStepGRT
 
 PHASES = ("render", "decode", "loss", "decode_backward", "render_backward", "exchange", "adam", "densify")
@@ -101,7 +99,6 @@ class _NHTStep:
         self.decoder = decoder
         self.decoder_weight_decay = settings["weight_decay"]
         self.color_refine_start = settings["color_refine_start"]
-        self._buffers = {}  # per resolution: the decoder's backward workspace and the [H*W,24] feature gradient
         super().__init__(params, lrs, conf=conf, **kw)
 
     def _new_optimizer(self, lrs, eps, selective):
@@ -110,9 +107,6 @@ class _NHTStep:
 
     def _new_exchange(self):
         return view_parallel.FlatGradientExchange(self.n, self.device, group=self.group, tail=self.decoder.network.params.numel())
-
-    _image_loss = GaussianTrainStepGRT._image_loss  # the decoded rgb and the render's alpha are split as on the 3DGRT layout
-    _l1_grads = GaussianTrainStepGRT._l1_grads
 
     @torch.no_grad()
     def activated(self):
@@ -192,29 +186,20 @@ class _NHTStep:
     def _decode_backward(self, features, dirs, d_rgb):
         """d_features [H*W,24]; the decoder's parameter gradient goes to the exchange buffer's tail."""
         rows = int(features.shape[0])
-        if rows not in self._buffers:
-            self._buffers = {rows: (fd.backward_workspace(self.decoder.config, rows, self.device),
-                                    torch.empty((rows, RAY_FEATURES), dtype=torch.float32, device=self.device))}
-        ws, d_features = self._buffers[rows]
+        ws, d_features = self._scratch("decode", rows, lambda: (fd.backward_workspace(self.decoder.config, rows, self.device),
+                                                                torch.empty((rows, RAY_FEATURES), dtype=torch.float32, device=self.device)))
         fd.decode_backward(features, dirs, self.decoder.network.params.data, self.decoder.config, d_rgb.reshape(rows, 3), d_features,
                            self.exchange.d_tail, ws)
         return d_features
 
 
-class GaussianTrainStepNHT(_NHTStep, TrainStep):
+class GaussianTrainStepNHT(_NHTStep, GaussianTrainStep):
     """NHT step on the 3DGUT path.  Constructor: (params, lrs, decoder, conf, **TrainStep options); `phase_events` records PHASES."""
 
-    def _init_renderer(self, conf):
-        self.raster = SplatRaster(conf)
-        self._zeros = {}
+    PHASES = PHASES
 
-    def _zero(self, H, W):
-        if (H, W) not in self._zeros:
-            self._zeros = {(H, W): torch.zeros((H, W, 1), dtype=torch.float32, device=self.device)}
-        return self._zeros[(H, W)]
-
-    def _forward(self, rays_o, rays_d, sensor, pose):
-        particles, feats = self.activated()
+    def _forward(self, view, particles, feats, train):
+        rays_o, rays_d, sensor, pose = view
         feats = self.raster._nht_features(feats)  # rounded once (fp16 under render.particle_feature_half) for the forward and the backward
         H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
         out, dst, hits, vis = self.raster.trace(self.frame, 0, particles, feats, rays_o, rays_d, None, sensor, 0, 1, pose, pose)
@@ -224,97 +209,72 @@ class GaussianTrainStepNHT(_NHTStep, TrainStep):
         dirs = world_ray_directions(c2w_rotation_from_pose7(pose), rays_d)
         rgb = self._decode(features, dirs).view(H, W, 3)
         self._mark("decode")
-        return particles, feats, out, dst, vis, features, alpha, dirs, rgb, hits
+        return Frame(rgb, 3, rgb, alpha, hits, vis, (view, particles, feats, out, dst, features, dirs))
+
+    def _backward(self, frame, d_rgb, d_alpha):
+        (rays_o, rays_d, sensor, pose), particles, feats, out, dst, features, dirs = frame.saved
+        H, W = frame.rgb.shape[:2]
+        zero = self._zeros(H, W, 1)[0]  # d_alpha on black, unmasked; d_dist always
+        d_features = self._decode_backward(features, dirs, d_rgb)
+        self._mark("decode_backward")
+        d_out = torch.cat([d_features.view(H, W, RAY_FEATURES), (zero if d_alpha is None else d_alpha).reshape(H, W, 1)], -1)
+        self.raster.trace_bwd(self.frame, 0, particles, feats, rays_o, rays_d, None, sensor, 0, 1, pose, pose, out, d_out, dst, zero,
+                              out=self.exchange.out())
+        self._mark("render_backward")
+        return ()
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, sensor, pose):
         """Forward only: (decoded rgb [H,W,3], encoded under post_processing; alpha [H,W,1])."""
-        out = self._forward(rays_o, rays_d, sensor, pose)
-        return self._post_process(out[8]), out[6]
-
-    @torch.no_grad()
-    def metrics_inputs(self, rays_o, rays_d, sensor, pose):
-        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": decoded rgb [H,W,3] before background and
-        post-processing, "alpha": [H,W,1], "hits": [H,W,1]}.  Arguments as render's; decoded with the decoder's current weights."""
-        out = self._forward(rays_o, rays_d, sensor, pose)
-        return {"pred": out[8], "alpha": out[6], "hits": out[9]}
+        f = self._forward((rays_o, rays_d, sensor, pose), *self.activated(), train=False)
+        return self._post_process(f.rgb), f.alpha
 
     @torch.no_grad()
     def step(self, rays_o, rays_d, sensor, pose, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view; arguments as GaussianTrainStep.step.  Returns this view's loss (a device scalar), the
         regularisers included while they apply."""
-        H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
-        if mask is not None:
-            mask = losses.mask_hw(mask, H, W)
-        particles, feats, out, dst, vis, features, alpha, dirs, rgb, _ = self._forward(rays_o, rays_d, sensor, pose)
-        zero1 = self._zero(H, W)
-        loss, (d_rgb, d_alpha) = self._loss((rgb, alpha, zero1), rgb, target_rgb.reshape(H, W, 3), H, W, mask)
-        self._mark("loss")
-        d_features = self._decode_backward(features, dirs, d_rgb)
-        self._mark("decode_backward")
-        d_out = torch.cat([d_features.view(H, W, RAY_FEATURES), d_alpha.reshape(H, W, 1)], -1)
-        self.raster.trace_bwd(self.frame, 0, particles, feats, rays_o, rays_d, None, sensor, 0, 1, pose, pose, out, d_out, dst, zero1,
-                              out=self.exchange.out())
-        self._mark("render_backward")
-        my_position = self.raster.sensor_position(sensor, pose, pose, W, H) if self.densifier is not None else None
-        return self._update(loss, particles, vis, all_sensor_positions, my_position)
-
-    def bytes_on_wire(self) -> int:
-        return self.exchange.bytes_on_wire()
+        return self._step((rays_o, rays_d, sensor, pose), target_rgb, all_sensor_positions, mask)
 
 
 class GaussianTrainStepGRTNHT(_NHTStep, GaussianTrainStepGRT):
     """NHT step on the 3DGRT path.  Constructor: (params, lrs, decoder, conf, **TrainStep options), conf read as threedgrt_tracer.Tracer
     reads it; `phase_events` records PHASES_GRT."""
 
-    def _forward(self, rays_o, rays_d, T_to_world, particles, feats):
-        """After the build from `particles`."""
-        ot = self.tracer.tracer_wrapper
+    PHASES = PHASES_GRT
+
+    def _forward(self, view, particles, feats, train):
+        rays_o, rays_d, T_to_world = view
         H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
-        feat, alpha, dst, nrm, hits, vis = ot.trace(self.frame, T_to_world, rays_o, rays_d, particles, feats, 0, 0, self.min_transmittance)
+        self._build(particles, train)
+        feat, alpha, dst, nrm, hits, vis = self.tracer.tracer_wrapper.trace(self.frame, T_to_world, rays_o, rays_d, particles, feats, 0, 0,
+                                                                            self.min_transmittance)
         self._mark("render")
         features = feat.view(H * W, RAY_FEATURES)
         dirs = world_ray_directions(c2w_rotation_from_T(T_to_world), rays_d)
         rgb = self._decode(features, dirs).view(H, W, 3)
         self._mark("decode")
-        return particles, feats, feat, alpha, dst, nrm, vis, dirs, rgb, hits
+        return Frame(rgb, 3, rgb, alpha[0], hits[0], vis, (view, particles, feats, feat, alpha, dst, nrm, features, dirs))
+
+    def _backward(self, frame, d_rgb, d_alpha):
+        (rays_o, rays_d, T_to_world), particles, feats, feat, alpha, dst, nrm, features, dirs = frame.saved
+        H, W = frame.rgb.shape[:2]
+        zero1, zero3 = self._zeros(H, W, 1), self._zeros(H, W, 3)
+        d_features = self._decode_backward(features, dirs, d_rgb)
+        self._mark("decode_backward")
+        self.tracer.tracer_wrapper.trace_bwd(self.frame, T_to_world, rays_o, rays_d, feat, alpha, dst, nrm, particles, feats,
+                                             d_features.view(1, H, W, RAY_FEATURES), zero1 if d_alpha is None else d_alpha, zero1, zero3, 0, 0,
+                                             self.min_transmittance, out=self.exchange.out())
+        self._mark("render_backward")
+        return ()
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, T_to_world):
         """Forward only: (decoded rgb [H,W,3], encoded under post_processing; alpha [H,W,1]).  The build it needs does not advance the
         step's BVH cadence."""
-        particles, feats = self.activated()
-        self.tracer.tracer_wrapper.build_bvh_packed(particles)
-        out = self._forward(rays_o, rays_d, T_to_world, particles, feats)
-        return self._post_process(out[8]), out[3][0]
-
-    @torch.no_grad()
-    def metrics_inputs(self, rays_o, rays_d, T_to_world):
-        """Forward only, what the test-set metrics read (metrics.image_metrics): {"pred": decoded rgb [H,W,3] before background and
-        post-processing, "alpha": [H,W,1], "hits": [H,W,1]}.  Arguments as render's; no BVH cadence is advanced."""
-        particles, feats = self.activated()
-        self.tracer.tracer_wrapper.build_bvh_packed(particles)
-        out = self._forward(rays_o, rays_d, T_to_world, particles, feats)
-        return {"pred": out[8], "alpha": out[3][0], "hits": out[9][0]}
+        f = self._forward((rays_o, rays_d, T_to_world), *self.activated(), train=False)
+        return self._post_process(f.rgb), f.alpha
 
     @torch.no_grad()
     def step(self, rays_o, rays_d, T_to_world, target_rgb, all_sensor_positions=None, mask=None):
         """One optimisation step on this rank's view; arguments as GaussianTrainStepGRT.step."""
-        H, W = int(rays_o.shape[1]), int(rays_o.shape[2])
-        if mask is not None:
-            mask = losses.mask_hw(mask, H, W)
-        particles, feats = self.activated()
-        self._build(particles)
-        self._mark("build")
-        _, _, feat, alpha, dst, nrm, vis, dirs, rgb, _ = self._forward(rays_o, rays_d, T_to_world, particles, feats)
-        zero1, zero3 = self._zero_grads(H, W)
-        loss, (d_rgb, d_alpha) = self._loss((rgb, alpha, zero1), rgb, target_rgb.reshape(H, W, 3), H, W, mask)
-        self._mark("loss")
-        d_features = self._decode_backward(feat.view(H * W, RAY_FEATURES), dirs, d_rgb)
-        self._mark("decode_backward")
-        self.tracer.tracer_wrapper.trace_bwd(self.frame, T_to_world, rays_o, rays_d, feat, alpha, dst, nrm, particles, feats,
-                                             d_features.view(1, H, W, RAY_FEATURES), d_alpha, zero1, zero3, 0, 0, self.min_transmittance,
-                                             out=self.exchange.out())
-        self._mark("render_backward")
-        my_position = self.sensor_position(T_to_world) if self.densifier is not None else None
-        return self._update(loss, particles, vis, all_sensor_positions, my_position)
+        return self._step((rays_o, rays_d, T_to_world), target_rgb, all_sensor_positions, mask)

@@ -150,14 +150,9 @@ def main():
 
     def fwd_bwd(v):
         with torch.no_grad():
-            particles, sph = st.activated()
-            pose, rgba, dst, _, sec, (so, sd, hit), _, _ = st._forward(rays_o, rays_d, sensor, poses[v], particles, sph, train=True)
-            d_rgba, d_sec = th.hybrid_composite_bwd(rgba, sec[0], hit, st.reflectivity, d_img)
-            z1, z3 = st._zero_grads(H, W)
-            st.raster.trace_bwd(st.frame, st.sph_degree, particles, sph, rays_o, rays_d, None, sensor, 0, 1, pose, pose, rgba, d_rgba, dst,
-                                torch.zeros_like(dst), out=st.exchange.out())
-            ot.trace_bwd(st.frame, st._identity, so, sd, sec[0], sec[1], sec[2], sec[3], particles, sph, d_sec, z1, z1, z3, 0, st.sph_degree,
-                         st.min_transmittance, out=st.exchange.out(), accumulate=True)
+            frame = st._forward((rays_o, rays_d, sensor, poses[v]), *st.activated(), train=True)
+            st._backward(frame, d_img, None)
+            *_, (_, _, hit) = frame.saved  # the secondary rays and their mirror hit mask
             return hit
 
     for i in range(2):
