@@ -18,6 +18,7 @@ import json
 import os
 import struct
 import zlib
+from collections.abc import Sequence
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -66,8 +67,8 @@ def _x_of(inputs, background, post_processing):
 
 def _pass(step, views, png: bool, lpips):
     """Score every view; returns (rows [F,K] numpy, render times ms [F], png bytes [(pred, target)] numpy, lpips [(v, v_cc)])."""
-    views = list(views)
-    if not views:
+    views = views if isinstance(views, Sequence) else list(views)  # a Sequence makes its items as they are read
+    if not len(views):
         raise ValueError("views: nothing to evaluate")
     dev = step.device
     rows = torch.empty((len(views), M.K), dtype=torch.float64, device=dev)
@@ -200,50 +201,31 @@ def _get(conf, path, default):
     return cfg_get(conf, path, default)
 
 
-def _decoder_from(arch: dict, conf, device):
-    import feature_decoder as fd
-
-    return fd.FeatureDecoder(int(arch["ray_feature_dim"]), hidden_dim=int(arch["hidden_dim"]), num_layers=int(arch["num_layers"]),
-                             dir_encoding=str(_get(conf, "model.nht_decoder.dir_encoding", "SphericalHarmonics")),
-                             dir_encoding_degree=int(_get(conf, "model.nht_decoder.dir_encoding_degree", 3)), sh_scale=float(arch["sh_scale"]),
-                             output_activation=str(arch["output_activation"]), unpremultiply_alpha=bool(arch.get("unpremultiply_alpha", False))
-                             ).to(device)
-
-
 def from_checkpoint(path: str, conf=None, device="cuda"):
     """A training step holding the scene of the `ckpt_*.pt` at `path` (written by checkpoint.save or by the reference trainer), built
     from its `config` (or `conf`) as evaluation renders it: render.method 3dgut or 3dgrt (with eval_config's overrides), SH or NHT
     features, the model's background colour and post-processing.  Returns the step; score it with evaluate / validate."""
     import checkpoint
+    import step_config
 
     device = torch.device(device)
     ckpt = torch.load(path, map_location=device, weights_only=False)
     conf = eval_config(conf if conf is not None else ckpt.get("config"))
     ft = str(_get(conf, "model.feature_type", "sh")).lower()
     state = checkpoint.from_reference_layout(ckpt, feature_type=ft)
-    method = str(_get(conf, "render.method", "3dgut")).lower()
     settings = state.get("settings") or {}
     bg = settings.get("background", _get(conf, "model.background.color", "black"))
-    kw = dict(background=bg, post_processing=_get(conf, "post_processing.method", None), sph_degree=None)
     params = {k: v.detach().to(device=device, dtype=torch.float32).contiguous() for k, v in state["params"].items()}
     lrs = {k: float(v) for k, v in state["lrs"].items()}
     if ft == "nht":
-        import train_step_nht as tsn
-
         dec = state["decoder"]
-        decoder = _decoder_from(dec["arch"], conf, device)
-        kw.pop("sph_degree")
-        cls = tsn.GaussianTrainStepGRTNHT if method == "3dgrt" else tsn.GaussianTrainStepNHT
-        step = cls(params, lrs, decoder, conf, **kw)
+        decoder = step_config.make_decoder(conf, device, arch=dec["arch"])
+        step = step_config.build_step(conf, params, 1.0, lrs=lrs, decoder=decoder, background=bg, train=False)
         decoder.network.params.data.copy_(dec["params"])
         if dec["ema"]:
             decoder.load_ema_state_dict({k: v.to(device) for k, v in dec["ema"].items()})
     else:
-        if method == "3dgrt":
-            from train_step_grt import GaussianTrainStepGRT as cls
-        else:
-            from train_step import GaussianTrainStep as cls
-        kw["sph_degree"] = int(state.get("sph_degree") if state.get("sph_degree") is not None else 3)
-        step = cls(params, lrs, conf=conf, **kw)
+        sph = int(state.get("sph_degree") if state.get("sph_degree") is not None else 3)
+        step = step_config.build_step(conf, params, 1.0, lrs=lrs, sph_degree=sph, background=bg, train=False)
     step.frame = int(state["frame"])
     return step
