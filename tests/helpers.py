@@ -98,16 +98,183 @@ def oracle_frame(sc, c2w, seed=0, pose=None, with_f64=False, d_dist="random", d_
     cfg = go.default_config()
     cam, pose = oracle_camera(sc, c2w, pose)
     ro, rd = sc.rays()
-    pr, bn, rgba, dist, hits = go.forward_all(cfg, cam, ro, rd, sc.particles, sc.sph, sc.sph_degree)
-    d_rgba, d_dist = output_grads(rgba.shape, seed, d_dist, d_alpha)
-    dp, ds = go.render_backward(cfg, cam, ro, rd, sc.particles, sc.sph, sc.sph_degree, pr, bn, rgba, dist, d_rgba, d_dist)
-    out = dict(cfg=cfg, cam=cam, pose=pose, ro=ro, rd=rd, pr=pr, bn=bn, rgba=rgba, dist=dist, hits=hits, d_rgba=d_rgba,
-               d_dist=d_dist, dp=dp, ds=ds)
-    if with_f64:
-        r64, d64, h64 = go.render_forward(cfg, cam, ro, rd, sc.particles, pr, bn, f64=True)
-        dp64, ds64 = go.render_backward(cfg, cam, ro, rd, sc.particles, sc.sph, sc.sph_degree, pr, bn, r64, d64, d_rgba, d_dist, f64=True)
-        out.update(rgba_64=r64, dist_64=d64, hits_64=h64, dp_64=dp64, ds_64=ds64)
+    pr = go.project(cfg, cam, sc.particles, sc.sph, sc.sph_degree)
+    bn = go.bin_tiles(cfg, cam, pr)
+    d_rgba, d_dist = output_grads((cam.height, cam.width, 4), seed, d_dist, d_alpha)
+    out = oracle_on_lists(cfg, cam, ro, rd, sc.particles, sc.sph, sc.sph_degree, pr, bn, d_rgba, d_dist, with_f64=with_f64)
+    out.update(cfg=cfg, cam=cam, pose=pose, ro=ro, rd=rd, pr=pr, bn=bn, d_rgba=d_rgba, d_dist=d_dist)
     return out
+
+
+def oracle_on_lists(cfg, cam, ro, rd, particles, sph, sph_degree, pr, bn, d_rgba, d_dist, k=0, with_f64=True, spreads=False):
+    """The oracle's forward (rgba, dist, hits) and backward (dp, ds) over the lists of the binning `bn`, with the radiance and tile counts
+    of the projection `pr`; with_f64 adds the float64 evaluation of the compositing on the same lists (keys *_64), the yardstick of the
+    gradient bar; spreads adds "spreads": the (dp, ds) of that and of the float32 oracle with nudged_configs, for check_gradients.  k > 0:
+    the sorted variant with a buffer of k hits."""
+    out = {}
+    if spreads:
+        out["spreads"] = [oracle_on_lists(c, cam, ro, rd, particles, sph, sph_degree, pr, bn, d_rgba, d_dist, k, with_f64=False)
+                          for c in nudged_configs(cfg)]
+        out["spreads"] = [(o["dp"], o["ds"]) for o in out["spreads"]]
+    for f64 in (False, True) if with_f64 else (False,):
+        if k:
+            rgba, dist, hits = go.render_forward_kbuffer(cfg, cam, k, ro, rd, particles, pr, bn, f64=f64)
+            dp, ds = go.render_backward_kbuffer(cfg, cam, k, ro, rd, particles, sph, sph_degree, pr, bn, rgba, dist, d_rgba, d_dist, f64=f64)
+        else:
+            rgba, dist, hits = go.render_forward(cfg, cam, ro, rd, particles, pr, bn, f64=f64)
+            dp, ds = go.render_backward(cfg, cam, ro, rd, particles, sph, sph_degree, pr, bn, rgba, dist, d_rgba, d_dist, f64=f64)
+        sfx = "_64" if f64 else ""
+        out.update({"rgba" + sfx: rgba, "dist" + sfx: dist, "hits" + sfx: hits, "dp" + sfx: dp, "ds" + sfx: ds})
+    if spreads:
+        out["spreads"].append((out["dp_64"], out["ds_64"]))
+    return out
+
+
+def nudged_configs(cfg, rel=5e-5):
+    """Two copies of the oracle config `cfg` with the accept thresholds (min_kernel_density, min_alpha) and the early stop
+    (min_transmittance) moved by -rel and +rel of their values.  The oracle run with them changes the gradient of exactly the particles
+    with a (pixel, particle) pair on the edge of a decision, which the render kernels' approximate exp may take the other way even where
+    the oracle's float32 and float64 evaluations agree."""
+    out = []
+    for s in (-rel, rel):
+        c = type(cfg).from_buffer_copy(cfg)
+        for f in ("min_kernel_density", "min_alpha", "min_transmittance"):
+            setattr(c, f, getattr(c, f) * (1.0 + s))
+        out.append(c)
+    return out
+
+
+GRAD_COLS = dict(pos=slice(0, 3), dns=slice(3, 4), quat=slice(4, 8), scl=slice(8, 11))
+
+
+def check_gradients(label, dp, ds, ref, spreads):
+    """The gradient bar of test_gut_headline_parity_gpu.py against the oracle's (ref_dp, ref_ds) = `ref`, with the oracle's own spread
+    taken over several evaluations on the same lists, `spreads` = [(dp, ds), ...] (float32 against float64, nudged_configs).  Per tensor
+    (pos, density, quat, scale, sph): err <= max(1e-3, 1.5 x the largest spread), and err <= 1e-3 once the ten particles whose gradient
+    moves most across those evaluations are left out -- picked from the oracle, never from the output under test."""
+    rdp, rds = np.asarray(ref[0], np.float64), np.asarray(ref[1], np.float64)
+    pairs = {k: (dp[:, v], rdp[:, v]) for k, v in GRAD_COLS.items()}
+    pairs["sph"] = (ds, rds)
+    errs = {k: rel_l2(a, b) for k, (a, b) in pairs.items()}
+    yard = {k: max(rel_l2(b if k == "sph" else a[:, GRAD_COLS[k]], pairs[k][1]) for a, b in spreads) for k in pairs}
+    e2 = np.zeros(len(dp))
+    for a, b in spreads:
+        e2 = np.maximum(e2, ((np.asarray(a, np.float64)[:, 0:11] - rdp[:, 0:11]) ** 2).sum(1) / max(float((rdp[:, 0:11] ** 2).sum()), 1e-300)
+                        + ((np.asarray(b, np.float64) - rds) ** 2).sum(1) / max(float((rds ** 2).sum()), 1e-300))
+    keep = np.ones(len(dp), bool)
+    keep[np.argsort(-e2)[:10]] = False
+    robust = {k: rel_l2(a[keep], b[keep]) for k, (a, b) in pairs.items()}
+    fmt = lambda d: {k: f"{v:.2e}" for k, v in d.items()}  # noqa: E731
+    print(f"[gradients] {label} rel-L2 vs oracle: {fmt(errs)}; oracle spread (bar max(1e-3, 1.5 x)): {fmt(yard)}; without the oracle's "
+          f"10 most unsettled particles (bar 1e-3): {fmt(robust)}")
+    for k in errs:
+        assert errs[k] <= max(1e-3, 1.5 * yard[k]), (k, errs[k], yard[k])
+        assert robust[k] <= 1e-3, (k, robust[k])
+
+
+def binning_from_lists(sorted_keys, sorted_values, ranges):
+    """An oracle Binning over sorted tile lists made elsewhere (the GPU's: gpu_binning).  The oracle's renders read only `sorted_values`
+    and `ranges` of a Binning (gut_oracle.c: gut_oracle_render_forward*, render_backward_impl).  The key fields hold the lists' own
+    (tile << 32 | depth bits) keys, sorted and unsorted alike: the order the lists were binned in is not known, and no render reads it."""
+    keys, values = np.asarray(sorted_keys, np.uint64), np.asarray(sorted_values, np.uint32)
+    return go.Binning(unsorted_keys=keys.copy(), unsorted_values=values.copy(), sorted_keys=keys, sorted_values=values,
+                      ranges=np.ascontiguousarray(ranges, np.uint32))
+
+
+def gpu_binning(ctx):
+    """The sorted tile lists the last forward of the native context `ctx` walked, as an oracle Binning.  DBG_SORTED_KEYS are the
+    reference's 64-bit keys, rebuilt on the device from the tile ranges, the sorted values and the depths."""
+    import b200_native as nat
+
+    return binning_from_lists(ctx.debug_copy(nat.DBG_SORTED_KEYS), ctx.debug_copy(nat.DBG_SORTED_VALUES), ctx.debug_copy(nat.DBG_TILE_RANGES))
+
+
+def sh_radiance(cam, particles, sph, sph_degree, rows):
+    """[len(rows), 3] radiance of the particles `rows` as gut_oracle_project evaluates it: the SH along the float32 unit direction from the
+    camera position (gut_oracle_sensor_matrices) to the particle, whatever the sensor model."""
+    campos = go.sensor_matrices(cam)[2]
+    out = np.zeros((len(rows), 3), np.float32)
+    for j, i in enumerate(rows):
+        s = np.asarray(particles[i, 0:3], np.float32) - campos
+        dist = np.sqrt(s[0] * s[0] + s[1] * s[1] + s[2] * s[2])
+        out[j] = go.sph_eval(sph_degree, sph[i], s / dist)
+    return out
+
+
+def projection_for_lists(pr, tiles_count, cam, particles, sph, sph_degree):
+    """The oracle's projection `pr` with the tile counts `tiles_count` of other lists (the GPU's).  The renders read two fields of a
+    Projection: the radiance `rgb`, and in the backward whether a particle's count is non-zero (only counted particles get the SH adjoint).
+    The oracle leaves the radiance zero where its own count is zero, so the particles only the other lists count get theirs from
+    sh_radiance.  The conic, extent and depth stay the oracle's: the renders evaluate each particle in 3D and never read them."""
+    tiles_count = np.asarray(tiles_count, np.uint32)
+    rgb = pr.rgb.copy()
+    extra = np.flatnonzero((tiles_count > 0) & (pr.tiles_count == 0))
+    if extra.size:
+        rgb[extra] = sh_radiance(cam, particles, sph, sph_degree, extra)
+    return dataclasses.replace(pr, tiles_count=tiles_count, rgb=rgb)
+
+
+FISHEYE_K = (0.04, -0.012, 0.003, -0.0006)    # the k1..k4 of test_scene_cameras_gpu.FISHEYE_FULL
+OPENCV_K = (-0.08, 0.015, 0.0012, -0.0009)    # the k1, k2, p1, p2 of test_scene_cameras_gpu.OPENCV_FULL
+
+
+def ftheta_sensor(width, height, reference_poly):
+    """An f-theta sensor whose polynomials use all six coefficients, so that every order of both shows in the projection.  The forward
+    polynomial is only roughly the backward one's inverse; its last coefficient moves a particle by a pixel at the edge of the frame."""
+    f = 0.9 * width
+    return dict(reference_poly=reference_poly, bw=[0.0, 1.0 / f, 0.0, 0.04 / f ** 3, 0.0, 0.01 / f ** 5],
+                fw=[0.0, f, 0.0, -0.04 * f, 0.0, 0.02 * f], cde=[1.0, 0.001, -0.002], max_angle=1.0,
+                principal=(width / 2.0 - 0.5, height / 2.0 - 0.5))
+
+
+def colmap_sensor(name, width, height, fx):
+    """(COLMAP camera model, its parameters) of the "opencv" (distorted pinhole of focal length fx) or "fisheye" sensor of a
+    width x height frame, principal points off centre."""
+    if name == "opencv":
+        return "OPENCV", [fx, fx, width / 2 + 0.4, height / 2 - 0.4, *OPENCV_K]
+    return "OPENCV_FISHEYE", [0.47 * width, 0.48 * width, width / 2 - 0.8, height / 2 + 0.8, *FISHEYE_K]
+
+
+SENSORS = ("opencv", "fisheye", "ftheta_bw", "ftheta_fw", "rs1", "rs2", "rs3", "rs4", "rs1_fisheye")
+
+
+def sensor_frame(name, width=128, height=128):
+    """(scene, oracle camera, rays_o, rays_d) of the C1 scene seen through the sensor `name` of SENSORS:
+      opencv       OpenCV pinhole with k1, k2, p1, p2 (COLMAP's OPENCV model), rays from the dataset's Newton inversion;
+      fisheye      OpenCV fisheye (OPENCV_FISHEYE) of about 1.5 rad half-angle, from an orbit close enough to the scene that particles
+                   reach beyond 1 rad off axis, where the high-order terms move them by a fraction of a pixel;
+      ftheta_bw/fw f-theta with the backward / forward polynomial as the reference (ftheta_sensor);
+      rs1..rs4     pinhole with a rolling shutter read out top to bottom, left to right, bottom to top, right to left, the sensor moving
+                   between two orbit cameras during the exposure;
+      rs1_fisheye  the fisheye above with the top-to-bottom rolling shutter."""
+    import scene_data
+
+    sc = scenes.scene_c1(width=width, height=height)
+    fisheye = name in ("fisheye", "rs1_fisheye")
+    if fisheye:
+        sc = dataclasses.replace(sc, camera_radius=2.5)
+    rolling = int(name[2]) if name.startswith("rs") else 0
+    if rolling:
+        p0, p1 = scenes.pose7_from_c2w(sc.camera(1, 40)), scenes.pose7_from_c2w(sc.camera(2, 40))
+    else:
+        p0 = p1 = scenes.pose7_from_c2w(sc.camera(5 if name == "opencv" else 1, 10))
+    if name.startswith("ftheta"):
+        ft = ftheta_sensor(width, height, 0 if name == "ftheta_bw" else 1)
+        cam = go.make_camera(width, height, 1.0, 1.0, 0.0, 0.0, p0, p1, ftheta=ft)
+        ro, rd = scenes.ftheta_rays(height, width, ft)
+        return dataclasses.replace(sc, fx=1.0, fy=1.0, ftheta=ft), cam, ro, rd
+    if fisheye or name == "opencv":
+        sensor = scene_data.colmap_camera(*colmap_sensor("fisheye" if fisheye else "opencv", width, height, sc.fx), width, height, 1)
+    else:
+        sensor = scene_data.colmap_camera("PINHOLE", [sc.fx, sc.fy, sc.cx, sc.cy], width, height, 1)
+    p = sensor.params
+    cam = go.make_camera(width, height, p["fx"], p["fy"], p["cx"], p["cy"], p0, p1, rolling_shutter=rolling,
+                         fisheye=(*p["radial"][:4], p["max_angle"]) if fisheye else None)
+    if name == "opencv":
+        cam.radial[:] = [float(v) for v in p["radial"]]
+        cam.tangential[:] = [float(v) for v in p["tangential"]]
+    ro, rd = sensor.host_rays()
+    return sc, cam, ro, rd
 
 
 def kbuffer_premises(label, cfg, cam, k, ro, rd, particles, pr, bn, hits):
