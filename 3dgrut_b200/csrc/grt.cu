@@ -160,22 +160,22 @@ __global__ void __launch_bounds__(256) proxy_kernel(int n, const float* __restri
     scene_box_extend(scene, b.lo.x, b.lo.y, b.lo.z, b.hi.x, b.hi.y, b.hi.z);
 }
 
-// size_levels > 0: the two top bits of the key are a size class of the proxy (radius relative to the scene diagonal), so the LBVH
-// splits the particles by size first and each class gets its own spatial subtree -- large proxies no longer inflate the boxes of
-// the subtrees that hold the many small ones (the crudest form of the "extended Morton code").
+// The two top bits of the key are a size class of the proxy (radius relative to the scene diagonal), so the LBVH splits the particles
+// by size first and each class gets its own spatial subtree -- large proxies no longer inflate the boxes of the subtrees that hold
+// the many small ones (the crudest form of the "extended Morton code").  Class 0: rel < kSmallProxy, class 1: the rest; a zero scene
+// diagonal (rel NaN or infinite) gives class 3.
+constexpr float kSmallProxy = 1.f / 48.f;
+
 __global__ void __launch_bounds__(256) morton_kernel(int n, const Proxy* __restrict__ proxies, const Box* __restrict__ boxes,
-                                                     const int* __restrict__ scene, int size_levels, float t0, float t1, float t2,
-                                                     uint32_t* __restrict__ codes, uint32_t* __restrict__ ids) {
+                                                     const int* __restrict__ scene, uint32_t* __restrict__ codes,
+                                                     uint32_t* __restrict__ ids) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const SceneBox sb = scene_box(scene);
     const Proxy p = proxies[i];
-    uint32_t cls = 0;
-    if (size_levels > 0) {
-        const float diag = sqrtf(sb.ex * sb.ex + sb.ey * sb.ey + sb.ez * sb.ez);
-        const float rel = boxes[i].lo.w / diag;   // proxy radius / scene diagonal
-        cls = rel < t0 ? 0u : (rel < t1 ? 1u : (rel < t2 ? 2u : 3u));
-    }
+    const float diag = sqrtf(sb.ex * sb.ex + sb.ey * sb.ey + sb.ez * sb.ez);
+    const float rel = boxes[i].lo.w / diag;   // proxy radius / scene diagonal
+    const uint32_t cls = rel < kSmallProxy ? 0u : (rel < 3e38f ? 1u : 3u);
     codes[i] = (cls << 30) | morton30(sb, p.a0.w, p.a1.w, p.a2.w);
     ids[i] = static_cast<uint32_t>(i);
 }
@@ -183,6 +183,9 @@ __global__ void __launch_bounds__(256) morton_kernel(int n, const Proxy* __restr
 // Leaves hold up to `leaf` consecutive particles of the sorted order: one thread per leaf writes the leaf's key (its first particle's),
 // its box (union) and the particles' proxies in leaf order.  Fewer, fatter leaves remove the bottom levels of the tree, where most
 // node visits happen; the particles of a leaf are tested back to back from one 64*leaf-byte record.
+// kLeaf particles per leaf: C4 on an H100 80GB HBM3 (700 W), bench.py --workload c4 --steps 30, two runs each: 1 -> 109.8,
+// 2 -> 112.0, 4 -> 108.6, 8 -> 98.9 frames/s
+constexpr int kLeaf = 2;
 __global__ void __launch_bounds__(256) leaf_kernel(int n, int leaf, const uint32_t* __restrict__ codes_sorted,
                                                    const uint32_t* __restrict__ ids_sorted, const Proxy* __restrict__ proxies,
                                                    const Box* __restrict__ boxes, uint32_t* __restrict__ leaf_codes,
@@ -229,7 +232,6 @@ __global__ void single_leaf_kernel(const Box* __restrict__ leaf_boxes, BvhNode* 
 struct TraceParams {
     int n, width, height, batch;   // rays are [batch, height, width, 3]
     int sph_degree;
-    int packet;                    // 1: coherent warps traverse as a packet (GRTB200_PACKET=0 turns it off for A/B runs)
     float min_transmittance, min_response, min_alpha, max_alpha;
     float r2w[12];                 // row-major 3x4
     float scene[6];
@@ -852,7 +854,7 @@ __global__ void __launch_bounds__(128, kTraceBlocksPerSm) trace_kernel(TracePara
     const float ex = P.scene[3] - P.scene[0], ey = P.scene[4] - P.scene[1], ez = P.scene[5] - P.scene[2];
     const float sx = ox - gx, sy = oy - gy, sz = oz - gz;
     const bool near_first = (dot > 0.f) && (dot * dot > 0.99f * n1 * n0) && (sx * sx + sy * sy + sz * sz <= 4e-4f * (ex * ex + ey * ey + ez * ez));
-    const bool coherent = P.packet && __all_sync(0xFFFFFFFFu, near_first);
+    const bool coherent = __all_sync(0xFFFFFFFFu, near_first);
     if (coherent) {
         trace_rays<PRIM, DEG, BWD, true, COUNT, FK>(P, r, warp_stack, feat);
     } else if (COUNT || r.valid) {   // the counting pass ends in warp shuffles: every lane takes part
@@ -892,7 +894,6 @@ struct grtb200_ctx {
          *codes_sorted = nullptr, *ids_sorted = nullptr, *children = nullptr, *parent = nullptr, *leaf_parent = nullptr, *flags = nullptr,
          *scene = nullptr, *sort_temp = nullptr, *grp_codes = nullptr, *grp_ids = nullptr, *grp_boxes = nullptr, *grp_proxies = nullptr;
     size_t cap = 0, sort_temp_bytes = 0;
-    int leaf = 2;   // particles per leaf of the last build
     // hit-list cache of the last forward (see TraceParams)
     void *hit_list = nullptr, *hit_count = nullptr;
     size_t hit_list_bytes = 0, hit_count_bytes = 0;
@@ -958,10 +959,6 @@ int fill_params(grtb200_ctx* c, TraceParams& P, int64_t n, const float* particle
     P.height = height;
     P.batch = batch;
     P.sph_degree = sph_degree;
-    {
-        const char* e = std::getenv("GRTB200_PACKET");
-        P.packet = (e && e[0] == '0') ? 0 : 1;
-    }
     P.min_transmittance = min_t;
     P.min_response = c->cfg.min_response;
     P.min_alpha = c->cfg.min_alpha;
@@ -973,7 +970,7 @@ int fill_params(grtb200_ctx* c, TraceParams& P, int64_t n, const float* particle
     P.rays_o = rays_o;
     P.rays_d = rays_d;
     P.proxies = static_cast<const LeafProxy*>(c->grp_proxies);
-    P.leaf = c->leaf;
+    P.leaf = kLeaf;
     P.nodes = static_cast<const BvhNode*>(c->nodes);
     return 0;
 }
@@ -1129,28 +1126,13 @@ static int build_bvh(grtb200_ctx* c, void* stream, int64_t n, const float* pos, 
                                                         static_cast<int*>(c->scene));
     c->launches++;
     {
-        int size_levels = 1;
-        float th[3] = {1.f / 48.f, 3e38f, 3e38f};  // proxy radius / scene diagonal; classes above the last finite threshold stay empty
-        int leaf = 2;  // particles per leaf (GRTB200_LEAF overrides it); C4 on an H100 80GB HBM3 (700 W), bench.py --workload c4
-                       // --steps 30, two runs each: 1 -> 109.8, 2 -> 112.0, 4 -> 108.6, 8 -> 98.9 frames/s
-        if (const char* e = std::getenv("GRTB200_SIZE_LEVELS")) size_levels = std::atoi(e);  // A/B switches for profiling
-        if (const char* e = std::getenv("GRTB200_SIZE_T")) {
-            float a = 0.f, b = 0.f, d = 0.f;
-            const int got = std::sscanf(e, "%f,%f,%f", &a, &b, &d);
-            th[0] = got >= 1 && a > 0.f ? 1.f / a : 3e38f;
-            th[1] = got >= 2 && b > 0.f ? 1.f / b : 3e38f;
-            th[2] = got >= 3 && d > 0.f ? 1.f / d : 3e38f;
-        }
-        if (const char* e = std::getenv("GRTB200_LEAF")) leaf = std::max(1, std::min(16, std::atoi(e)));
-        c->leaf = leaf;
-        const int ng = (ni + leaf - 1) / leaf;
+        const int ng = (ni + kLeaf - 1) / kLeaf;
         const unsigned gblocks = (ng + 255) / 256;
         morton_kernel<<<blocks, 256, 0, s>>>(ni, static_cast<const Proxy*>(c->proxies), static_cast<const Box*>(c->leaf_boxes),
-                                             static_cast<const int*>(c->scene), size_levels, th[0], th[1], th[2],
-                                             static_cast<uint32_t*>(c->codes), static_cast<uint32_t*>(c->ids));
+                                             static_cast<const int*>(c->scene), static_cast<uint32_t*>(c->codes), static_cast<uint32_t*>(c->ids));
         run_sort32_pairs(s, c->sort_temp, c->sort_temp_bytes, static_cast<const uint32_t*>(c->codes), static_cast<uint32_t*>(c->codes_sorted),
                          static_cast<const uint32_t*>(c->ids), static_cast<uint32_t*>(c->ids_sorted), n, 32);
-        leaf_kernel<<<gblocks, 256, 0, s>>>(ni, leaf, static_cast<const uint32_t*>(c->codes_sorted), static_cast<const uint32_t*>(c->ids_sorted),
+        leaf_kernel<<<gblocks, 256, 0, s>>>(ni, kLeaf, static_cast<const uint32_t*>(c->codes_sorted), static_cast<const uint32_t*>(c->ids_sorted),
                                             static_cast<const Proxy*>(c->proxies), static_cast<const Box*>(c->leaf_boxes),
                                             static_cast<uint32_t*>(c->grp_codes), static_cast<uint32_t*>(c->grp_ids),
                                             static_cast<Box*>(c->grp_boxes), static_cast<LeafProxy*>(c->grp_proxies));

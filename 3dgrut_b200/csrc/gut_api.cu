@@ -9,7 +9,6 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <new>
 #include <string>
@@ -272,8 +271,8 @@ int check_args(gutb200_ctx* c, const gutb200_camera* cam, int64_t n, const void*
     if (reinterpret_cast<uintptr_t>(particles) & 15) return fail(c, "particle buffer must be 16-byte aligned");
     if (c->cfg.k_buffer_size < 0 || c->cfg.k_buffer_size > 16) return fail(c, "k_buffer_size %d out of range (0..16)", c->cfg.k_buffer_size);
     if (c->cfg.kernel_degree != 2 && c->cfg.kernel_degree != 4) return fail(c, "kernel_degree %d not built (2 or 4)", c->cfg.kernel_degree);
-    if (((c->cfg.subtile_culling >> 4) & 3) == 3)
-        return fail(c, "subtile_culling sub-block code 3 (bits 4-5) not built (0 = quarter-warps, 1 = half-warps, 2 = whole warps)");
+    if (const int code = (c->cfg.subtile_culling >> 4) & 3)
+        return fail(c, "subtile_culling sub-block code %d (bits 4-5) not built: only 0 (quarter-warps) is", code);
     return 0;
 }
 
@@ -355,7 +354,6 @@ void gutb200_default_config(gutb200_config* c) {  // configs/render/3dgut.yaml, 
     c->subtile_culling = 7;  // bit 1: sub-tile screens in render; bit 2: renderBackward walks the forward's hit words (bit 0: unused since round 2)
     c->n_rolling_shutter_iterations = 5;  // configs/render/3dgut.yaml:18
     c->k_buffer_size = 0;                 // configs/render/3dgut.yaml: k_buffer_size 0 (unsorted)
-    if (const char* e = std::getenv("GUTB200_SUBTILE_CULLING")) c->subtile_culling = std::atoi(e);  // A/B switch for profiling
 }
 
 int gutb200_create(const gutb200_config* cfg, int device, gutb200_ctx** out) {

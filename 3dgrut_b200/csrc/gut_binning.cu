@@ -18,8 +18,6 @@
 // The keys are unique inside a tile (a particle enters a tile once), so the result is exactly the reference's order whatever order
 // the atomics claimed the slots in; only sorted artefacts are observable and they stay bit-identical (tests/test_gut_parity_gpu.py).
 // Work: I x 8 B written once, sorted in place on chip; no N-sized depth sort, no scan over N, no multi-pass radix sort over I.
-#include <cstdlib>
-
 #include "gut_common.cuh"
 
 namespace gutb200 {
@@ -232,23 +230,18 @@ __device__ __forceinline__ bool scan_digits(uint32_t (*s_cnt)[256], uint32_t* s_
 }
 
 // Slot of this lane's key among the warp's 32 (in lane order, so the pass is stable); `have` is warp-divergent, the call warp-uniform.
-template <bool BALLOT>
 __device__ __forceinline__ uint32_t rank_key(uint32_t* cnt_row, unsigned long long k, int shift, bool have) {
     const int lane = threadIdx.x & 31;
     const uint32_t dg = have ? (static_cast<uint32_t>(k >> shift) & 255u) : 256u + lane;  // idle lanes: unique pseudo-digits
-    unsigned peers;
-    if (BALLOT) {  // lanes with the same 8-bit digit, from one ballot per bit (the multi-split CUB's ranking uses)
-        peers = __ballot_sync(kFullMask, have);
+    // lanes with the same 8-bit digit, from one ballot per bit (the multi-split CUB's ranking uses)
+    unsigned peers = __ballot_sync(kFullMask, have);
 #pragma unroll
-        for (int b = 0; b < 8; ++b) {
-            const bool bit = (dg >> b) & 1u;
-            const unsigned bal = __ballot_sync(kFullMask, bit);
-            peers &= bit ? bal : ~bal;
-        }
-        if (!have) peers = 1u << lane;
-    } else {
-        peers = __match_any_sync(kFullMask, dg);
+    for (int b = 0; b < 8; ++b) {
+        const bool bit = (dg >> b) & 1u;
+        const unsigned bal = __ballot_sync(kFullMask, bit);
+        peers &= bit ? bal : ~bal;
     }
+    if (!have) peers = 1u << lane;
     const int leader = __ffs(peers) - 1;
     uint32_t slot = 0;
     if (have && lane == leader) slot = atomicAdd(&cnt_row[dg], static_cast<uint32_t>(__popc(peers)));
@@ -364,7 +357,6 @@ __device__ __forceinline__ bool bucket_pass(const unsigned long long* __restrict
     return false;
 }
 
-template <bool BALLOT>
 __global__ void __launch_bounds__(kSortThreads) tile_sort_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ ranges,
                                                                  const uint32_t* __restrict__ totals, unsigned long long* keys,
                                                                  unsigned long long* keys_alt, uint32_t* __restrict__ sorted_values) {
@@ -407,7 +399,7 @@ __global__ void __launch_bounds__(kSortThreads) tile_sort_kernel(const uint32_t*
             for (int u = 0; u < kStagePerLane; ++u) {   // 32 keys at a time, in order: the pass is stable
                 if (w0 + u * 32 >= w1) break;           // warp-uniform
                 const bool have = w0 + u * 32 + lane < w1;
-                const uint32_t slot = rank_key<BALLOT>(s_cnt[warp], k[u], shift, have);
+                const uint32_t slot = rank_key(s_cnt[warp], k[u], shift, have);
                 if (have) s_keys[slot] = k[u];
             }
             __syncthreads();   // the counters are zeroed next: every warp is done claiming slots
@@ -446,7 +438,7 @@ __global__ void __launch_bounds__(kSortThreads) tile_sort_kernel(const uint32_t*
             for (int u = 0; u < kSortUnroll; ++u) {   // 32 keys at a time, in order: the pass is stable
                 if (i0 + u * 32 >= w1) break;         // warp-uniform
                 const bool have = i0 + u * 32 + lane < w1;
-                const uint32_t slot = rank_key<BALLOT>(s_cnt[warp], k[u], shift, have);
+                const uint32_t slot = rank_key(s_cnt[warp], k[u], shift, have);
                 if (have) dst[slot] = k[u];
             }
         }
@@ -485,19 +477,12 @@ void launch_tile_scan(cudaStream_t s, int num_tiles, const uint32_t* counts, uin
 cudaError_t launch_tile_sort(cudaStream_t s, int num_tiles, const uint32_t* order, const uint32_t* ranges, const uint32_t* totals,
                              unsigned long long* keys, unsigned long long* keys_alt, uint32_t* sorted_values) {
     if (num_tiles <= 0) return cudaSuccess;
-    static const bool use_match = [] { const char* e = std::getenv("GUTB200_SORT_MATCH"); return e && std::atoi(e) != 0; }();  // A/B switch
     constexpr size_t kStageBytes = kStageKeys * sizeof(unsigned long long);
-    static const cudaError_t opt_in = [] {   // static + dynamic shared memory exceeds the default 48 KB per CTA
-        cudaError_t e = cudaFuncSetAttribute(tile_sort_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kStageBytes));
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(tile_sort_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kStageBytes));
-        return e;
-    }();
+    // static + dynamic shared memory exceeds the default 48 KB per CTA
+    static const cudaError_t opt_in =
+        cudaFuncSetAttribute(tile_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kStageBytes));
     if (opt_in != cudaSuccess) return opt_in;
-    if (use_match)
-        tile_sort_kernel<false><<<num_tiles, kSortThreads, kStageBytes, s>>>(order, ranges, totals, keys, keys_alt, sorted_values);
-    else
-        tile_sort_kernel<true><<<num_tiles, kSortThreads, kStageBytes, s>>>(order, ranges, totals, keys, keys_alt, sorted_values);
+    tile_sort_kernel<<<num_tiles, kSortThreads, kStageBytes, s>>>(order, ranges, totals, keys, keys_alt, sorted_values);
     return cudaGetLastError();
 }
 

@@ -123,10 +123,10 @@ __global__ void __launch_bounds__(kTilePixels) render_forward_kernel(FrameCamera
 //   every lane stores its row (g[0..15], the depth slots 16..18 when the warp carries a distance gradient; zeros without a hit) as
 //   float4 at a stride of kGradRow floats -- 8 consecutive lanes then hit 8 distinct 16-byte bank groups, so the stores are
 //   conflict-free --, and lane r (r < 5, or < 4 without depth slots) of each sub-block sums float4 column r over the sub-block's
-//   rows and lands it with one 16-byte vector RED.  For SUBL 8 and 16 the readers of one lane octet read two rows 4 lanes apart,
-//   columns 0..3: 16-byte groups 5 row + r and 5 row + 20 + r are again 8 distinct ones.
+//   rows and lands it with one 16-byte vector RED.  The readers of one lane octet read two rows 4 lanes apart, columns 0..3:
+//   16-byte groups 5 row + r and 5 row + 20 + r are again 8 distinct ones.
 // This replaced a transposing butterfly over the sub-block (14 SHFL + 14 FADD + ~28 SEL per lane, 3 more 5-level sums for the depth
-// slots and a second RED): 5 STS.128 + SUBL LDS.128 on the summing lanes, 5 REDs per flushed row instead of 9 (4 instead of 8 without
+// slots and a second RED): 5 STS.128 + 8 LDS.128 on the summing lanes, 5 REDs per flushed row instead of 9 (4 instead of 8 without
 // the depth slots).  render_backward on C2 (H100 80GB HBM3, 700 W, 1980 MHz, three runs each): 0.454-0.460 -> 0.417-0.422 ms; with the rgb / opacity
 // loss (no depth slots) unchanged at 0.354-0.358 ms.
 
@@ -136,24 +136,15 @@ struct BwdSmem : BwdRecords<kBatch> {
     float4 rows[kTilePixels / 32][32 * kGradRow / 4];  // gradient rows of one lockstep iteration, [warp][lane * 5 + column]
 };
 
-// Sub-blocks of SUBL lanes (32: the warp, 16: half = 4x4 pixels, 8: quarter = 4x2 pixels): the sub-block id uses lane bits b2 (and
-// b4), the lanes within it the others.  sub_lane = the i-th lane of the sub-block whose lowest lane is `first`, sub_rank = its inverse.
-template <int SUBL>
-__device__ __forceinline__ int sub_first(int lane) { return SUBL == 32 ? 0 : SUBL == 16 ? (lane & 4) : (lane & 20); }
+// Sub-blocks are the warp's quarters (8 lanes, 4x2 pixels): the sub-block id uses lane bits b2 and b4, the lanes within it the others.
+// sub_lane = the i-th lane of the sub-block whose lowest lane is `first`, sub_rank = its inverse.
+constexpr int kSubLanes = 8;
 
-template <int SUBL>
-__device__ __forceinline__ int sub_lane(int first, int i) {
-    if (SUBL == 32) return i;
-    if (SUBL == 16) return first | (i & 3) | ((i & 12) << 1);
-    return first | (i & 3) | ((i & 4) << 1);
-}
+__device__ __forceinline__ int sub_first(int lane) { return lane & 20; }
 
-template <int SUBL>
-__device__ __forceinline__ int sub_rank(int lane) {
-    if (SUBL == 32) return lane;
-    if (SUBL == 16) return (lane & 3) | ((lane >> 1) & 12);
-    return (lane & 3) | ((lane >> 1) & 4);
-}
+__device__ __forceinline__ int sub_lane(int first, int i) { return first | (i & 3) | ((i & 4) << 1); }
+
+__device__ __forceinline__ int sub_rank(int lane) { return (lane & 3) | ((lane >> 1) & 4); }
 
 
 // per-pixel backward state (initializeBackwardRay, kernels/cuda/common/rayPayloadBackward.cuh:31-73)
@@ -180,7 +171,7 @@ struct RadianceHit {
     }
 };
 
-template <int DEG, bool FAST, int SUBL>
+template <int DEG, bool FAST>
 __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& sm, const Ray& ray, float ofx, float ofy, float ofz, int tid,
                                               int lane, uint32_t begin, uint32_t end, const float* __restrict__ particles,
                                               const float* __restrict__ rgb, const uint32_t* __restrict__ sorted_values,
@@ -190,9 +181,9 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
     const bool depth_grads = __any_sync(kFull, alive && (st.Dgrad != 0.f));
     const int quarter = lane_quarter(lane);
     // lanes of this lane's sub-block, and the float4 column of the gradient row this lane sums (columns >= 5 / 4: none)
-    const unsigned sub_lanes = SUBL == 32 ? kFull : SUBL == 16 ? (quarter_lanes(quarter & 1) | quarter_lanes((quarter & 1) | 2)) : quarter_lanes(quarter);
-    const int first = sub_first<SUBL>(lane);
-    const int col = sub_rank<SUBL>(lane);
+    const unsigned sub_lanes = quarter_lanes(quarter);
+    const int first = sub_first(lane);
+    const int col = sub_rank(lane);
     const int cols = depth_grads ? 5 : 4;
     float4* rows = sm.rows[tid >> 5];
     backward_batches<FAST>(sm, sm.hw, ofx, ofy, ofz, tid, begin, end, particles, sorted_values, hit_words, use_words, alive,
@@ -202,15 +193,12 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
         [](uint32_t, int) {},
         [&](int count) {
         // chunks of 32 entries.  Every sub-block of the warp walks ITS OWN entries -- those some pixel of the sub-block accepted in the
-        // forward (hit words) -- in lockstep with the other sub-blocks: one pass of the adjoint serves up to 32 / SUBL particles, and
-        // the reduction tree is log2(SUBL) levels deep.
+        // forward (hit words) -- in lockstep with the other sub-blocks: one pass of the adjoint serves up to 4 particles, and each
+        // particle's rows are summed over kSubLanes lanes.
         for (int c = 0; c < count; c += 32) {
             if (__all_sync(kFull, !alive)) break;
             const uint32_t* hw = sm.hw + (c >> 5) * kWordsPerChunk + (tid >> 5) * 4;
-            unsigned todo;
-            if (SUBL == 32) todo = hw[0] | hw[1] | hw[2] | hw[3];
-            else if (SUBL == 16) todo = hw[quarter & 1] | hw[(quarter & 1) | 2];
-            else todo = hw[quarter];
+            unsigned todo = hw[quarter];
             if (count - c < 32) todo &= (1u << (count - c)) - 1u;
             while (__any_sync(kFull, todo != 0u)) {
                 const bool act = todo != 0u;
@@ -231,10 +219,10 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
                     if (depth_grads) mine[4] = make_float4(g[16], g[17], g[18], 0.f);  // warp-uniform
                     __syncwarp();
                     if ((hits & sub_lanes) && col < cols) {  // this sub-block's particle received something
-                        float4 s = rows[sub_lane<SUBL>(first, 0) * (kGradRow / 4) + col];
+                        float4 s = rows[sub_lane(first, 0) * (kGradRow / 4) + col];
 #pragma unroll
-                        for (int i = 1; i < SUBL; ++i) {
-                            const float4 v = rows[sub_lane<SUBL>(first, i) * (kGradRow / 4) + col];
+                        for (int i = 1; i < kSubLanes; ++i) {
+                            const float4 v = rows[sub_lane(first, i) * (kGradRow / 4) + col];
                             s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
                         }
                         atomicAdd(reinterpret_cast<float4*>(grad_acc + static_cast<size_t>(__float_as_uint(sm.cl[j].w)) * kGradRow) + col, s);
@@ -250,7 +238,7 @@ __device__ __forceinline__ void backward_tile(const FrameConfig& cfg, BwdSmem& s
 // 3 CTAs per SM (72-80 registers, 45 KB of shared memory per CTA; 24 warps per SM).  4 CTAs would fit in shared memory but cap the
 // kernel at 64 registers, where every instantiation spills (36 B stores, 64 B loads per thread).  Measured at C2 on an H100 80GB HBM3
 // (700 W), bench.py --steps 50, three runs each, render_backward: 3 -> 0.417-0.422 ms, 4 (with the spills) -> 0.413-0.414 ms.
-template <int DEG, int SUBL>
+template <int DEG>
 __global__ void __launch_bounds__(kTilePixels, 3) render_backward_kernel(FrameCamera cam, FrameConfig cfg,
                                                                       const float* __restrict__ rays_o,
                                                                       const float* __restrict__ rays_d,
@@ -290,9 +278,9 @@ __global__ void __launch_bounds__(kTilePixels, 3) render_backward_kernel(FrameCa
     const uint32_t* words = hit_words + static_cast<size_t>(chunk_base[tr.tile]) * kWordsPerChunk;
     const bool use_words = (cfg.subtile_culling & 4) != 0;
     if (fast)
-        backward_tile<DEG, true, SUBL>(cfg, sm, tr.ray, ofx, ofy, ofz, tid, tid & 31, begin, end, particles, rgb, sorted_values, words, use_words, tr.valid, st, grad_acc);
+        backward_tile<DEG, true>(cfg, sm, tr.ray, ofx, ofy, ofz, tid, tid & 31, begin, end, particles, rgb, sorted_values, words, use_words, tr.valid, st, grad_acc);
     else
-        backward_tile<DEG, false, SUBL>(cfg, sm, tr.ray, ofx, ofy, ofz, tid, tid & 31, begin, end, particles, rgb, sorted_values, words, use_words, tr.valid, st, grad_acc);
+        backward_tile<DEG, false>(cfg, sm, tr.ray, ofx, ofy, ofz, tid, tid & 31, begin, end, particles, rgb, sorted_values, words, use_words, tr.valid, st, grad_acc);
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -559,16 +547,10 @@ void launch_render_backward(cudaStream_t s, const FrameCamera& cam, const FrameC
                             const uint32_t* ranges, const uint32_t* tile_order, const uint32_t* chunk_base, const uint32_t* hit_words,
                             const float* out_rgba, const float* d_rgba, const float* out_dist, const float* d_dist, float* grad_acc) {
     const unsigned grid = cam.grid_x * cam.grid_y;
-    // sub-block width of the backward walk: bits 4..5 of the switch (0 = default quarter-warps, 1 = half-warps, 2 = whole warp;
-    // check_args rejects 3)
-    const int sub = (cfg.subtile_culling >> 4) & 3;
-#define GUT_BWD(DEG_, SUB_) render_backward_kernel<DEG_, SUB_><<<grid, kTilePixels, 0, s>>>(cam, cfg, rays_o, rays_d, particles, rgb, sorted_values, ranges, tile_order, chunk_base, hit_words, out_rgba, d_rgba, out_dist, d_dist, grad_acc)
-    if (cfg.kernel_degree == 4) {
-        if (sub == 2) GUT_BWD(4, 32); else if (sub == 1) GUT_BWD(4, 16); else GUT_BWD(4, 8);
-    } else {
-        if (sub == 2) GUT_BWD(2, 32); else if (sub == 1) GUT_BWD(2, 16); else GUT_BWD(2, 8);
-    }
-#undef GUT_BWD
+    if (cfg.kernel_degree == 4)
+        render_backward_kernel<4><<<grid, kTilePixels, 0, s>>>(cam, cfg, rays_o, rays_d, particles, rgb, sorted_values, ranges, tile_order, chunk_base, hit_words, out_rgba, d_rgba, out_dist, d_dist, grad_acc);
+    else
+        render_backward_kernel<2><<<grid, kTilePixels, 0, s>>>(cam, cfg, rays_o, rays_d, particles, rgb, sorted_values, ranges, tile_order, chunk_base, hit_words, out_rgba, d_rgba, out_dist, d_dist, grad_acc);
 }
 
 void launch_project_backward(cudaStream_t s, const FrameCamera& cam, int64_t n, const float* particles, const float* sph,

@@ -113,7 +113,8 @@ __device__ __forceinline__ bool tile_common_origin(const FrameCamera& cam, const
 }
 
 // Lane bits of a warp's 8x4 pixel block: b0..b2 = x, b3..b4 = y (tile_pixel).  Quarter q = b2 | b4 << 1 is a 4x2-pixel block; the
-// forward records one hit word per (32-entry chunk, warp, quarter); halves (4x4 pixels, split by b2) and the whole warp OR them.
+// forward records one hit word per (32-entry chunk, warp, quarter); the work counters OR them for halves (4x4 pixels, split by b2)
+// and the whole warp.
 __device__ __forceinline__ int lane_quarter(int lane) { return ((lane >> 2) & 1) | ((lane >> 3) & 2); }
 __device__ __forceinline__ unsigned quarter_lanes(int q) { return (0x0F0Fu << ((q & 1) * 4)) << ((q >> 1) * 16); }
 constexpr int kWordsPerChunk = (kTilePixels / 32) * 4;  // 8 warps x 4 quarters

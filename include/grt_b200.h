@@ -22,9 +22,8 @@
  * Forward state kept for the backward (ours, no reference twin): grtb200_trace records each ray's accepted hits in a buffer owned
  * by the context; grtb200_trace_bwd replays them when it is called with the forward's arguments (same ray / particle / output
  * pointers, pose and BVH) and otherwise re-traces like the reference (src/kernels/cuda/referenceBwdOptix.cu:103-170).
- * Profiling switches read from the environment at call time: GRTB200_PACKET=0 (per-thread traversal), GRTB200_SIZE_LEVELS=0 /
- * GRTB200_SIZE_T=a[,b[,c]] (size classes of the LBVH key), GRTB200_LEAF=k (particles per leaf), GRTB200_HITCAP=k (hits recorded
- * per ray, 0 = always re-trace).
+ * The environment variable GRTB200_HITCAP=k, read at each forward, sets the hits recorded per ray (0 = always re-trace); rays with
+ * more hits than that are re-traced by the backward.
  */
 #ifndef GRT_B200_H
 #define GRT_B200_H

@@ -74,8 +74,8 @@ typedef struct gutb200_config {
     int32_t k_buffer_size;    /* GAUSSIAN_K_BUFFER_SIZE (render.splat.k_buffer_size): 0 = unsorted (default), 1..16 = sorted 3DGUT */
     int32_t subtile_culling;  /* ours (no reference twin), bit mask, default 7: bit 1 = exact-conservative sub-tile screens in render,
                                * bit 2 = renderBackward walks only the list entries some pixel of a sub-block accepted in the forward
-                               * ("hit words"); bits 4..5 = sub-block of that walk: 0 quarter-warp (4x2 pixels), 1 half-warp (4x4),
-                               * 2 whole warp (8x4), 3 rejected; bit 0 unused.  Forward results are bit-identical with bit 1 on or off. */
+                               * ("hit words"; the sub-blocks are quarter-warps, 4x2 pixels); bits 4..5 must be 0; bit 0 unused.
+                               * Forward results are bit-identical with bit 1 on or off. */
 } gutb200_config;
 
 typedef struct gutb200_ctx gutb200_ctx;

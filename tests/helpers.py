@@ -361,3 +361,48 @@ def tile_pixels(tiles, height, width):
 
 def frac_within(a, b, atol):
     return float(np.mean(np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)) <= atol))
+
+
+def shuffled_pixels(height, width, seed=0):
+    """A fixed seeded permutation of the pixels of a height x width frame.  3DGRT traces each 8x4 block of consecutive rays as one warp
+    and walks the tree as a packet only when the warp's rays are coherent: rays put in this order come from all over the frame, so every
+    warp fails that vote and takes the per-lane walk, where the camera's own order takes the packet walk."""
+    return np.random.default_rng(seed).permutation(height * width)
+
+
+def permute_pixels(a, perm):
+    """`a` ([H, W, ...], [1, H, W, ...] or [H * W, ...]) with its pixels in the order `perm`: pixel j of the result is pixel perm[j]."""
+    a = np.asarray(a)
+    return np.ascontiguousarray(a.reshape(len(perm), -1)[perm].reshape(a.shape))
+
+
+def unpermute_pixels(a, perm):
+    """The inverse of permute_pixels: the outputs of rays traced in the order `perm`, back in the camera's order."""
+    a = np.asarray(a)
+    out = np.empty_like(a).reshape(len(perm), -1)
+    out[perm] = a.reshape(len(perm), -1)
+    return out.reshape(a.shape)
+
+
+def packet_share(particles, sph, c2w, ro, rd, **config):
+    """Share of the rays (ro, rd: [1, H, W, 3]) that one 3DGRT forward walks as a packet, from grtb200_debug_trace_counters; `config`
+    sets fields of grtb200_config."""
+    import b200_native as nat
+    import torch
+
+    cfg = nat.grt_default_config()
+    for k, v in config.items():
+        setattr(cfg, k, v)
+    ctx = nat.GrtContext(cfg, 0)
+    s = torch.cuda.current_stream().cuda_stream
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda()  # noqa: E731
+    p, f, tro, trd = t(particles), t(sph), t(ro), t(rd)
+    n = int(p.shape[0])
+    ctx.build_bvh_packed(s, n, p.data_ptr())
+    vis = torch.zeros(n, device="cuda")
+    r2w = np.ascontiguousarray(np.asarray(c2w, np.float32)[:3, :4])
+    b, h, w = ro.shape[:3]
+    c = ctx.trace_counters(s, n, p.data_ptr(), f.data_ptr(), 3, 1e-3, b, h, w, tro.data_ptr(), trd.data_ptr(), r2w.ctypes.data, vis.data_ptr())
+    ctx.close()
+    print(f"[walk] trace counters {c}: packet-walked rays {100 * c['packet_rays'] / c['rays']:.1f} %")
+    return c["packet_rays"] / c["rays"]

@@ -6,7 +6,7 @@ import pytest
 
 import grt_ico_oracle as gio
 import scenes
-from helpers import image_error_report, rel_l2
+from helpers import image_error_report, packet_share, permute_pixels, rel_l2, shuffled_pixels, unpermute_pixels
 from test_grt_parity_gpu import _Batch, _Gaussians
 
 pytestmark = pytest.mark.gpu
@@ -77,17 +77,20 @@ def test_icosahedron_forward_and_gradients(degree, cam_index, size):
     assert max(errs.values()) <= 1e-3
 
 
-def _frame(sc, c2w, d_out, degree=4):
+def _frame(sc, c2w, d_out, degree=4, perm=None):
+    """perm: the rays are traced in that pixel order (shuffled_pixels), and the image and hits are returned in the camera's order."""
     dev = torch.device("cuda", 0)
     tr = _tracer(degree)
     g = _Gaussians(sc, dev)
     tr.build_acc(g, rebuild=True)
-    out = tr.render(g, _Batch(sc, c2w, dev), train=True)
+    rays = None if perm is None else tuple(permute_pixels(a, perm) for a in sc.rays())
+    out = tr.render(g, _Batch(sc, c2w, dev, rays), train=True)
     img = torch.cat([out["pred_features"], out["pred_opacity"], out["pred_dist"]], -1)
-    (img * torch.from_numpy(d_out).to(dev)).sum().backward()
+    (img * torch.from_numpy(d_out if perm is None else permute_pixels(d_out, perm)).to(dev)).sum().backward()
     torch.cuda.synchronize()
     grads = [t.grad.detach().cpu().numpy() for t in (g.positions, g.density, g.rotation, g.scale, g._sph)]
-    return img[0].detach().cpu().numpy(), out["hits_count"][0].detach().cpu().numpy(), grads
+    img, hits = img[0].detach().cpu().numpy(), out["hits_count"][0].detach().cpu().numpy()
+    return (img, hits, grads) if perm is None else (unpermute_pixels(img, perm), unpermute_pixels(hits, perm), grads)
 
 
 @pytest.fixture(scope="module")
@@ -111,15 +114,22 @@ def test_retrace_gives_the_replayed_gradients(c2_frame, monkeypatch):
         assert err <= 1e-5
 
 
-@pytest.mark.parametrize("switch,off", [("GRTB200_PACKET", "0"), ("GRTB200_LEAF", "1"), ("GRTB200_SIZE_LEVELS", "0")])
-def test_traversal_variants_give_the_same_image(c2_frame, switch, off, monkeypatch):
+def test_traversal_variants_give_the_same_image(c2_frame):
+    """The same rays traced in a seeded pixel order, so that every warp fails the coherence vote and takes the per-lane walk where the
+    camera's order takes the packet walk: the same image, hit counts and gradients."""
+    import b200_native as nat
+
     sc, c2w, d_out, (img1, hits1, g1) = c2_frame
-    monkeypatch.setenv(switch, off)
-    img0, hits0, g0 = _frame(sc, c2w, d_out)
+    perm = shuffled_pixels(sc.height, sc.width)
+    ro, rd = sc.rays()
+    cfg = dict(kernel_degree=4, density_clamping=0, primitive=nat.GRT_PRIMITIVES["icosahedron"])
+    assert packet_share(sc.particles, sc.sph, c2w, ro, rd, **cfg) >= 0.9
+    assert packet_share(sc.particles, sc.sph, c2w, permute_pixels(ro, perm), permute_pixels(rd, perm), **cfg) <= 0.1
+    img0, hits0, g0 = _frame(sc, c2w, d_out, perm=perm)
     P = sc.width * sc.height
-    print(f"[ico] {switch}: hit counts differ on {(hits1 != hits0).sum()} of {P} rays")
+    print(f"[ico] shuffled: hit counts differ on {(hits1 != hits0).sum()} of {P} rays")
     assert (hits1 != hits0).mean() <= 1e-3
-    mean_e, max_e, bad = image_error_report(f"ico {switch}: image", img1, img0, atol=1e-4)
+    mean_e, max_e, bad = image_error_report("ico shuffled: image", img1, img0, atol=1e-4)
     assert mean_e <= 1e-6 and max_e <= 2e-2 and bad <= max(3, int(2e-4 * P))
     for name, a, b in zip(("positions", "density", "rotation", "scale", "sph"), g1, g0):
         assert rel_l2(a, b) <= 1e-3

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import scenes
-from helpers import image_error_report, ray_sample, rel_l2
+from helpers import image_error_report, packet_share, permute_pixels, ray_sample, rel_l2, shuffled_pixels, unpermute_pixels
 from oracle import gut_oracle as go
 
 pytestmark = pytest.mark.gpu
@@ -95,11 +95,28 @@ CASES = {
 }
 
 
-@pytest.mark.parametrize("packet", ["1", "0"])
+def _walk_rays(sc, c2w, ro, rd, walk, deg, prim, clamping=True):
+    """The rays of `walk`: "packet" the camera's order, where every warp's rays are coherent; "per-lane" a seeded pixel order that no
+    warp's rays are coherent in.  Returns (ro, rd, perm), perm None for the camera's order."""
+    import b200_native as nat
+
+    perm = shuffled_pixels(sc.height, sc.width) if walk == "per-lane" else None
+    if perm is not None:
+        ro, rd = permute_pixels(ro, perm), permute_pixels(rd, perm)
+    share = packet_share(sc.particles, sc.sph, c2w, ro, rd, kernel_degree=deg, primitive=nat.GRT_PRIMITIVES[prim],
+                         density_clamping=int(clamping))
+    assert share >= 0.9 if perm is None else share <= 0.1
+    return ro, rd, perm
+
+
+def _unpermuted(out, perm):
+    return out if perm is None else {k: (v if k == "vis" else unpermute_pixels(v, perm)) for k, v in out.items()}
+
+
+@pytest.mark.parametrize("walk", ["packet", "per-lane"])
 @pytest.mark.parametrize("case", list(CASES))
-def test_normals_match_the_f64_oracle(case, packet, monkeypatch):
-    """packet 0: the per-lane walk (GRTB200_PACKET=0) instead of the packet walk of coherent warps."""
-    monkeypatch.setenv("GRTB200_PACKET", packet)
+def test_normals_match_the_f64_oracle(case, walk):
+    """per-lane: the same rays in a seeded pixel order, so that every warp takes the per-lane walk instead of the packet walk."""
     make, cam, deg, prim, clamping = CASES[case]
     sc = make()
     ro, rd = sc.rays()
@@ -108,8 +125,9 @@ def test_normals_match_the_f64_oracle(case, packet, monkeypatch):
     cfg.kernel_degree = deg
     ref, lists = gnr.frame(cfg, sc.particles, ro[0], rd[0], c2w, primitive=prim, clamping=clamping)
     assert (lists["count"] > 0).sum() > 100
-    out = _Gpu(sc.particles, sc.sph, c2w, ro, rd, deg, prim, clamping).forward(normals=True)
-    _check_parity(f"normals {case} packet={packet}", out["nrm"], ref)
+    wro, wrd, perm = _walk_rays(sc, c2w, ro, rd, walk, deg, prim, clamping)
+    out = _unpermuted(_Gpu(sc.particles, sc.sph, c2w, wro, wrd, deg, prim, clamping).forward(normals=True), perm)
+    _check_parity(f"normals {case} {walk} walk", out["nrm"], ref)
     none = out["hits"] == 0  # rays that accepted no hit (the fisheye frame's corners): written, and zero
     assert np.array_equal(out["nrm"][none], np.zeros((int(none.sum()), 3), np.float32))
 
@@ -132,14 +150,14 @@ def test_normals_at_c4_on_a_ray_sample(frame):
     _check_parity(f"normals {frame}", out["nrm"][idx], ref)
 
 
-@pytest.mark.parametrize("packet", ["1", "0"])
+@pytest.mark.parametrize("walk", ["packet", "per-lane"])
 @pytest.mark.parametrize("prim", ["instances", "icosahedron"])
 @pytest.mark.parametrize("deg", [4, 2])
-def test_normals_leave_every_other_output_bit_identical(deg, prim, packet, monkeypatch):
-    monkeypatch.setenv("GRTB200_PACKET", packet)
+def test_normals_leave_every_other_output_bit_identical(deg, prim, walk):
     sc = scenes.scene_c2(n=40_000, width=160, height=128)
-    ro, rd = sc.rays()
-    g = _Gpu(sc.particles, sc.sph, np.asarray(sc.camera(2, 10), np.float32), ro, rd, deg, prim)
+    c2w = np.asarray(sc.camera(2, 10), np.float32)
+    ro, rd, _ = _walk_rays(sc, c2w, *sc.rays(), walk, deg, prim)
+    g = _Gpu(sc.particles, sc.sph, c2w, ro, rd, deg, prim)
     plain, with_n = g.forward(normals=False), g.forward(normals=True)
     assert plain["hits"].sum() > 1000
     for k in ("rgb", "alpha", "dist", "hits", "vis"):

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import scenes
-from helpers import image_error_report, rel_l2
+from helpers import image_error_report, packet_share, permute_pixels, rel_l2, shuffled_pixels, unpermute_pixels
 from oracle import gut_oracle as go
 
 pytestmark = pytest.mark.gpu
@@ -41,8 +41,8 @@ class _Gaussians:
 
 
 class _Batch:
-    def __init__(self, sc, c2w, device):
-        ro, rd = sc.rays()
+    def __init__(self, sc, c2w, device, rays=None):
+        ro, rd = sc.rays() if rays is None else rays
         self.rays_ori = torch.from_numpy(ro).to(device)
         self.rays_dir = torch.from_numpy(rd).to(device)
         self.T_to_world = torch.from_numpy(np.asarray(c2w, np.float32))[None].to(device)
@@ -155,36 +155,46 @@ def test_hybrid_primary_raster_plus_traced_secondary():
     assert g.positions.grad is not None and float(g.positions.grad.abs().sum()) > 0 and torch.isfinite(g._sph.grad).all()
 
 
-def _grt_frame(sc, c2w, d_out):
-    """One forward + backward through the Tracer; returns numpy (rgba, dist, hits, grads...)."""
+def _grt_frame(sc, c2w, d_out, perm=None):
+    """One forward + backward through the Tracer; returns numpy (rgba + dist, hits, grads).  perm: the rays are traced in that pixel
+    order (shuffled_pixels), and the image and hits are returned in the camera's order."""
     import threedgrt_tracer
 
     dev = torch.device("cuda", 0)
     tr = threedgrt_tracer.Tracer({"render": {"min_transmittance": 0.001}})
     g = _Gaussians(sc, dev)
     tr.build_acc(g, rebuild=True)
-    out = tr.render(g, _Batch(sc, c2w, dev), train=True)
+    rays = None if perm is None else tuple(permute_pixels(a, perm) for a in sc.rays())
+    out = tr.render(g, _Batch(sc, c2w, dev, rays), train=True)
     img = torch.cat([out["pred_features"], out["pred_opacity"], out["pred_dist"]], -1)
-    (img * torch.from_numpy(d_out).to(dev)).sum().backward()
+    (img * torch.from_numpy(d_out if perm is None else permute_pixels(d_out, perm)).to(dev)).sum().backward()
     torch.cuda.synchronize()
     grads = [t.grad.detach().cpu().numpy() for t in (g.positions, g.density, g.rotation, g.scale, g._sph)]
-    return img[0].detach().cpu().numpy(), out["hits_count"][0].detach().cpu().numpy(), grads
+    img, hits = img[0].detach().cpu().numpy(), out["hits_count"][0].detach().cpu().numpy()
+    return (img, hits, grads) if perm is None else (unpermute_pixels(img, perm), unpermute_pixels(hits, perm), grads)
 
 
-@pytest.mark.parametrize("switch,off", [("GRTB200_PACKET", "0"), ("GRTB200_SIZE_LEVELS", "0"), ("GRTB200_LEAF", "1"),
-                                        ("GRTB200_HITCAP", "0"), ("GRTB200_HITCAP", "8")])
+@pytest.mark.parametrize("switch,off", [pytest.param("shuffled", None, id="shuffled"), ("GRTB200_HITCAP", "0"), ("GRTB200_HITCAP", "8")])
 def test_traversal_variants_give_the_same_image(switch, off, monkeypatch):
-    """Packet traversal, the size-class bit of the LBVH key and the leaf size change HOW the tree is built / walked, not which
-    hits a ray finds; the hit-list cache changes how the backward finds the forward's hits (HITCAP=0: re-trace like the
-    reference, HITCAP=8: nearly every ray overflows its list and takes the re-trace fallback).  The same rays through either
-    variant must give the same image, hit counts and gradients."""
+    """The walk changes HOW the tree is traversed, not which hits a ray finds: "shuffled" traces the same rays in a seeded pixel order,
+    so that every warp fails the coherence vote and takes the per-lane walk where the camera's order takes the packet walk.  The
+    hit-list cache changes how the backward finds the forward's hits (HITCAP=0: re-trace like the reference, HITCAP=8: nearly every ray
+    overflows its list and takes the re-trace fallback).  The same rays through either variant must give the same image, hit counts and
+    gradients."""
     sc = scenes.scene_c2(n=60_000, width=256, height=256)
     c2w = np.asarray(sc.camera(2, 10), np.float32)
     rng = np.random.default_rng(0)
     d_out = rng.normal(size=(1, sc.height, sc.width, 5)).astype(np.float32)
     img1, hits1, g1 = _grt_frame(sc, c2w, d_out)
-    monkeypatch.setenv(switch, off)
-    img0, hits0, g0 = _grt_frame(sc, c2w, d_out)
+    if switch == "shuffled":
+        perm = shuffled_pixels(sc.height, sc.width)
+        ro, rd = sc.rays()
+        assert packet_share(sc.particles, sc.sph, c2w, ro, rd) >= 0.9
+        assert packet_share(sc.particles, sc.sph, c2w, permute_pixels(ro, perm), permute_pixels(rd, perm)) <= 0.1
+        img0, hits0, g0 = _grt_frame(sc, c2w, d_out, perm)
+    else:
+        monkeypatch.setenv(switch, off)
+        img0, hits0, g0 = _grt_frame(sc, c2w, d_out)
     assert hits1.sum() > 0
     # not bit-identical: a hit whose t* lies before its box entry (ray clipping a corner of the proxy) survives or not depending on
     # which node boxes got culled by the shrinking 16th-hit bound -- the same ambiguity OptiX has; hence the standard tolerances

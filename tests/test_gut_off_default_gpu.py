@@ -1,6 +1,6 @@
 """GPU parity of the CUDA 3DGUT path against the CPU oracle OFF the default path: active SH degrees 0-2 (the first 3000 steps of every
-training run raise the degree from 0), each render setting of gutb200_config away from its default, the backward's half-warp and
-whole-warp sub-blocks (subtile_culling bits 4-5), and cloned particles (equal depth keys, as densification produces them).
+training run raise the degree from 0), each render setting of gutb200_config away from its default, and cloned particles (equal depth
+keys, as densification produces them).
 
 Every case sets the same field on the oracle's config and on the native one.  Bars (DESIGN.md section 5, as test_gut_parity_gpu.py):
   * tile counts, depth bits, sorted keys and values, tile ranges and visibility: BIT-EXACT;
@@ -10,9 +10,6 @@ Every case sets the same field on the oracle's config and on the native one.  Ba
     the gradient bar is the yardstick rule of test_gut_headline_parity_gpu.py: err <= max(1e-3, 1.5 x (oracle f32 vs oracle f64 on the
     same lists)), and err <= 1e-3 flat once the oracle's ten largest f32-vs-f64 flip particles are left out.  Both are printed."""
 import dataclasses
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -390,54 +387,7 @@ def test_render_setting_parity(setting, frame, k):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
-# 3. the backward's sub-block widths (subtile_culling bits 4-5: 16 = half-warps, 32 = whole warps)
-
-
-def _banded_rays(sc):
-    """The three bands of test_per_pixel_ray_origins_take_the_general_path: the frame's origin (backward FAST), another origin common to
-    the tile (backward GENERAL with the origin-offset terms), per-pixel jitter."""
-    ro, rd = sc.rays()
-    rng = np.random.default_rng(3)
-    ro = (ro + 0.02 * rng.normal(size=ro.shape)).astype(np.float32)
-    ro[:, :32] = ro[0, 0, 0]
-    ro[:, 32:64] = ro[0, 0, 0] + np.array([0.03, -0.02, 0.05], np.float32)
-    return ro, rd
-
-
-@pytest.mark.parametrize("frame", ["c1_cam0", "dense", "bands"])
-@pytest.mark.parametrize("kernel_degree", [2, 4])
-@pytest.mark.parametrize("mode", [23, 39])
-def test_backward_sub_block_widths(mode, kernel_degree, frame):
-    """subtile_culling 23 (half-warp sub-blocks) and 39 (whole-warp sub-blocks) against the oracle; the forward does not depend on the
-    backward's sub-block and must be bit-identical to the default mode 7."""
-    if frame == "bands":
-        sc, cam_index, n_cams = scenes.scene_c1(), 4, 10
-        ro, rd = _banded_rays(sc)
-    else:
-        sc, cam_index, n_cams = _c1_frame(frame)
-        ro = rd = None
-    pose = tracer_pose(sc.camera(cam_index, n_cams))
-    dense = frame == "dense"
-    ref = _oracle(sc, pose, dict(kernel_degree=kernel_degree), 3, seed=mode + kernel_degree, ro=ro, rd=rd, with_f64=dense)
-    label = f"subtile_culling={mode} kernel_degree={kernel_degree} {frame}"
-    _list_stats(label, ref["bn"])
-    got = _native(sc, pose, dict(kernel_degree=kernel_degree, subtile_culling=mode), 3, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
-    base = _native(sc, pose, dict(kernel_degree=kernel_degree, subtile_culling=7), 3, ref["ro"], ref["rd"], ref["d_rgba"], ref["d_dist"])
-    for k in ("rgba", "dist", "hits"):
-        assert np.array_equal(got[k].view(np.uint32), base[k].view(np.uint32)), f"{label}: forward {k} differs from mode 7"
-    _check_integers(label, got, ref)
-    _check_image(label, got["rgba"], got["dist"], got["hits"], ref)
-    _check_gradients(label, got["dp"], got["ds"], ref)
-    e = max(rel_l2(got["dp"], base["dp"]), rel_l2(got["ds"], base["ds"]))
-    # the sub-block decides which list entries the backward walks (those some pixel of the sub-block accepted in the forward); the
-    # backward re-tests every pair it walks, so only a borderline pair accepted by one arithmetic and not the other can differ, plus the
-    # order of the atomic sums -- the bar of test_subtile_culling_is_bit_identical for hit words on / off
-    print(f"[off-default] {label}: gradients vs mode 7 rel-L2 {e:.2e} (bar 3e-4)")
-    assert e <= 3e-4
-
-
-# ---------------------------------------------------------------------------------------------------------------------------------
-# 4. cloned particles: equal depth keys
+# 3. cloned particles: equal depth keys
 
 
 def clone_scene(base, singles, doubles, forties, seed=0):
@@ -480,7 +430,7 @@ def _equal_t_clone_pairs(sc, group, ref):
 
 
 def check_cloned_particles_3dgut(k=0):
-    """The clone comparison on its own (also run in a child process with GUTB200_SORT_MATCH=1).  k > 0: the sorted variant, where equal
+    """The clone comparison on its own.  k > 0: the sorted variant, where equal
     hit distances leave the buffer's strict insertion order to decide which copy is composited first and so how the gradients split."""
     base = scenes.scene_c2(n=50_000, width=256, height=256)
     sc, group = clone_scene(base, 6000, 300, 8)
@@ -516,29 +466,13 @@ def test_cloned_particles_3dgut_sorted():
     check_cloned_particles_3dgut(16)
 
 
-def test_cloned_particles_3dgut_match_any_sort():
-    """The same comparison with the match.any variant of tile_sort (GUTB200_SORT_MATCH=1, read once per process): in a child process,
-    which must run to completion and exit."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, GUTB200_SORT_MATCH="1")
-    env["PYTHONPATH"] = os.pathsep.join([root, os.path.join(root, "3dgrut_b200"), os.path.join(root, "tests")]
-                                        + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    code = "import test_gut_off_default_gpu as t; t.check_cloned_particles_3dgut(); print('[off-default] match-any sort: done')"
-    r = subprocess.run([sys.executable, *flags, "-c", code], env=env, cwd=root, capture_output=True, text=True, timeout=900)
-    print(r.stdout)
-    print(r.stderr[-4000:])
-    assert r.returncode == 0
-    assert "match-any sort: done" in r.stdout
-
-
 # ---------------------------------------------------------------------------------------------------------------------------------
-# 5. argument checks
+# 4. argument checks
 
 
 def test_out_of_range_arguments_are_rejected():
-    """sph_degree outside 0..3 (it used to be clamped silently) and subtile_culling sub-block code 3 (it used to fall back to
-    quarter-warps) fail with a message on forward, backward and backward_compact."""
+    """sph_degree outside 0..3 (it used to be clamped silently) and any non-zero subtile_culling bits 4-5 (only quarter-warp sub-blocks
+    are built) fail with a message on forward, backward and backward_compact."""
     import b200_native as nat
 
     sc = scenes.scene_c1(n=64, width=32, height=32)
@@ -575,10 +509,12 @@ def test_out_of_range_arguments_are_rejected():
             bwd(ctx, deg, compact=True)
     bwd(ctx, 3)
     ctx.close()
-    cfg = nat.default_config()
-    cfg.subtile_culling = 7 | (3 << 4)
-    bad = nat.Context(cfg, 0)
-    with pytest.raises(RuntimeError, match="sub-block code 3"):
-        fwd(bad, 3)
-    bad.close()
+    for mode in (23, 39, 7 | (3 << 4)):
+        cfg = nat.default_config()
+        cfg.subtile_culling = mode
+        bad = nat.Context(cfg, 0)
+        for call in (lambda: fwd(bad, 3), lambda: bwd(bad, 3), lambda: bwd(bad, 3, compact=True)):
+            with pytest.raises(RuntimeError, match=f"subtile_culling sub-block code {(mode >> 4) & 3} "):
+                call()
+        bad.close()
     torch.cuda.synchronize()
