@@ -124,6 +124,13 @@ SIGNATURES = {
     "grtb200_launch_count": (_i64, [_vp]),
     "grtb200_set_replay": (_int, [_vp, _i32]),
     "grtb200_debug_trace_counters": (_int, _grt_trace + [_vp, _vp]),
+    "grtb200_mesh_create": (_int, [_int, _vpp]),
+    "grtb200_mesh_destroy": (None, [_vp]),
+    "grtb200_mesh_last_error": (_str, [_vp]),
+    "grtb200_build_mesh_bvh": (_int, [_vp, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i32, _vp]),
+    "grtb200_mesh_closest_hit": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "grtb200_trace_playground": (_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i32, _f32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp,
+                                        _vp]),
     # include/nht_b200.h (NHT feature decoder: fused tensor-core MLP)
     "nhtb200_last_error": (_str, []),
     "nhtb200_n_params": (_i64, [_nht]),
@@ -428,6 +435,34 @@ class GrtContext(_Handle):
 
     def launch_count(self) -> int:
         return int(self._lib.grtb200_launch_count(self._h))
+
+    def trace_playground(self, stream, mesh, n, particles, sph, sph_degree, min_t, batch, height, width, rays_o, rays_d, r2w_host, ray_max_t,
+                         background_host, smooth_normals, out_rgb, out_alpha, visibility):
+        """Forward render with the meshes of `mesh` (a MeshBvh or None) inserted: out_rgb [R,3], out_alpha [R] (grtb200_trace_playground)."""
+        self._check(self._lib.grtb200_trace_playground(self._h, stream, None if mesh is None else mesh._h, n, particles, sph, sph_degree, min_t,
+                                                       batch, height, width, rays_o, rays_d, r2w_host, ray_max_t, background_host,
+                                                       int(bool(smooth_normals)), out_rgb, out_alpha, visibility), "grtb200_trace_playground")
+
+
+class MeshBvh(_Handle):
+    """Owning wrapper of a grtb200_mesh*: the LBVH over the triangles of the playground meshes."""
+
+    PREFIX = "grtb200_mesh"
+
+    def __init__(self, device: int = 0):
+        self._lib = load()
+        self._h = C.c_void_p()
+        self._check_create(self._lib.grtb200_mesh_create(int(device), C.byref(self._h)), None)
+
+    def build(self, stream, n_vertices, vertices, vertex_normals, n_faces, faces, face_material, n_materials, materials):
+        """(Re)build over device arrays: vertices / vertex_normals [V,3] fp32, faces [F,3] int32, face_material [F] int32, materials
+        [M,8] fp32 (grtb200_build_mesh_bvh; synchronises the stream, copies everything)."""
+        self._check(self._lib.grtb200_build_mesh_bvh(self._h, stream, n_vertices, vertices, vertex_normals, n_faces, faces, face_material,
+                                                     n_materials, materials), "grtb200_build_mesh_bvh")
+
+    def closest_hit(self, stream, n_rays, rays_o, rays_d, out_t, out_tri):
+        """World rays [R,3] -> out_t [R] fp32 (1e5 where nothing is hit), out_tri [R] int32 (-1) (grtb200_mesh_closest_hit)."""
+        self._check(self._lib.grtb200_mesh_closest_hit(self._h, stream, n_rays, rays_o, rays_d, out_t, out_tri), "grtb200_mesh_closest_hit")
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -38,6 +38,8 @@ UNITS = {
     "nht_decoder.cu": [],
     # 3DGRUT hybrid: mirror rays and the composite, no contraction so that they match hybrid.py's torch expressions bit for bit
     "hybrid.cu": ["-fmad=false"],
+    # playground mesh LBVH build and closest-hit queries (the triangle test itself is written with round-to-nearest intrinsics)
+    "playground.cu": [],
     # exact k-nearest neighbours: the box bound and the distance must round the same way (DESIGN.md section 19)
     "gut_knn.cu": ["-fmad=false"],
 }

@@ -38,6 +38,7 @@
 #include "../../include/grt_b200.h"
 #include "hit_math.cuh"
 #include "lbvh.cuh"
+#include "mesh_bvh.cuh"
 #include "nht_features.cuh"
 
 namespace gutb200 {
@@ -714,6 +715,64 @@ __device__ __forceinline__ void backward_hit(const TraceParams& P, uint32_t pid,
     kind.scatter(P, pid);
 }
 
+// The forward state of one ray across its k-nearest queries: transmittance, integrated distance, the largest hit distance processed so
+// far, the accepted hits counted for the output and, for the hit lists, the accepted hits so far and those of them at distance `last`.
+// A playground ray carries it, T above all, from one segment to the next.
+struct FwdState {
+    float T, D, last, hits;
+    uint32_t nrec, nlast;
+};
+
+// The forward's walk (one optixTrace of __raygen__rg per iteration) over the hits at t in (s.last + kEpsT, t1 + kEpsT) while T is above
+// min_transmittance, integrating every accepted hit into `kind` and `s`.  PACKET: every lane of the warp calls it (`want` false: the lane
+// only takes part in the votes).  tix..tiz: the clamped inverse direction of the node slab tests.
+template <int PRIM, int DEG, bool PACKET, bool COUNT, int FK>
+__device__ __forceinline__ void forward_walk(const TraceParams& P, const TraceRay& r, bool want, float tix, float tiy, float tiz, float t1,
+                                             Kind<FK>& kind, FwdState& s, LaneCounters& cc, int* __restrict__ warp_stack) {
+    float kt[kK];
+    uint32_t kid[kK];
+    while (true) {  // one k-nearest query (optixTrace of __raygen__rg) per iteration
+        want = want && (s.last <= t1) && (s.T > P.min_transmittance);
+        if (PACKET ? !__any_sync(0xFFFFFFFFu, want) : !want) break;
+        knn_query<PRIM, PACKET, COUNT>(P, want, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, tix, tiy, tiz, s.last + kEpsT, t1 + kEpsT, kt, kid, cc, warp_stack);
+        if (kid[0] == kNone) want = false;
+        if (!want) continue;
+        float lt[kK];
+        uint32_t li[kK];
+#pragma unroll
+        for (int i = 0; i < kK; ++i) { lt[i] = kt[i]; li[i] = kid[i]; }
+        kind.chunk(P, r.dx, r.dy, r.dz);
+#pragma unroll 1
+        for (int i = 0; i < kK; ++i) {
+            const uint32_t pid = li[i];
+            if ((pid == kNone) || !(s.T > P.min_transmittance)) continue;
+            const ParticleFrame f = load_frame(P.particles, pid);
+            const CanonicalHit h = canonical_hit<DEG>(f, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, P.min_response, P.min_alpha, P.max_alpha);
+            if (COUNT) {
+                cc.cands++;
+                cc.hits += h.accept ? 1 : 0;
+            }
+            if (h.accept) {
+                const float w = h.alpha * s.T;
+                if (kind.add(P, pid, f, h, w)) {
+                    s.hits += 1.f;
+                    P.visibility[pid] = __int_as_float(1);  // benign race, same value (referenceOptix.cu:158-161)
+                }
+                s.T *= (1.f - h.alpha);
+                s.D += hit_distance(f, h) * w;
+                if (P.hit_list && s.nrec < static_cast<uint32_t>(P.hit_cap)) P.hit_list[static_cast<int64_t>(s.nrec) * P.rays + r.ray] = pid;
+                s.nrec++;
+            }
+            if (lt[i] > s.last) {  // hits arrive in ascending t
+                s.last = lt[i];
+                s.nlast = 0;
+            }
+            s.nlast += h.accept ? 1u : 0u;
+        }
+        if (li[kK - 1] == kNone) want = false;  // fewer than 16 hits: the ray is exhausted, the reference's next trace would return nothing
+    }
+}
+
 // Per-ray work after the rays are set up: the forward (BWD = false; COUNT: the work counters instead of the image) or the re-trace of
 // the backward, each one loop of k-nearest queries for every feature kind.  PACKET: the warp's 32 rays traverse together (warp-uniform
 // loops, every lane of the warp must call this, `r.valid` marks the lanes that own a ray).  The two loops differ in their interval, stop
@@ -735,52 +794,11 @@ __device__ __forceinline__ void trace_rays(const TraceParams& P, const TraceRay&
     Kind<FK> kind(feat);
     bool want = r.valid && (P.n > 0);
     if constexpr (!BWD) {
-        float T = 1.f, D = 0.f, last = fmaxf(0.f, t0 - kEpsT), hits = 0.f;
-        uint32_t nrec = 0;        // accepted hits so far
-        uint32_t nlast = 0;       // of those, the ones at distance `last` (the largest processed so far)
+        FwdState s{1.f, 0.f, fmaxf(0.f, t0 - kEpsT), 0.f, 0u, 0u};
         kind.clear();
-        float kt[kK];
-        uint32_t kid[kK];
-        while (true) {  // one k-nearest query (optixTrace of __raygen__rg) per iteration
-            want = want && (last <= t1) && (T > P.min_transmittance);
-            if (PACKET ? !__any_sync(0xFFFFFFFFu, want) : !want) break;
-            knn_query<PRIM, PACKET, COUNT>(P, want, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, tix, tiy, tiz, last + kEpsT, t1 + kEpsT, kt, kid, cc, warp_stack);
-            if (kid[0] == kNone) want = false;
-            if (!want) continue;
-            float lt[kK];
-            uint32_t li[kK];
-#pragma unroll
-            for (int i = 0; i < kK; ++i) { lt[i] = kt[i]; li[i] = kid[i]; }
-            kind.chunk(P, r.dx, r.dy, r.dz);
-#pragma unroll 1
-            for (int i = 0; i < kK; ++i) {
-                const uint32_t pid = li[i];
-                if ((pid == kNone) || !(T > P.min_transmittance)) continue;
-                const ParticleFrame f = load_frame(P.particles, pid);
-                const CanonicalHit h = canonical_hit<DEG>(f, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, P.min_response, P.min_alpha, P.max_alpha);
-                if (COUNT) {
-                    cc.cands++;
-                    cc.hits += h.accept ? 1 : 0;
-                }
-                if (h.accept) {
-                    const float w = h.alpha * T;
-                    if (kind.add(P, pid, f, h, w)) {
-                        hits += 1.f;
-                        P.visibility[pid] = __int_as_float(1);  // benign race, same value (referenceOptix.cu:158-161)
-                    }
-                    T *= (1.f - h.alpha);
-                    D += hit_distance(f, h) * w;
-                    if (P.hit_list && nrec < static_cast<uint32_t>(P.hit_cap)) P.hit_list[static_cast<int64_t>(nrec) * P.rays + r.ray] = pid;
-                    nrec++;
-                }
-                if (lt[i] > last) {  // hits arrive in ascending t
-                    last = lt[i];
-                    nlast = 0;
-                }
-                nlast += h.accept ? 1u : 0u;
-            }
-            if (li[kK - 1] == kNone) want = false;  // fewer than 16 hits: the ray is exhausted, the reference's next trace would return nothing
-        }
+        forward_walk<PRIM, DEG, PACKET, COUNT, FK>(P, r, want, tix, tiy, tiz, t1, kind, s, cc, warp_stack);
+        const float T = s.T, D = s.D, last = s.last, hits = s.hits;
+        const uint32_t nrec = s.nrec, nlast = s.nlast;
         if (COUNT) {
             unsigned long long v[8] = {r.valid ? 1ull : 0ull, cc.queries, cc.nodes, cc.boxes, cc.proxies, cc.cands, cc.hits, (PACKET && r.valid) ? 1ull : 0ull};
 #pragma unroll
@@ -836,6 +854,19 @@ __device__ __forceinline__ void trace_rays(const TraceParams& P, const TraceRay&
     }
 }
 
+// packet traversal pays when the warp's rays are coherent: directions within ~6 degrees of lane 0's and origins within 2 % of the scene
+// diagonal; otherwise every thread walks the tree on its own.  Every lane of the warp calls this.
+__device__ __forceinline__ bool coherent_warp(const TraceParams& P, const TraceRay& r) {
+    const float dx = r.dx, dy = r.dy, dz = r.dz, ox = r.ox, oy = r.oy, oz = r.oz;
+    const float fx = __shfl_sync(0xFFFFFFFFu, dx, 0), fy = __shfl_sync(0xFFFFFFFFu, dy, 0), fz = __shfl_sync(0xFFFFFFFFu, dz, 0);
+    const float gx = __shfl_sync(0xFFFFFFFFu, ox, 0), gy = __shfl_sync(0xFFFFFFFFu, oy, 0), gz = __shfl_sync(0xFFFFFFFFu, oz, 0);
+    const float dot = dx * fx + dy * fy + dz * fz, n1 = dx * dx + dy * dy + dz * dz, n0 = fx * fx + fy * fy + fz * fz;
+    const float ex = P.scene[3] - P.scene[0], ey = P.scene[4] - P.scene[1], ez = P.scene[5] - P.scene[2];
+    const float sx = ox - gx, sy = oy - gy, sz = oz - gz;
+    const bool near_first = (dot > 0.f) && (dot * dot > 0.99f * n1 * n0) && (sx * sx + sy * sy + sz * sz <= 4e-4f * (ex * ex + ey * ey + ez * ez));
+    return __all_sync(0xFFFFFFFFu, near_first);
+}
+
 template <int PRIM, int DEG, bool BWD, bool COUNT, int FK>
 __global__ void __launch_bounds__(128, kTraceBlocksPerSm) trace_kernel(TraceParams P) {
     __shared__ int s_stack[4][kStack];  // one traversal stack per warp (packet walks)
@@ -844,18 +875,7 @@ __global__ void __launch_bounds__(128, kTraceBlocksPerSm) trace_kernel(TracePara
     if (!ray_pixel(P, r)) return;
     world_ray(P, r);
     int* warp_stack = s_stack[threadIdx.x >> 5];
-
-    // packet traversal pays when the block's rays are coherent: directions within ~6 degrees of lane 0's and origins within 2 % of
-    // the scene diagonal; otherwise every thread walks the tree on its own
-    const float dx = r.dx, dy = r.dy, dz = r.dz, ox = r.ox, oy = r.oy, oz = r.oz;
-    const float fx = __shfl_sync(0xFFFFFFFFu, dx, 0), fy = __shfl_sync(0xFFFFFFFFu, dy, 0), fz = __shfl_sync(0xFFFFFFFFu, dz, 0);
-    const float gx = __shfl_sync(0xFFFFFFFFu, ox, 0), gy = __shfl_sync(0xFFFFFFFFu, oy, 0), gz = __shfl_sync(0xFFFFFFFFu, oz, 0);
-    const float dot = dx * fx + dy * fy + dz * fz, n1 = dx * dx + dy * dy + dz * dz, n0 = fx * fx + fy * fy + fz * fz;
-    const float ex = P.scene[3] - P.scene[0], ey = P.scene[4] - P.scene[1], ez = P.scene[5] - P.scene[2];
-    const float sx = ox - gx, sy = oy - gy, sz = oz - gz;
-    const bool near_first = (dot > 0.f) && (dot * dot > 0.99f * n1 * n0) && (sx * sx + sy * sy + sz * sz <= 4e-4f * (ex * ex + ey * ey + ez * ez));
-    const bool coherent = __all_sync(0xFFFFFFFFu, near_first);
-    if (coherent) {
+    if (coherent_warp(P, r)) {
         trace_rays<PRIM, DEG, BWD, true, COUNT, FK>(P, r, warp_stack, feat);
     } else if (COUNT || r.valid) {   // the counting pass ends in warp shuffles: every lane takes part
         trace_rays<PRIM, DEG, BWD, false, COUNT, FK>(P, r, warp_stack, feat);
@@ -877,6 +897,151 @@ __global__ void __launch_bounds__(128) replay_bwd_kernel(TraceParams P) {
     kind.init(P, r.ray);
 #pragma unroll 1
     for (uint32_t i = 0; i < count; ++i) backward_hit<DEG>(P, P.hit_list[static_cast<int64_t>(i) * P.rays + r.ray], r, st, kind);
+}
+
+// ---- playground: meshes inside the scene (grtb200_trace_playground, DESIGN.md section 22) ----------------------------------------------
+// The constants of the reference's playgroundKernel.cu / handleGlass.
+constexpr int kMaxBounces = 32;          // MAX_BOUNCES: mirror reflections (and total internal reflections)
+constexpr int kMaxSegments = 1000;       // TIMEOUT_ITERATIONS
+constexpr float kRefractShift = 1e-5f;   // REFRACTION_EPS_SHIFT
+constexpr float kOutsideIor = 1.0003f;   // n1
+constexpr float kStopAlpha = 0.995f;
+constexpr float kBounceTMin = 1e-9f;     // tmin of a Gaussian segment after a bounce
+constexpr float kRayMaxT = 1e9f;         // ray_max_t where the caller gives none
+
+struct PlaygroundParams {
+    TraceParams P;                 // the Gaussians, rays and options of grtb200_trace (SH radiance)
+    gutb200::MeshView mesh;
+    const float* ray_max_t;        // [R] or nullptr (kRayMaxT)
+    float bg[3];
+    int smooth;                    // interpolated vertex normals, else the triangle's own
+};
+
+// The Gaussians of ray r on (a, b) inside the scene box: the forward walk of grtb200_trace, starting from the state s (T and the radiance
+// in `kind` carried from the segments before).  With a = 0 and b past the scene box this is grtb200_trace's walk exactly.
+template <int PRIM, int DEG, bool PACKET>
+__device__ __forceinline__ void gaussian_segment(const TraceParams& P, const TraceRay& r, bool want, float a, float b, ShRadiance& kind,
+                                                 FwdState& s, int* __restrict__ warp_stack) {
+    const float idx_ = 1.0f / r.dx, idy_ = 1.0f / r.dy, idz_ = 1.0f / r.dz;
+    const float tix = 1.0f / (fabsf(r.dx) > 1e-20f ? r.dx : copysignf(1e-20f, r.dx));
+    const float tiy = 1.0f / (fabsf(r.dy) > 1e-20f ? r.dy : copysignf(1e-20f, r.dy));
+    const float tiz = 1.0f / (fabsf(r.dz) > 1e-20f ? r.dz : copysignf(1e-20f, r.dz));
+    float t0, t1;
+    scene_clip(P.scene, r.ox, r.oy, r.oz, idx_, idy_, idz_, t0, t1);
+    t0 = fmaxf(t0, a);
+    t1 = fminf(t1, b);
+    s.last = fmaxf(0.f, t0 - kEpsT);
+    LaneCounters cc;
+    forward_walk<PRIM, DEG, PACKET, false, kFeatSH>(P, r, want && (P.n > 0), tix, tiy, tiz, t1, kind, s, cc, warp_stack);
+}
+
+__device__ __forceinline__ void normalize3(float& x, float& y, float& z) {
+    const float l2 = x * x + y * y + z * z;
+    const float il = l2 > 0.f ? rsqrtf(l2) : 1.f;  // safe_normalize
+    x *= il; y *= il; z *= il;
+}
+
+// the unit normal at hit h: normalize(cross(e1, e2)), or the vertex normals interpolated with the barycentrics (1 - u - v, u, v)
+__device__ __forceinline__ void hit_normal(const PlaygroundParams& G, const MeshHit& h, float& nx, float& ny, float& nz) {
+    if (G.smooth) {
+        const int a = G.mesh.faces[3 * h.tri], b = G.mesh.faces[3 * h.tri + 1], c = G.mesh.faces[3 * h.tri + 2];
+        const float w = 1.f - h.u - h.v;
+        const float* vn = G.mesh.vnormals;
+        nx = w * vn[3 * a] + h.u * vn[3 * b] + h.v * vn[3 * c];
+        ny = w * vn[3 * a + 1] + h.u * vn[3 * b + 1] + h.v * vn[3 * c + 1];
+        nz = w * vn[3 * a + 2] + h.u * vn[3 * b + 2] + h.v * vn[3 * c + 2];
+    } else {
+        const float4 e1 = G.mesh.tris[3 * h.tri + 1], e2 = G.mesh.tris[3 * h.tri + 2];
+        nx = e1.y * e2.z - e1.z * e2.y;
+        ny = e1.z * e2.x - e1.x * e2.z;
+        nz = e1.x * e2.y - e1.y * e2.x;
+    }
+    normalize3(nx, ny, nz);
+}
+
+// One ray: the first segment as grtb200_trace walks it (as a packet when the warp is coherent), then per thread a closest mesh hit, the
+// material's bounce and the Gaussians of the next segment, until the ray leaves every mesh, meets a diffuse surface, reaches alpha 0.995,
+// 32 bounces or 1000 segments.  One transmittance T is carried through all of it: mirror and glass are lossless, a diffuse hit adds
+// T c |dot(d, n)| and makes the ray opaque.
+template <int PRIM, int DEG>
+__global__ void __launch_bounds__(128) playground_kernel(PlaygroundParams G, float* __restrict__ out_rgb, float* __restrict__ out_alpha) {
+    __shared__ int s_stack[4][kStack];
+    const TraceParams& P = G.P;
+    TraceRay r;
+    if (!ray_pixel(P, r)) return;
+    world_ray(P, r);
+    int* warp_stack = s_stack[threadIdx.x >> 5];
+    const float tmax = G.ray_max_t ? G.ray_max_t[r.ray] : kRayMaxT;
+    MeshHit h = mesh_closest_hit(G.mesh, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz);
+    ShRadiance kind(nullptr);
+    kind.clear();
+    FwdState s{1.f, 0.f, 0.f, 0.f, 0u, 0u};
+    const float end0 = h.tri >= 0 ? h.t : tmax;
+    if (coherent_warp(P, r))
+        gaussian_segment<PRIM, DEG, true>(P, r, r.valid, 0.f, end0, kind, s, warp_stack);
+    else if (r.valid)
+        gaussian_segment<PRIM, DEG, false>(P, r, true, 0.f, end0, kind, s, warp_stack);
+    if (!r.valid) return;
+    int bounces = 0, segments = 1;
+#pragma unroll 1
+    while (h.tri >= 0) {
+        const int m = G.mesh.tri_material[h.tri];
+        const float4 mk = G.mesh.materials[2 * m], mc = G.mesh.materials[2 * m + 1];
+        const int kind_m = static_cast<int>(mk.x);
+        float nx, ny, nz;
+        hit_normal(G, h, nx, ny, nz);
+        float dx = r.dx, dy = r.dy, dz = r.dz;
+        normalize3(dx, dy, dz);
+        const float dn = dx * nx + dy * ny + dz * nz;
+        if (kind_m == GRTB200_MATERIAL_DIFFUSE) {  // get_diffuse_color without a texture: opaque, ends the ray
+            const float shade = fabsf(dn);
+            kind.Cx += s.T * mc.x * shade;
+            kind.Cy += s.T * mc.y * shade;
+            kind.Cz += s.T * mc.z * shade;
+            s.T = 0.f;
+            break;
+        }
+        // the normal turned against the ray: the front face when dot(d, n) < 0
+        const float sg = dn < 0.f ? 1.f : -1.f;
+        const float fx = sg * nx, fy = sg * ny, fz = sg * nz;
+        const float cos_i = -(dx * fx + dy * fy + dz * fz);  // >= 0
+        float t = h.t;
+        float ex, ey, ez;
+        bool reflect = kind_m == GRTB200_MATERIAL_MIRROR;
+        if (!reflect) {  // glass: Snell refraction, n1 outside, the mesh's ior inside (refract / handleGlass)
+            const float eta = mk.y / kOutsideIor;
+            const float ri = dn < 0.f ? 1.f / eta : eta;
+            const float ct = fminf(cos_i, 1.f);
+            const float st = sqrtf(fmaxf(0.f, 1.f - ct * ct));
+            if (ri * st <= 1.f) {
+                const float px = ri * (dx + ct * fx), py = ri * (dy + ct * fy), pz = ri * (dz + ct * fz);
+                const float q = -sqrtf(fabsf(1.f - (px * px + py * py + pz * pz)));
+                ex = px + q * fx; ey = py + q * fy; ez = pz + q * fz;
+                normalize3(ex, ey, ez);
+                t += kRefractShift;
+            } else {
+                reflect = true;  // total internal reflection
+            }
+        }
+        if (reflect) {  // handleMirror: d - 2 dot(d, n) n about the turned normal
+            ex = dx + 2.f * cos_i * fx; ey = dy + 2.f * cos_i * fy; ez = dz + 2.f * cos_i * fz;
+            normalize3(ex, ey, ez);
+            ++bounces;
+        }
+        r.ox += t * r.dx; r.oy += t * r.dy; r.oz += t * r.dz;
+        r.dx = ex; r.dy = ey; r.dz = ez;
+        if (!(1.f - s.T < kStopAlpha) || bounces >= kMaxBounces || segments >= kMaxSegments) break;
+        h = mesh_closest_hit(G.mesh, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz);
+        gaussian_segment<PRIM, DEG, false>(P, r, true, kBounceTMin, h.tri >= 0 ? h.t : tmax, kind, s, warp_stack);
+        ++segments;
+    }
+    // the background on 1 - alpha (BackgroundColor at evaluation), rounded as rgb + bg * (1 - alpha), then clamped to [0, 1]
+    const float alpha = 1.f - s.T, keep = __fsub_rn(1.f, alpha);
+    const int64_t ray = r.ray;
+    out_rgb[ray * 3] = fminf(fmaxf(__fadd_rn(kind.Cx, __fmul_rn(G.bg[0], keep)), 0.f), 1.f);
+    out_rgb[ray * 3 + 1] = fminf(fmaxf(__fadd_rn(kind.Cy, __fmul_rn(G.bg[1], keep)), 0.f), 1.f);
+    out_rgb[ray * 3 + 2] = fminf(fmaxf(__fadd_rn(kind.Cz, __fmul_rn(G.bg[2], keep)), 0.f), 1.f);
+    out_alpha[ray] = fminf(fmaxf(alpha, 0.f), 1.f);
 }
 
 int fail(grtb200_ctx* c, const char* fmt, ...);
@@ -1392,6 +1557,44 @@ int grtb200_trace_bwd_nht(grtb200_ctx* c, void* stream, int64_t n, const float* 
     if (fk < 0) return 1;
     return trace_bwd(c, fk, stream, n, particles, static_cast<const float*>(features), 0, min_transmittance, batch, height, width, rays_o,
                      rays_d, ray_to_world_host, out_features, out_alpha, out_dist, d_features_out, d_alpha, d_dist, d_particles, d_features);
+}
+
+// Playground render (DESIGN.md section 22): fill_params as grtb200_trace, the mesh view of `mesh`, one launch.
+int grtb200_trace_playground(grtb200_ctx* c, void* stream, const grtb200_mesh* mesh, int64_t n, const float* particles, const float* sph,
+                             int32_t sph_degree, float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                             const float* rays_d, const float* ray_to_world_host, const float* ray_max_t, const float* background_host,
+                             int32_t smooth_normals, float* out_rgb, float* out_alpha, float* visibility) {
+    if (!c) return 1;
+    if (!background_host || !out_rgb || !out_alpha || (n > 0 && !visibility)) return fail(c, "trace_playground: null background or output");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    GRT_CUDA(c, cudaSetDevice(c->device));
+    PlaygroundParams G;
+    if (int rc = fill_params(c, G.P, n, particles, sph, sph_degree, min_transmittance, batch, height, width, rays_o, rays_d, ray_to_world_host, s))
+        return rc;
+    G.P.visibility = visibility;
+    G.mesh = gutb200::mesh_view(mesh);
+    G.ray_max_t = ray_max_t;
+    for (int k = 0; k < 3; ++k) G.bg[k] = background_host[k];
+    G.smooth = smooth_normals != 0;
+    if (n > 0) GRT_CUDA(c, cudaMemsetAsync(visibility, 0, static_cast<size_t>(n) * 4, s));
+    const unsigned blocks = ray_blocks(G.P);
+    if (blocks == 0) return 0;
+    constexpr int kInst = GRTB200_PRIMITIVE_INSTANCES, kIco = GRTB200_PRIMITIVE_ICOSAHEDRON;
+    const bool ico = c->cfg.primitive == kIco;
+    if (c->cfg.kernel_degree == 4) {
+        if (ico)
+            playground_kernel<kIco, 4><<<blocks, 128, 0, s>>>(G, out_rgb, out_alpha);
+        else
+            playground_kernel<kInst, 4><<<blocks, 128, 0, s>>>(G, out_rgb, out_alpha);
+    } else {
+        if (ico)
+            playground_kernel<kIco, 2><<<blocks, 128, 0, s>>>(G, out_rgb, out_alpha);
+        else
+            playground_kernel<kInst, 2><<<blocks, 128, 0, s>>>(G, out_rgb, out_alpha);
+    }
+    c->launches++;
+    GRT_CUDA(c, cudaGetLastError());
+    return 0;
 }
 
 }  // extern "C"

@@ -129,6 +129,45 @@ int grtb200_debug_trace_counters(grtb200_ctx* ctx, void* stream, int64_t n, cons
                                  float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
                                  const float* rays_d, const float* ray_to_world_host, float* visibility_scratch, uint64_t* counters8);
 
+/* ---- Playground: triangle meshes inside a trained scene (forward only; DESIGN.md section 22) -------------------------------------------
+ *
+ *   grtb200_mesh_create / destroy / last_error   a handle that owns one LBVH over the triangles of all inserted meshes
+ *   grtb200_build_mesh_bvh                       (re)build it: call when the meshes change, not per frame
+ *   grtb200_mesh_closest_hit                     closest hit of world-space rays (t in (1e-5, 1e5), both faces, ties -> lowest index)
+ *   grtb200_trace_playground                     <- the Playground's __raygen__rg (threedgrut_playground/src/kernels/cuda/playgroundKernel.cu)
+ *
+ * Mesh layouts (device, world space): vertices [V,3] fp32; vertex_normals [V,3] fp32 unit normals; faces [F,3] int32; face_material [F]
+ * int32 rows of materials [M,8] fp32 = (kind, ior, 0, 0, r, g, b, 0) with kind one of GRTB200_MATERIAL_*.  The build copies all of it.
+ */
+#define GRTB200_MATERIAL_MIRROR 0
+#define GRTB200_MATERIAL_GLASS 1
+#define GRTB200_MATERIAL_DIFFUSE 2
+
+typedef struct grtb200_mesh grtb200_mesh;
+
+/* Returns 2 without a usable CUDA device. */
+int grtb200_mesh_create(int device, grtb200_mesh** out);
+void grtb200_mesh_destroy(grtb200_mesh* mesh);
+const char* grtb200_mesh_last_error(const grtb200_mesh* mesh);
+/* Synchronises `stream` (before replacing the previous tree and after the build).  n_faces = 0 leaves an empty mesh set. */
+int grtb200_build_mesh_bvh(grtb200_mesh* mesh, void* stream, int64_t n_vertices, const float* vertices, const float* vertex_normals,
+                           int64_t n_faces, const int32_t* faces, const int32_t* face_material, int32_t n_materials, const float* materials);
+/* rays_o / rays_d [R,3] world space; out_t [R] (1e5 where nothing is hit), out_tri [R] int32 (-1 where nothing is hit). */
+int grtb200_mesh_closest_hit(grtb200_mesh* mesh, void* stream, int64_t n_rays, const float* rays_o, const float* rays_d, float* out_t,
+                             int32_t* out_tri);
+
+/* Forward render of the Gaussians of the last grtb200_build_bvh with the meshes of `mesh` (null: no meshes) inserted.  Arguments up to
+ * ray_to_world_host are grtb200_trace's (SH radiance).  Each ray alternates a closest mesh hit and the k-nearest Gaussian walk of
+ * grtb200_trace on the segment up to it (to ray_max_t [R], or 1e9 where ray_max_t is null, when no mesh is hit), with one transmittance
+ * carried through every segment; mirror and glass redirect the ray (at most 32 mirror bounces, 1000 segments), diffuse ends it.  The ray
+ * stops once its alpha reaches 0.995.  smooth_normals: interpolated vertex normals, else the triangle's own.  background_host: 3 floats
+ * (host), composited on 1 - alpha.  out_rgb [R,3] and out_alpha [R] are clamped to [0, 1]; visibility [N] marks the Gaussians hit.  A ray
+ * that meets no mesh gets grtb200_trace's radiance and alpha exactly (then composited and clamped).  Records no hit lists. */
+int grtb200_trace_playground(grtb200_ctx* ctx, void* stream, const grtb200_mesh* mesh, int64_t n, const float* particles, const float* sph,
+                             int32_t sph_degree, float min_transmittance, int32_t batch, int32_t height, int32_t width, const float* rays_o,
+                             const float* rays_d, const float* ray_to_world_host, const float* ray_max_t, const float* background_host,
+                             int32_t smooth_normals, float* out_rgb, float* out_alpha, float* visibility);
+
 #ifdef __cplusplus
 }
 #endif
