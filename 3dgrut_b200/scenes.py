@@ -149,6 +149,16 @@ class Scene:
             return fisheye_rays(self.height, self.width, self.fx, self.fy, self.cx, self.cy, self.fisheye)
         return pinhole_rays(self.height, self.width, self.fx, self.fy, self.cx, self.cy)
 
+    def pinhole_sensor(self):
+        """The 3DGUT sensor of the pinhole rays(): global shutter, no distortion.  Imports the tracer (and torch) only when called."""
+        from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
+
+        if self.fisheye is not None or self.ftheta is not None:
+            raise ValueError(f"scene {self.name} has a fisheye or f-theta camera, not a pinhole")
+        return fromOpenCVPinholeCameraModelParameters(np.array([self.width, self.height]), ShutterType.GLOBAL,
+                                                      np.array([self.cx, self.cy], np.float32), np.array([self.fx, self.fy], np.float32),
+                                                      np.zeros(6, np.float32), np.zeros(2, np.float32), np.zeros(4, np.float32))
+
 
 def _pack(pos, dns, quat, scl):
     n = pos.shape[0]

@@ -390,6 +390,21 @@ def particle_record(p: dict) -> torch.Tensor:
                       torch.zeros_like(p["density"])], dim=1).contiguous()
 
 
+def raw_params(particles: torch.Tensor, sph: torch.Tensor | None = None, features: torch.Tensor | None = None) -> dict:
+    """The raw parameter dict of the activated [N,12] record: the inverse of particle_record, with the density clamped to
+    [1e-4, 1 - 1e-4] before its logit.  Exactly one of sph ([N,48] SH: features_albedo, features_specular) and features ([N,F] NHT)."""
+    if (sph is None) == (features is None):
+        raise ValueError("raw_params takes exactly one of sph and features")
+    d = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
+    raw = {"positions": particles[:, 0:3].clone(), "density": torch.log(d / (1 - d)), "rotation": particles[:, 4:8].clone(),
+           "scale": torch.log(particles[:, 8:11])}
+    if sph is not None:
+        raw.update(features_albedo=sph[:, 0:3].clone(), features_specular=sph[:, 3:48].clone())
+    else:
+        raw["features"] = features.clone()
+    return raw
+
+
 def regulariser_loss(particles, lambda_opacity: float, lambda_scale: float):
     """lambda_opacity mean|density| + lambda_scale mean|scale| on the activated [N,12] record (trainer.py:722-736); 0 when both are 0."""
     reg = 0.0

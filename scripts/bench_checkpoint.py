@@ -13,28 +13,14 @@ from __future__ import annotations
 
 import argparse
 import os
-import subprocess
-import sys
 import tempfile
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 LRS = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=2.5e-3, features_specular=1.25e-4)
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def _filesystem(path: str) -> str:
@@ -64,11 +50,8 @@ def main():
     import densify
     import train_step
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_checkpoint.py measures on a CUDA device; none is present")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    print(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}")
+    dev = benchkit.cuda_device("bench_checkpoint.py")
+    print(f"device: {benchkit.card(dev)}")
     print(f"checkpoint directory: {args.dir} on {_filesystem(args.dir)}")
     workdir = tempfile.mkdtemp(prefix="bench_checkpoint_", dir=args.dir)
 

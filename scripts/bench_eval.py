@@ -9,33 +9,16 @@
   eval frame evaluate.evaluate on C2 (300k Gaussians, 800x800, 3DGUT) over --frames views, per frame: render + metrics, with and without
              writing the PNG files (to a temporary directory).
 
-Prints the card name and power limit first."""
+Prints the card (benchkit.card) first."""
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 import tempfile
 import time
 
-import numpy as np
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 SIZES = ((800, 800), (822, 1237))  # (H, W)
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def _reference_chain(x, y, win):
@@ -103,38 +86,21 @@ def bench_metrics(reps, torch):
               f"{chain[2]:.5f}, cc_ssim {got['cc_ssim']:.6f} vs {chain[3]:.6f}")
 
 
-class _Batch:
-    """A gpu_batch as threedgut_tracer.Tracer reads a pinhole camera: camera-space rays, T_to_world, the scene's intrinsics."""
-
-    def __init__(self, sc, rays_o, rays_d, c2w):
-        from threedgut_tracer.tracer import ShutterType
-
-        self.rays_ori, self.rays_dir, self.T_to_world = rays_o, rays_d, c2w.to(rays_o.device)
-        self.intrinsics_OpenCVPinholeCameraModelParameters = dict(
-            resolution=np.array([sc.width, sc.height]), shutter_type=ShutterType.GLOBAL, principal_point=np.array([sc.cx, sc.cy], np.float32),
-            focal_length=np.array([sc.fx, sc.fy], np.float32), radial_coeffs=np.zeros(6, np.float32), tangential_coeffs=np.zeros(2, np.float32),
-            thin_prism_coeffs=np.zeros(4, np.float32))
-
-
 def bench_eval_frame(frames, torch):
     import evaluate
     import scenes
     import train_step
-    from threedgut_tracer.tracer import Tracer
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c2()
-    P, S = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
-    dns = P[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    raw = {"positions": P[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": P[:, 4:8].clone(), "scale": torch.log(P[:, 8:11]),
-           "features_albedo": S[:, 0:3].clone(), "features_specular": S[:, 3:48].clone()}
+    raw = train_step.raw_params(torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev))
     lrs = dict(positions=1e-4, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
     st = train_step.GaussianTrainStep(raw, lrs, background="white")
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
 
     poses = [scenes.pose7_from_c2w(sc.camera(i, frames)) for i in range(frames)]
-    sensor = Tracer._create_camera_parameters(_Batch(sc, rays_o, rays_d, torch.from_numpy(np.asarray(sc.camera(0, frames), np.float32))[None]))[0]
+    sensor = sc.pinhole_sensor()
     gen = torch.Generator(device=dev).manual_seed(0)
     targets = []
     for p in poses:  # the render on the white background, with noise
@@ -161,10 +127,7 @@ def main():
 
     import torch
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_eval.py needs a CUDA device")
-    torch.cuda.set_device(0)
-    print(f"device: {torch.cuda.get_device_name(0)}, power limit {_power_limit(0)}")
+    print(f"device: {benchkit.card(benchkit.cuda_device('bench_eval.py'))}")
     bench_metrics(args.reps, torch)
     bench_eval_frame(args.frames, torch)
 

@@ -5,7 +5,7 @@ Stages (CUDA events, L2 flushed before every timed call, warmup first): NHT forw
 (grtb200_trace_bwd_nht, replaying the forward's hit lists), SH forward (grtb200_trace) and SH backward (grtb200_trace_bwd), alternating
 in one process; each backward follows an untimed forward of its kind.  Both feature precisions are timed (fp32 and fp16 rows) unless
 --only fp32|fp16.  The NHT configs' max_alpha 0.999 is used for both kinds; features are drawn from U(-pi/2, pi/2), the init range of
-configs/base_gs.yaml.  Prints the card name and power limit and one JSON line.  A CUDA device is required.
+configs/base_gs.yaml.  Prints the card (benchkit.card) and one JSON line.  A CUDA device is required.
 
   python scripts/bench_grt_nht.py [--iters 20] [--warmup 5] [--only fp32|fp16]
 """
@@ -14,23 +14,11 @@ from __future__ import annotations
 import argparse
 import json
 import math
-import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "3dgrut_b200"))
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"{torch.cuda.get_device_name()} (power limit unavailable: {e})"
+import benchkit
 
 
 def main():
@@ -39,8 +27,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--only", choices=("fp32", "fp16"), default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_grt_nht: a CUDA device is required")
+    info = benchkit.card(benchkit.cuda_device("bench_grt_nht.py"))
+    print(f"device: {info}")
     import b200_native as nat
     import scenes
 
@@ -108,8 +96,6 @@ def main():
     med = {k: float(np.median(v)) for k, v in times.items()}
     med["sh_forward"] = float(np.median(sum((times[k] for k in times if k.startswith("sh_forward")), [])))
     med["sh_backward"] = float(np.median(sum((times[k] for k in times if k.startswith("sh_backward")), [])))
-    info = card()
-    print(f"card: {info}")
     for k, v in med.items():
         print(f"{k:>26}: {v:.3f} ms")
     print(json.dumps({"scene": "C4 300k 800x800 (3DGRT)", "max_alpha": 0.999, "card": info, "median_ms": med}))

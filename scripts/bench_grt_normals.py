@@ -5,37 +5,22 @@
 C4 is the C2 scene (300k Gaussians, 800x800) through 3DGRT, on the default `instances` config and on the icosahedron paper config
 (degree-2 kernel, no density clamping).  The BVH is built once per config; each timed step is one forward trace of an orbit view, with
 normals (grtb200_trace_normals) and without (grtb200_trace) alternately, each timed with CUDA events.  The hit-list recording for the
-backward is off, as in an inference render (Tracer.render without gradients), where the normals view is used.  Prints the card and its
-power limit and the median trace times.
+backward is off, as in an inference render (Tracer.render without gradients), where the normals view is used.  Prints the card
+(benchkit.card) and the median trace times.
 """
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 CONFIGS = {
     "instances": {"min_transmittance": 0.001},
     "icosahedron paper": {"min_transmittance": 0.001, "primitive_type": "icosahedron", "particle_kernel_degree": 2,
                           "particle_kernel_density_clamping": False},
 }
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -50,10 +35,8 @@ def main():
     import scenes
     import threedgrt_tracer
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_grt_normals: a CUDA device is required")
-    dev = torch.device("cuda", 0)
-    print(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}")
+    dev = benchkit.cuda_device("bench_grt_normals.py")
+    print(f"device: {benchkit.card(dev)}")
     sc = scenes.scene_c2(n=args.n)
     H, W = sc.height, sc.width
     particles = torch.from_numpy(sc.particles).to(dev)

@@ -4,33 +4,18 @@
 
 A step is the step of bench.py's c4 line (full BVH build + trace + trace_bwd of one orbit view).  The primitives alternate step by step
 so that clock drift hits both alike; every stage is timed with CUDA events.  Both use the 3DGRT default kernel (degree 4, density
-clamping), so only the proxy differs.  Prints the card and its power limit, median stage times, and the work counters of one forward
+clamping), so only the proxy differs.  Prints the card (benchkit.card), median stage times, and the work counters of one forward
 per ray (grtb200_debug_trace_counters): k-nearest queries, node visits, proxy tests, candidate and accepted hits.
 """
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 PRIMITIVES = ("instances", "icosahedron")
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -45,8 +30,8 @@ def main():
     import scenes
     import threedgrt_tracer
 
-    dev = torch.device("cuda", 0)
-    print(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}")
+    dev = benchkit.cuda_device("bench_grt_proxies.py")
+    print(f"device: {benchkit.card(dev)}")
     sc = scenes.scene_c2(n=args.n)
     H, W = sc.height, sc.width
     tracers = {p: threedgrt_tracer.Tracer({"render": {"min_transmittance": 0.001, "primitive_type": p}}).tracer_wrapper for p in PRIMITIVES}

@@ -16,17 +16,11 @@ and scales perturbed, the targets are the scene rendered from 10 orbit views."""
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 CONFIGS = {
     "instances": {"render": {"min_transmittance": 0.001}},
@@ -35,15 +29,6 @@ CONFIGS = {
 }
 PHASES = ("build", "trace", "loss", "backward", "exchange", "adam")
 LRS = dict(positions=1.6e-4, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=2.5e-3, features_specular=1.25e-4)
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -58,20 +43,13 @@ def main():
     import torch.distributed as dist
 
     import scenes
+    import train_step
     import train_step_grt
     import view_parallel as vp
 
-    world = int(os.environ.get("WORLD_SIZE", "1"))
-    rank = int(os.environ.get("RANK", "0"))
-    local = int(os.environ.get("LOCAL_RANK", "0"))
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_grt_train.py measures on a CUDA device; none is present")
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    if world > 1:
-        dist.init_process_group("nccl", device_id=dev)
-    log = print if rank == 0 else (lambda *a, **k: None)
-    log(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(local)}, ranks {world}")
+    dev = benchkit.cuda_device("bench_grt_train.py")
+    rank, world, log = benchkit.ranks(dev)
+    log(f"device: {benchkit.card(dev)}, ranks {world}")
 
     sc = scenes.scene_c2(n=args.n)
     H, W = sc.height, sc.width
@@ -81,11 +59,6 @@ def main():
     n_views = 10
     poses = [torch.from_numpy(np.asarray(sc.camera(i, n_views), np.float32))[None] for i in range(n_views)]
 
-    def raw_from(particles, sph):
-        dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-                "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
     weights = dict(lambda_l1=0.8, lambda_ssim=0.2) if args.ssim else dict(lambda_l1=1.0, lambda_ssim=0.0)
     gen = torch.Generator(device=dev).manual_seed(0)
     P2 = P.clone()
@@ -93,10 +66,10 @@ def main():
     P2[:, 8:11] *= torch.exp(0.1 * torch.randn((sc.n, 3), device=dev, generator=gen))
     steps, targets = {}, {}
     for name, conf in CONFIGS.items():
-        truth = train_step_grt.GaussianTrainStepGRT(raw_from(P, S), LRS, conf=conf)
+        truth = train_step_grt.GaussianTrainStepGRT(train_step.raw_params(P, S), LRS, conf=conf)
         targets[name] = [truth.render(rays_o, rays_d, p)[0][0].clone() for p in poses]
         del truth
-        steps[name] = train_step_grt.GaussianTrainStepGRT(raw_from(P2, S), LRS, conf=conf, **weights)
+        steps[name] = train_step_grt.GaussianTrainStepGRT(train_step.raw_params(P2, S), LRS, conf=conf, **weights)
     host_targets = {k: [t.cpu().pin_memory() for t in v] for k, v in targets.items()}
 
     counters = {k: 0 for k in CONFIGS}

@@ -11,35 +11,20 @@ Prints one JSON line with
     exchange buffer, with a fixed image gradient (no loss, no exchange, no Adam),
   - the fraction of pixels whose ray meets the mirror, over the timed views,
   - the 3DGRT work counters of one secondary trace next to those of the C4 primary trace (300k Gaussians at 800x800, the C2 scene),
-  - the peak device memory, the card's name and its power limit, read in the same run.
+  - the peak device memory and the card (benchkit.card), read in the same run.
 With more than one rank every rank trains its own view and rank 0 also reports views/s over all ranks.  The start is the scene with its
 positions and scales perturbed; the targets are the hybrid renders of the scene from 6 orbit views.  Writes no file."""
 from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 LRS = dict(positions=1.6e-4, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=2.5e-3, features_specular=1.25e-4)
 N_VIEWS = 6
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def _median(v):
@@ -60,45 +45,31 @@ def main():
 
     import scenes
     import threedgrt_tracer
+    import train_step
     import train_step_hybrid as th
     import view_parallel as vp
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
-    world = int(os.environ.get("WORLD_SIZE", "1"))
-    rank = int(os.environ.get("RANK", "0"))
-    local = int(os.environ.get("LOCAL_RANK", "0"))
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_hybrid_train.py measures on a CUDA device; none is present")
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    if world > 1:
-        dist.init_process_group("nccl", device_id=dev)
-    card, power = torch.cuda.get_device_name(dev), _power_limit(local)
+    dev = benchkit.cuda_device("bench_hybrid_train.py")
+    rank, world, _ = benchkit.ranks(dev)
+    card = benchkit.card(dev)
 
     sc = scenes.scene_c5(n=args.n)
     H, W = sc.height, sc.width
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     P, S = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
     poses = [torch.from_numpy(np.asarray(sc.camera(i, N_VIEWS), np.float32))[None] for i in range(N_VIEWS)]
 
-    def raw_from(particles, sph):
-        dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-                "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
     weights = dict(lambda_l1=0.8, lambda_ssim=0.2) if args.ssim else dict(lambda_l1=1.0, lambda_ssim=0.0)
-    truth = th.GaussianTrainStepHybrid(raw_from(P, S), LRS, mirror=scenes.C5_MIRROR)
+    truth = th.GaussianTrainStepHybrid(train_step.raw_params(P, S), LRS, mirror=scenes.C5_MIRROR)
     targets = [truth.render(rays_o, rays_d, sensor, p)[0].clone() for p in poses]
     del truth
     gen = torch.Generator(device=dev).manual_seed(0)
     P2 = P.clone()
     P2[:, 0:3] += 0.005 * torch.randn((sc.n, 3), device=dev, generator=gen)
     P2[:, 8:11] *= torch.exp(0.1 * torch.randn((sc.n, 3), device=dev, generator=gen))
-    st = th.GaussianTrainStepHybrid(raw_from(P2, S), LRS, mirror=scenes.C5_MIRROR, **weights)
+    st = th.GaussianTrainStepHybrid(train_step.raw_params(P2, S), LRS, mirror=scenes.C5_MIRROR, **weights)
     del P2
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats(dev)
@@ -197,7 +168,7 @@ def main():
         "fwd_bwd_ms_median": _median(fb), "fwd_bwd_frames_per_s": 1000.0 / _median(fb),
         "hit_fraction": float(np.mean(hits)), "hit_fraction_per_view": hits,
         "secondary_trace_counters": sec_counters, "c4_primary_trace_counters": c4_counters,
-        "peak_memory_gb": peak / 1e9, "device": card, "power_limit": power,
+        "peak_memory_gb": peak / 1e9, "device": card,
     }
     if world > 1:
         result["views_per_s_all_ranks"] = world * 1000.0 / float(np.median(f))

@@ -13,25 +13,11 @@ from __future__ import annotations
 
 import argparse
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
-
-
-def _gpu_info(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
+import benchkit
 
 
 def _cloud(kind: str, n: int, seed: int = 0) -> np.ndarray:
@@ -98,10 +84,8 @@ def main():
 
     import initialization as I
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_init.py needs a CUDA device")
-    dev = torch.device("cuda", 0)
-    print(f"GPU: {_gpu_info(0)}  CPU threads: {os.cpu_count()}  torch {torch.__version__}")
+    dev = benchkit.cuda_device("bench_init.py")
+    print(f"device: {benchkit.card(dev)}  CPU threads: {os.cpu_count()}  torch {torch.__version__}")
     conf_pts = {"initialization": {"use_observation_points": False}}
     print(f"{'workload':<34} {'N':>9} {'knn ms':>9} {'from_points ms':>15} {'CPU KD-tree ms':>16}")
     for kind in ("uniform", "c3_like"):

@@ -8,31 +8,16 @@ in one process, at 800x800 and 1237x822 (0.8 L1 + 0.2 (1 - SSIM), white backgrou
 
 Each variant is timed with CUDA events around `--reps` back-to-back calls (the two launches and the host wrapper), in `--rounds` rounds
 that alternate the variants; the median per-call time is printed with the device time of the kernels alone (torch.profiler), the card
-name and its power limit."""
+(benchkit.card)."""
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 SIZES = ((800, 800), (822, 1237))  # (H, W)
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -47,11 +32,8 @@ def main():
 
     import losses
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_loss_post.py needs a CUDA device")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    print(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}")
+    dev = benchkit.cuda_device("bench_loss_post.py")
+    print(f"device: {benchkit.card(dev)}")
     white = (1.0, 1.0, 1.0)
     variants = {}
     for H, W in SIZES:

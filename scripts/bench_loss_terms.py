@@ -9,31 +9,16 @@
     python scripts/bench_loss_terms.py [--reps 200] [--rounds 5]
 
 Each variant is timed with CUDA events around `--reps` back-to-back launches, in `--rounds` rounds that alternate the variants; the
-median per-launch time over the rounds is printed with the card name and its power limit."""
+median per-launch time over the rounds is printed with the card (benchkit.card)."""
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 LRS = dict(positions=1.6e-4, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=2.5e-3, features_specular=1.25e-4)
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -49,9 +34,8 @@ def main():
     import losses
     import optimizers
 
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    print(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}")
+    dev = benchkit.cuda_device("bench_loss_terms.py")
+    print(f"device: {benchkit.card(dev)}")
     H = W = args.size
     gen = torch.Generator(device=dev).manual_seed(0)
     tgt = torch.rand((H, W, 3), device=dev, generator=gen)

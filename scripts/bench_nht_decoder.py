@@ -8,18 +8,14 @@ from __future__ import annotations
 import argparse
 import ctypes as C
 import json
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "3dgrut_b200")]
+import benchkit
 
-import b200_native as nat  # noqa: E402
-import feature_decoder as fd  # noqa: E402
-from oracle import nht_tcnn_ref  # noqa: E402
+import b200_native as nat
+import feature_decoder as fd
+from oracle import nht_tcnn_ref
 
 F, DEGREE, LAYERS, SH_SCALE = 24, 3, 3, 3.0
 PEAK_FLOPS, PEAK_BYTES = 989e12, 3.35e12
@@ -51,11 +47,8 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_nht_decoder.py needs a CUDA device")
-    dev = torch.device("cuda", 0)
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print(f"card: {torch.cuda.get_device_name(0)}; nvidia-smi: {smi}")
+    dev = benchkit.cuda_device("bench_nht_decoder.py")
+    print(f"device: {benchkit.card(dev)}")
     cfg = fd.decoder_config(F, 128, LAYERS, "SphericalHarmonics", DEGREE, SH_SCALE, "Sigmoid")
     lib = nat.nht_lib()
     params = fd.initial_params(cfg, torch.Generator().manual_seed(0)).to(dev)

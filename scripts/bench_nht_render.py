@@ -3,7 +3,7 @@
 Stages (CUDA events, L2 flushed before every timed call, warmup first): NHT render forward (gutb200_forward_nht), NHT render backward
 (gutb200_backward_nht), decoder forward, decoder forward + backward, and the whole NHT training frame (render -> decode -> L1 gradient ->
 decode backward -> render backward).  The SH forward + backward (gutb200_forward / gutb200_backward) runs in the same process, alternating
-with the NHT runs.  Features are drawn from U(-pi/2, pi/2), the init range of configs/base_gs.yaml.  Prints the card name and power limit
+with the NHT runs.  Features are drawn from U(-pi/2, pi/2), the init range of configs/base_gs.yaml.  Prints the card (benchkit.card)
 and one JSON line.  A CUDA device is required.
 
   python scripts/bench_nht_render.py [--iters 20] [--warmup 5] [--half]
@@ -13,23 +13,11 @@ from __future__ import annotations
 import argparse
 import json
 import math
-import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "3dgrut_b200"))
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"{torch.cuda.get_device_name()} (power limit unavailable: {e})"
+import benchkit
 
 
 def main():
@@ -38,8 +26,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--half", action="store_true", help="fp16 particle features (render.particle_feature_half)")
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_nht_render: a CUDA device is required")
+    info = benchkit.card(benchkit.cuda_device("bench_nht_render.py"))
+    print(f"device: {info}")
     import b200_native as nat
     import feature_decoder as fdm
     import scenes
@@ -129,8 +117,6 @@ def main():
                 times[name].append(ev0.elapsed_time(ev1))
     med = {k: float(np.median(v)) for k, v in times.items()}
     med["sh_frame"] = med["sh_forward"] + med["sh_backward"]
-    info = card()
-    print(f"card: {info}")
     for k, v in med.items():
         print(f"{k:>26}: {v:.3f} ms (min {min(times[k]) if k in times else v:.3f})")
     print(json.dumps({"scene": "C2 300k 800x800", "features": "fp16" if a.half else "fp32", "card": info, "median_ms": med}))

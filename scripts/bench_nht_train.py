@@ -4,7 +4,7 @@ random NHT features, then the fused NHT Adam launch against what the reference r
 
     python scripts/bench_nht_train.py [--steps 20] [--warmup 5] [--n 300000]
 
-Prints, with the card's name and power limit:
+Prints, with the card (benchkit.card):
   - device-timed steps/s of each step (CUDA events around the step; the two renderers alternate step by step),
   - the per-phase split (CUDA events between the phases, `phase_events`, in a separate loop): render, decode (the [H,W,25] slice copies
     that feed the decoder included), loss, decode_backward, render_backward, exchange, adam, densify; 3DGRT adds the BVH build,
@@ -15,30 +15,15 @@ from __future__ import annotations
 import argparse
 import json
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 LRS = dict(positions=1.6e-4, density=0.05, rotation=1e-3, scale=5e-3, features=2.5e-3, decoder=6.8e-4)
 CONF = {"model": {"feature_type": "nht", "nht_features": {"dim": 48, "activation": {"type": "sincos", "num_frequencies": 1},
                                                            "interpolation_type": "barycentric"}},
         "render": {"min_transmittance": 0.001, "pipeline_type": "referenceSlang", "backward_pipeline_type": "referenceSlangBwd"}}
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -53,13 +38,11 @@ def main():
     import feature_decoder as fdm
     import optimizers
     import scenes
+    import train_step
     import train_step_nht as tsn
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_nht_train.py measures on a CUDA device; none is present")
-    dev = torch.device("cuda", 0)
-    card = f"{torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}"
+    dev = benchkit.cuda_device("bench_nht_train.py")
+    card = benchkit.card(dev)
     print(f"device: {card}")
 
     sc = scenes.scene_c2(n=args.n)
@@ -72,21 +55,14 @@ def main():
     c2w = [np.asarray(sc.camera(i, n_views), np.float32) for i in range(n_views)]
     T = [torch.from_numpy(m)[None] for m in c2w]
     pose7 = [scenes.pose7_from_c2w(m) for m in c2w]
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
-
-    def raw():
-        dns = P[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": P[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": P[:, 4:8].clone(),
-                "scale": torch.log(P[:, 8:11]), "features": feats.clone()}
+    sensor = sc.pinhole_sensor()
 
     def decoder():
         torch.manual_seed(0)
         return fdm.FeatureDecoder(24, hidden_dim=128, num_layers=3, sh_scale=3.0).to(dev)
 
-    steps = {"C2 3DGUT": tsn.GaussianTrainStepNHT(raw(), LRS, decoder(), CONF),
-             "C4 3DGRT": tsn.GaussianTrainStepGRTNHT(raw(), LRS, decoder(), CONF)}
+    steps = {"C2 3DGUT": tsn.GaussianTrainStepNHT(train_step.raw_params(P, features=feats), LRS, decoder(), CONF),
+             "C4 3DGRT": tsn.GaussianTrainStepGRTNHT(train_step.raw_params(P, features=feats), LRS, decoder(), CONF)}
     targets = [(0.5 + 0.3 * torch.rand((H, W, 3), device=dev, generator=torch.Generator(device=dev).manual_seed(i))).contiguous()
                for i in range(n_views)]
     counters = {k: 0 for k in steps}

@@ -9,30 +9,15 @@ render over an orbit of views, alternating with the plain trace (grtb200_trace, 
   glass sphere    a glass sphere (ior 1.5) of 19,800 triangles between the camera and the Gaussians
   diffuse cube    a diffuse cube between the camera and the Gaussians
 The meshes follow the orbiting camera: the mesh BVH is rebuilt for every view, outside the timed window.  "mesh px" is the fraction of
-pixels whose colour differs from the plain trace.  Prints the card and its power limit beside the median render times.
+pixels whose colour differs from the plain trace.  Prints the card (benchkit.card) beside the median render times.
 """
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
+import benchkit
 
 
 def main():
@@ -47,10 +32,8 @@ def main():
     import playground as pg
     import scenes
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_playground: a CUDA device is required")
-    dev = torch.device("cuda", 0)
-    card = f"{torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}"
+    dev = benchkit.cuda_device("bench_playground.py")
+    card = benchkit.card(dev)
     sc = scenes.scene_c2(n=args.n)
     H, W = sc.height, sc.width
     ro_np, rd_np = sc.rays()

@@ -6,22 +6,16 @@ configs/base_gs.yaml with the MCMC perturbation: exp position decay, progressive
 Per variant it prints
   - device-timed steps/s (CUDA events around the step, inputs already on the device), median and range,
   - end-to-end steps/s with host inputs (target image copied from pinned host memory each step, wall clock to a synchronise),
-and the card's name and power limit.  Both variants render at SH degree 3 (the scheduled one starts at init_n_features 3), so the two
+and the card (benchkit.card).  Both variants render at SH degree 3 (the scheduled one starts at init_n_features 3), so the two
 do the same device work: what differs is the schedule's host update after Adam.  The loss is 0.8 L1 + 0.2 (1 - SSIM)."""
 from __future__ import annotations
 
 import argparse
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (ROOT, os.path.join(ROOT, "3dgrut_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import benchkit
 
 # configs/base_gs.yaml's schedule (the keys the schedule reads), starting at SH degree 3
 CONF = {
@@ -33,15 +27,6 @@ CONF = {
     "render": {"particle_radiance_sph_degree": 3},
 }
 SCENE_EXTENT = 3.0
-
-
-def _power_limit(index: int) -> str:
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30)
-        return out.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def main():
@@ -57,32 +42,21 @@ def main():
     import scenes
     import schedule
     import train_step
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_schedule.py measures on a CUDA device; none is present")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    print(f"device: {torch.cuda.get_device_name(dev)}, power limit {_power_limit(0)}")
+    dev = benchkit.cuda_device("bench_schedule.py")
+    print(f"device: {benchkit.card(dev)}")
 
     sc = scenes.scene_c2(n=args.n)
     H, W = sc.height, sc.width
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     P, S = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
     n_views = 10
     poses = [scenes.pose7_from_c2w(sc.camera(i, n_views)) for i in range(n_views)]
 
-    def raw_from(particles, sph):
-        dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-                "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
     sched = schedule.TrainingSchedule.from_config(CONF, scene_extent=SCENE_EXTENT)
-    truth = train_step.GaussianTrainStep(raw_from(P, S), sched.initial_lrs())
+    truth = train_step.GaussianTrainStep(train_step.raw_params(P, S), sched.initial_lrs())
     targets = [truth.render(rays_o, rays_d, sensor, p)[0][..., :3].clone() for p in poses]
     del truth
     host_targets = [t.cpu().pin_memory() for t in targets]
@@ -93,10 +67,10 @@ def main():
     # the MCMC perturbation every step (it reads the position rate); no relocation or growth, so N stays the same in both variants
     mcmc = densify.MCMCConfig(relocate_start=10 ** 9, add_start=10 ** 9, perturb_start=0, perturb_end=-1, seed=1)
     weights = dict(lambda_l1=0.8, lambda_ssim=0.2)
-    steps = {"schedule=None": train_step.GaussianTrainStep(raw_from(P2, S), sched.initial_lrs(), densify_conf=mcmc, scene_extent=SCENE_EXTENT,
-                                                           **weights),
-             "schedule": train_step.GaussianTrainStep(raw_from(P2, S), None, schedule=sched, densify_conf=mcmc, scene_extent=SCENE_EXTENT,
-                                                      **weights)}
+    steps = {"schedule=None": train_step.GaussianTrainStep(train_step.raw_params(P2, S), sched.initial_lrs(), densify_conf=mcmc,
+                                                           scene_extent=SCENE_EXTENT, **weights),
+             "schedule": train_step.GaussianTrainStep(train_step.raw_params(P2, S), None, schedule=sched, densify_conf=mcmc,
+                                                      scene_extent=SCENE_EXTENT, **weights)}
     counters = {k: 0 for k in steps}
 
     def one(name, host=False):

@@ -6,7 +6,7 @@ SSIM, configs/strategy/*.yaml), times K steps of train() (validation, checkpoint
 bare loop, `--repeats` pairs in alternating order.  K defaults to 1500, so that the strategies (which start at step 500) densify, prune,
 relocate and add inside the timed window.  Reports steps/s of each, the loop's median overhead per step beside the range of each, and
 from a separate bare run the per-phase device time (phase_events), the densifier's per-step gradient buffer on its own, the number of
-steps on which the strategy changed the Gaussians, the dataset start-up time, and the card's name and power limit.  One JSON line.
+steps on which the strategy changed the Gaussians, the dataset start-up time, and the card (benchkit.card).  One JSON line.
 
     python scripts/bench_train.py --steps 1500 --repeats 4
 """
@@ -15,13 +15,13 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "3dgrut_b200"), os.path.join(ROOT, "tests")]
+import benchkit
+
+sys.path.insert(0, os.path.join(benchkit.ROOT, "tests"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
@@ -33,28 +33,14 @@ import trainer  # noqa: E402
 from scene_fixtures import run_conf, write_nerf  # noqa: E402
 
 
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        return out.stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
-
-
 def write_scene(root, views=100):
-    from train_step import GaussianTrainStep
-    import threedgut_tracer.tracer as tr
+    from train_step import GaussianTrainStep, raw_params
 
     sc = scenes.scene_c2()
-    p = torch.from_numpy(sc.particles).cuda()
-    d = p[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    params = {"positions": p[:, 0:3].contiguous(), "density": torch.log(d / (1 - d)), "rotation": p[:, 4:8].contiguous(),
-              "scale": torch.log(p[:, 8:11]).contiguous(), "features_albedo": torch.from_numpy(sc.sph[:, :3]).cuda().contiguous(),
-              "features_specular": torch.from_numpy(sc.sph[:, 3:]).cuda().contiguous()}
+    params = raw_params(torch.from_numpy(sc.particles).cuda(), torch.from_numpy(sc.sph).cuda())
     truth = GaussianTrainStep(params, {k: 0.0 for k in params}, sph_degree=3)
     ro, rd = (torch.from_numpy(a).cuda() for a in scenes.pinhole_rays(sc.height, sc.width, sc.fx, sc.fy, sc.cx, sc.cy))
-    sensor = tr.fromOpenCVPinholeCameraModelParameters([sc.width, sc.height], tr.ShutterType.GLOBAL, [sc.cx, sc.cy], [sc.fx, sc.fy],
-                                                        np.zeros(6), np.zeros(2), np.zeros(4))
+    sensor = sc.pinhole_sensor()
     frames = {}
     for split, n, off in (("train", views, 0.0), ("val", 2, 0.31), ("test", 4, 0.57)):
         rows = []
@@ -143,9 +129,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=4, help="(train(), bare loop) pairs, their order alternating")
     ap.add_argument("--views", type=int, default=100)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_train.py measures on a CUDA device; none is visible")
-    result = {"card": card(), "steps": args.steps, "repeats": args.repeats}
+    result = {"card": benchkit.card(benchkit.cuda_device("bench_train.py")), "steps": args.steps, "repeats": args.repeats}
     with tempfile.TemporaryDirectory() as tmp:
         root = os.path.join(tmp, "c2")
         t = time.perf_counter()

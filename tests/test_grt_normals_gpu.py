@@ -12,6 +12,7 @@ import pytest
 import scenes
 from helpers import image_error_report, packet_share, permute_pixels, ray_sample, rel_l2, shuffled_pixels, unpermute_pixels
 from oracle import gut_oracle as go
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 
@@ -260,12 +261,6 @@ def test_tracer_render_pred_normals_and_their_missing_gradient(prim):
 LRS = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
 
 
-def _raw_from(particles, sph):
-    dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-            "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
-
 def _no_normals_entry(monkeypatch):
     import b200_native as nat
 
@@ -290,7 +285,7 @@ def test_grt_train_step_ignores_the_normals_key(monkeypatch):
     target = (torch.rand((96, 96, 3), device=dev, generator=torch.Generator(device=dev).manual_seed(3)) * 0.8).contiguous()
     ends = {}
     for normals in (False, True):
-        step = train_step_grt.GaussianTrainStepGRT(_raw_from(P, S), LRS, conf={"render": {"enable_normals": normals}})
+        step = train_step_grt.GaussianTrainStepGRT(raw_params(P, S), LRS, conf={"render": {"enable_normals": normals}})
         for i in range(3):
             step.step(rays_o, rays_d, poses[i], target)
         torch.cuda.synchronize()
@@ -306,7 +301,7 @@ def test_hybrid_train_step_steps_with_the_normals_key(monkeypatch):
 
     _no_normals_entry(monkeypatch)
     sc, rays_o, rays_d, P, S, poses, sensor = _setup()
-    step = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS, conf={"render": {"enable_normals": True}})
+    step = th.GaussianTrainStepHybrid(raw_params(P, S), LRS, conf={"render": {"enable_normals": True}})
     target = (torch.rand((sc.height, sc.width, 3), device=P.device, generator=torch.Generator(device=P.device).manual_seed(3)) * 0.8).contiguous()
     before = step.params["positions"].detach().clone()
     losses = [float(step.step(rays_o, rays_d, sensor, poses[1], target)) for _ in range(2)]

@@ -8,6 +8,7 @@ import pytest
 
 import scenes
 from helpers import rel_l2
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -18,12 +19,6 @@ PAPER = {"render": {"primitive_type": "icosahedron", "particle_kernel_degree": 2
                     "max_consecutive_bvh_update": 15}}
 CONFIGS = {"instances": INSTANCES, "icosahedron_paper": PAPER}
 LRS = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
-
-
-def _raw_from(particles, sph):
-    dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-            "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
 
 
 def _setup(n=600, size=96, dev=None):
@@ -161,7 +156,7 @@ def test_one_step_matches_autograd(config, weights):
     import train_step_grt
 
     sc, rays_o, rays_d, P, S, poses = _setup()
-    step = train_step_grt.GaussianTrainStepGRT(_raw_from(P, S), LRS, conf=CONFIGS[config], lambda_l1=weights[0], lambda_ssim=weights[1])
+    step = train_step_grt.GaussianTrainStepGRT(raw_params(P, S), LRS, conf=CONFIGS[config], lambda_l1=weights[0], lambda_ssim=weights[1])
     gen = torch.Generator(device=P.device).manual_seed(3)
     target = (torch.rand((sc.height, sc.width, 3), device=P.device, generator=gen) * 0.8).contiguous()
     particles, sph = step.activated()
@@ -196,10 +191,10 @@ def _fit_setup(config, raw_perturb, **kw):
     import train_step_grt
 
     sc, rays_o, rays_d, P, S, poses = _setup()
-    truth = train_step_grt.GaussianTrainStepGRT(_raw_from(P, S), LRS, conf=CONFIGS[config])
+    truth = train_step_grt.GaussianTrainStepGRT(raw_params(P, S), LRS, conf=CONFIGS[config])
     targets = [truth.render(rays_o, rays_d, p)[0][0].clone() for p in poses]
     P2, S2 = raw_perturb(sc, P.clone(), S.clone())
-    fit = train_step_grt.GaussianTrainStepGRT(_raw_from(P2, S2), LRS, conf=CONFIGS[config], **kw)
+    fit = train_step_grt.GaussianTrainStepGRT(raw_params(P2, S2), LRS, conf=CONFIGS[config], **kw)
 
     def mean_loss():
         return float(np.mean([float((fit.render(rays_o, rays_d, p)[0][0] - t).abs().mean()) for p, t in zip(poses, targets)]))
@@ -301,7 +296,7 @@ def _rank_worker(rank, world, port, out_dir):
         dev = torch.device("cuda", rank)
         sc, rays_o, rays_d, P, S, poses = _setup(dev=dev)
         targets = torch.from_numpy(np.load(os.path.join(out_dir, "targets.npy"))).to(dev)
-        fit = train_step_grt.GaussianTrainStepGRT(_raw_from(*_perturb(sc, P.clone(), S.clone())), LRS, selective=True)
+        fit = train_step_grt.GaussianTrainStepGRT(raw_params(*_perturb(sc, P.clone(), S.clone())), LRS, selective=True)
         seen = _capture_adam(fit)
         for it in range(20):
             views = [vp.views_for_rank(it, r, world, 6)[0] for r in range(world)]
@@ -323,7 +318,7 @@ def test_two_ranks_stay_bit_identical(tmp_path):
 
     world = 2
     sc, rays_o, rays_d, P, S, poses = _setup()
-    truth = train_step_grt.GaussianTrainStepGRT(_raw_from(P, S), LRS)
+    truth = train_step_grt.GaussianTrainStepGRT(raw_params(P, S), LRS)
     targets = torch.stack([truth.render(rays_o, rays_d, p)[0][0] for p in poses])
     np.save(tmp_path / "targets.npy", targets.cpu().numpy())
     mp.spawn(_rank_worker, args=(world, _free_port(), str(tmp_path)), nprocs=world, join=True)
@@ -334,7 +329,7 @@ def test_two_ranks_stay_bit_identical(tmp_path):
     # the first step's exchanged gradient == the serial sum of the two ranks' single-view gradients (each normalised by the batch of 2)
     want_p = want_s = 0.0
     for r in range(world):
-        single = train_step_grt.GaussianTrainStepGRT(_raw_from(*_perturb(sc, P.clone(), S.clone())), LRS)
+        single = train_step_grt.GaussianTrainStepGRT(raw_params(*_perturb(sc, P.clone(), S.clone())), LRS)
         seen = _capture_adam(single)
         v = vp.views_for_rank(0, r, world, 6)[0]
         single.step(rays_o, rays_d, poses[v], targets[v])

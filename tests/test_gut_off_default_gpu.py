@@ -293,7 +293,6 @@ def test_compact_exchange_at_sh_degree(deg, k):
     [N,4] radiance gradients equals the sum of the two views' full d_sph rows, zeros beyond (deg + 1)^2 included.  k = 16: the compact
     backward of the sorted variant (G8's COMPACT, non-canonical instantiation, which reads final gradients from the accumulator rows)."""
     import threedgut_tracer
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1()
@@ -302,9 +301,7 @@ def test_compact_exchange_at_sh_degree(deg, k):
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     W, H = sc.width, sc.height
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     gen = torch.Generator(device=dev).manual_seed(deg)
     full_ds, gs, pos = [], [], []
     for view in (2, 7):

@@ -548,7 +548,6 @@ def test_compact_exchange_without_distance_gradient(d_dist):
 
 def _compact_exchange(d_dist):
     import threedgut_tracer
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1()
@@ -557,9 +556,7 @@ def _compact_exchange(d_dist):
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     W, H = sc.width, sc.height
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     full_dp, full_ds, gs, pos, ref_ds = [], [], [], [], []
     for view in (2, 7):
         pose = scenes.pose7_from_c2w(sc.camera(view, 10))

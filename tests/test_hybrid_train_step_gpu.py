@@ -9,6 +9,7 @@ import pytest
 
 import scenes
 from helpers import rel_l2
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -18,12 +19,6 @@ INSTANCES = {"render": {}}
 PAPER = {"render": {"primitive_type": "icosahedron", "particle_kernel_density_clamping": False, "max_consecutive_bvh_update": 15}}
 CONFIGS = {"instances": INSTANCES, "icosahedron_paper": PAPER}
 LRS = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
-
-
-def _raw_from(particles, sph):
-    dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-            "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
 
 
 class _Batch:
@@ -40,16 +35,13 @@ class _Batch:
 
 
 def _setup(n=600, size=96, dev=None):
-    from threedgut_tracer.tracer import Tracer
-
     dev = dev or torch.device("cuda", 0)
     sc = scenes.scene_c1(n=n, width=size, height=size)
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     P, S = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
     poses = [torch.from_numpy(np.asarray(sc.camera(i, 6), np.float32))[None] for i in range(6)]  # host [1,4,4] camera-to-world
-    sensor = Tracer._create_camera_parameters(_Batch(sc, rays_o, rays_d, poses[0]))[0]
-    return sc, rays_o, rays_d, P, S, poses, sensor
+    return sc, rays_o, rays_d, P, S, poses, sc.pinhole_sensor()
 
 
 def _capture_adam(step):
@@ -256,7 +248,7 @@ def test_one_step_matches_autograd(config, weights, background):
     mask = None
     if white:
         mask = (torch.rand((H, W), device=dev, generator=torch.Generator(device=dev).manual_seed(4)) > 0.2).float()
-    step = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS, conf=CONFIGS[config], lambda_l1=weights[0], lambda_ssim=weights[1],
+    step = th.GaussianTrainStepHybrid(raw_params(P, S), LRS, conf=CONFIGS[config], lambda_l1=weights[0], lambda_ssim=weights[1],
                                       background="white" if white else "black")
     gen = torch.Generator(device=dev).manual_seed(3)
     target = (torch.rand((H, W, 3), device=dev, generator=gen) * 0.8).contiguous()
@@ -303,8 +295,8 @@ def test_reflectivity_zero_gives_the_3dgut_steps_gradients():
     sc, rays_o, rays_d, P, S, poses, sensor = _setup()
     gen = torch.Generator(device=P.device).manual_seed(7)
     target = (torch.rand((sc.height, sc.width, 3), device=P.device, generator=gen) * 0.8).contiguous()
-    hyb = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS, mirror=dict(reflectivity=0.0), lambda_l1=0.8, lambda_ssim=0.2)
-    gut = [train_step.GaussianTrainStep(_raw_from(P, S), LRS, conf=th.hybrid_render_conf(None), lambda_l1=0.8, lambda_ssim=0.2) for _ in range(2)]
+    hyb = th.GaussianTrainStepHybrid(raw_params(P, S), LRS, mirror=dict(reflectivity=0.0), lambda_l1=0.8, lambda_ssim=0.2)
+    gut = [train_step.GaussianTrainStep(raw_params(P, S), LRS, conf=th.hybrid_render_conf(None), lambda_l1=0.8, lambda_ssim=0.2) for _ in range(2)]
     a, b = _capture_adam(hyb), [_capture_adam(s) for s in gut]
     hyb.step(rays_o, rays_d, sensor, poses[3], target)
     for s in gut:
@@ -327,7 +319,7 @@ def test_render_matches_render_hybrid():
 
     sc, rays_o, rays_d, P, S, poses, sensor = _setup()
     conf = th.hybrid_render_conf(None)
-    step = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS)
+    step = th.GaussianTrainStepHybrid(raw_params(P, S), LRS)
     particles, sph = step.activated()
     g = _Gaussians(particles, sph, 3)
     gut, grt = threedgut_tracer.Tracer(conf), threedgrt_tracer.Tracer(conf)
@@ -359,10 +351,10 @@ def _fit(start, steps, conf=INSTANCES, **kw):
     import train_step_hybrid as th
 
     sc, rays_o, rays_d, P, S, poses, sensor = _setup()
-    truth = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS, conf=conf)
+    truth = th.GaussianTrainStepHybrid(raw_params(P, S), LRS, conf=conf)
     targets = [truth.render(rays_o, rays_d, sensor, p)[0].clone() for p in poses]
     P2, S2 = start(sc, P.clone(), S.clone())
-    fit = th.GaussianTrainStepHybrid(_raw_from(P2, S2), LRS, conf=conf, **kw)
+    fit = th.GaussianTrainStepHybrid(raw_params(P2, S2), LRS, conf=conf, **kw)
 
     def mean_loss():
         return float(np.mean([float((fit.render(rays_o, rays_d, sensor, p)[0] - t).abs().mean()) for p, t in zip(poses, targets)]))
@@ -433,7 +425,7 @@ def _rank_worker(rank, world, port, out_dir):
         dev = torch.device("cuda", rank)
         sc, rays_o, rays_d, P, S, poses, sensor = _setup(dev=dev)
         targets = torch.from_numpy(np.load(os.path.join(out_dir, "targets.npy"))).to(dev)
-        fit = th.GaussianTrainStepHybrid(_raw_from(*_perturb(sc, P.clone(), S.clone())), LRS, selective=True)
+        fit = th.GaussianTrainStepHybrid(raw_params(*_perturb(sc, P.clone(), S.clone())), LRS, selective=True)
         for it in range(20):
             views = [vp.views_for_rank(it, r, world, 6)[0] for r in range(world)]
             positions = np.stack([np.asarray(poses[v][0, :3, 3], np.float32) for v in views])
@@ -453,7 +445,7 @@ def test_two_ranks_stay_bit_identical(tmp_path):
 
     world = 2
     sc, rays_o, rays_d, P, S, poses, sensor = _setup()
-    truth = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS)
+    truth = th.GaussianTrainStepHybrid(raw_params(P, S), LRS)
     targets = torch.stack([truth.render(rays_o, rays_d, sensor, p)[0] for p in poses])
     np.save(tmp_path / "targets.npy", targets.cpu().numpy())
     mp.spawn(_rank_worker, args=(world, _free_port(), str(tmp_path)), nprocs=world, join=True)

@@ -9,7 +9,8 @@ import pytest
 
 import scenes
 from helpers import rel_l2
-from test_grt_train_step_gpu import CONFIGS, LRS, _Batch, _free_port, _ImageLoss, _perturb, _raw_from, _setup
+from test_grt_train_step_gpu import CONFIGS, LRS, _Batch, _free_port, _ImageLoss, _perturb, _setup
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -53,13 +54,8 @@ class _Harness:
         self.dev = self.P.device
         self.H, self.W = self.sc.height, self.sc.width
         if self.gut:
-            from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
-
-            sc = self.sc
-            self.sensor = fromOpenCVPinholeCameraModelParameters(np.array([sc.width, sc.height]), ShutterType.GLOBAL,
-                                                                 np.array([sc.cx, sc.cy], np.float32), np.array([sc.fx, sc.fy], np.float32),
-                                                                 np.zeros(6, np.float32), np.zeros(2, np.float32), np.zeros(4, np.float32))
-            self.views = [scenes.pose7_from_c2w(sc.camera(i, 6)) for i in range(6)]
+            self.sensor = self.sc.pinhole_sensor()
+            self.views = [scenes.pose7_from_c2w(self.sc.camera(i, 6)) for i in range(6)]
             self.conf = SORTED if kind == "gut_sorted" else None
         else:
             self.conf = CONFIGS[kind[len("grt_"):]]
@@ -116,7 +112,7 @@ class _Harness:
 def _step_against_autograd(hz, background, use_mask, lo, ls, weights=(0.8, 0.2)):
     """One bias-corrected step; returns ({group: rel-L2 of exp_avg / (1 - b1) against the autograd raw gradient}, step loss, autograd loss)."""
     H, W, dev = hz.H, hz.W, hz.dev
-    raw = _raw_from(hz.P, hz.S)
+    raw = raw_params(hz.P, hz.S)
     st = hz.make({k: v.clone() for k, v in raw.items()}, lambda_l1=weights[0], lambda_ssim=weights[1], background=background, background_seed=5,
                  lambda_opacity=lo, lambda_scale=ls)
     gen = torch.Generator(device=dev).manual_seed(3)
@@ -210,13 +206,13 @@ def _mean_composited_l1(hz, st, targets, bg=0.0):
 @pytest.mark.parametrize("kind", KINDS)
 def test_fit_over_a_white_background(kind):
     hz = _Harness(kind)
-    truth = hz.make(_raw_from(hz.P, hz.S))
+    truth = hz.make(raw_params(hz.P, hz.S))
     targets = []
     for v in range(6):
         rgb, alpha = hz.render(truth, v)
         targets.append((rgb + (1.0 - alpha)).clone())
     P2, S2 = _perturb(hz.sc, hz.P.clone(), hz.S.clone())
-    fit = hz.make(_raw_from(P2, S2), background="white")
+    fit = hz.make(raw_params(P2, S2), background="white")
     before = _mean_composited_l1(hz, fit, targets, 1.0)
     for it in range(90):
         hz.step(fit, it % 6, targets[it % 6])
@@ -232,7 +228,7 @@ def test_mcmc_fit_with_the_regularisers(kind):
     import densify
 
     hz = _Harness(kind)
-    truth = hz.make(_raw_from(hz.P, hz.S))
+    truth = hz.make(raw_params(hz.P, hz.S))
     targets = [hz.render(truth, v)[0].clone() for v in range(6)]
     P2, S2 = _perturb(hz.sc, hz.P.clone(), hz.S.clone())
     gen = torch.Generator(device=hz.dev).manual_seed(9)
@@ -244,7 +240,7 @@ def test_mcmc_fit_with_the_regularisers(kind):
     results = {}
     for lam in (0.0, 0.01):  # base_mcmc.yaml: lambda_opacity = lambda_scale = 0.01
         conf = densify.MCMCConfig(relocate_start=5, relocate_frequency=20, add_start=5, add_frequency=20, perturb_start=0, noise_lr=5e3, seed=2)
-        fit = hz.make(_raw_from(P2.clone(), S2.clone()), densify_conf=conf, lambda_opacity=lam, lambda_scale=lam)
+        fit = hz.make(raw_params(P2.clone(), S2.clone()), densify_conf=conf, lambda_opacity=lam, lambda_scale=lam)
         before = _mean_composited_l1(hz, fit, targets)
         for it in range(90):
             hz.step(fit, it % 6, targets[it % 6])
@@ -276,7 +272,7 @@ def _rank_worker(rank, world, port, out_dir):
         dev = torch.device("cuda", rank)
         sc, rays_o, rays_d, P, S, poses = _setup(dev=dev)
         targets = torch.from_numpy(np.load(os.path.join(out_dir, "targets.npy"))).to(dev)
-        fit = train_step_grt.GaussianTrainStepGRT(_raw_from(*_perturb(sc, P.clone(), S.clone())), LRS, selective=True, background="random",
+        fit = train_step_grt.GaussianTrainStepGRT(raw_params(*_perturb(sc, P.clone(), S.clone())), LRS, selective=True, background="random",
                                                   lambda_opacity=0.01, lambda_scale=0.01)
         first_bg = None
         for it in range(20):
@@ -299,7 +295,7 @@ def test_two_ranks_with_random_background_and_regularisers_stay_bit_identical(tm
 
     world = 2
     sc, rays_o, rays_d, P, S, poses = _setup()
-    truth = train_step_grt.GaussianTrainStepGRT(_raw_from(P, S), LRS)
+    truth = train_step_grt.GaussianTrainStepGRT(raw_params(P, S), LRS)
     targets = torch.stack([truth.render(rays_o, rays_d, p)[0][0] for p in poses])
     np.save(tmp_path / "targets.npy", targets.cpu().numpy())
     mp.spawn(_rank_worker, args=(world, _free_port(), str(tmp_path)), nprocs=world, join=True)

@@ -12,6 +12,7 @@ from helpers import rel_l2
 from test_grt_train_step_gpu import _free_port, _setup
 from test_loss_terms_step_gpu import _ImageLoss
 from test_nht_train_step import _einsum_dirs
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -34,18 +35,10 @@ def _decoder(seed=0):
     return fdm.FeatureDecoder(24, hidden_dim=128, num_layers=3, sh_scale=3.0).cuda()  # the shipped net (configs/base_gs.yaml)
 
 
-def _raw_from(particles, feats):
-    dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-            "scale": torch.log(particles[:, 8:11]), "features": feats.clone()}
-
-
 class _Harness:
     """C1, 600 Gaussians, 96x96, 6 views, random NHT features, through either NHT step."""
 
     def __init__(self, kind, half=False):
-        from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
-
         import scenes
 
         self.kind, self.half = kind, half
@@ -55,9 +48,7 @@ class _Harness:
         rng = np.random.default_rng(5)
         self.F = torch.from_numpy(rng.uniform(-math.pi / 2, math.pi / 2, (self.sc.n, 48)).astype(np.float32)).to(self.dev)
         sc = self.sc
-        self.sensor = fromOpenCVPinholeCameraModelParameters(np.array([sc.width, sc.height]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                             np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32),
-                                                             np.zeros(2, np.float32), np.zeros(4, np.float32))
+        self.sensor = sc.pinhole_sensor()
         self.views = [scenes.pose7_from_c2w(sc.camera(i, 6)) for i in range(6)]
 
     def make(self, raw, decoder, conf=None, **kw):
@@ -109,7 +100,7 @@ def _step_against_autograd(hz, composite):
     weights, lo, ls = ((0.8, 0.2), 0.01, 0.02) if composite else ((1.0, 0.0), 0.0, 0.0)
     dec = _decoder()
     params0 = dec.network.params.detach().clone()
-    raw = _raw_from(hz.P, hz.F)
+    raw = raw_params(hz.P, features=hz.F)
     kw = dict(background="white", lambda_opacity=lo, lambda_scale=ls) if composite else {}
     st = hz.make({k: v.clone() for k, v in raw.items()}, dec, lambda_l1=weights[0], lambda_ssim=weights[1], **kw)
     gen = torch.Generator(device=dev).manual_seed(3)
@@ -277,7 +268,7 @@ def test_trace_bwd_into_out_equals_the_plain_call(kind):
 
     hz = _Harness(kind)
     dev = hz.dev
-    raw = _raw_from(hz.P, hz.F)
+    raw = raw_params(hz.P, features=hz.F)
     st = hz.make(raw, _decoder())
     particles, feats = st.activated()
     g = torch.Generator(device=dev).manual_seed(8)
@@ -322,7 +313,7 @@ def _fit_decoder():
 
 
 def _targets(hz, dec, views=6):
-    truth = hz.make(_raw_from(hz.P, hz.F), dec)
+    truth = hz.make(raw_params(hz.P, features=hz.F), dec)
     return [hz.render(truth, v)[0].clone() for v in range(views)]
 
 
@@ -331,7 +322,7 @@ def _perturbed(hz):
     P2 = hz.P.clone()
     P2[:, 0:3] += torch.from_numpy(0.03 * rng.normal(size=(hz.sc.n, 3)).astype(np.float32)).to(hz.dev)
     F2 = hz.F + torch.from_numpy(0.5 * rng.normal(size=(hz.sc.n, 48)).astype(np.float32)).to(hz.dev)
-    return _raw_from(P2, F2)
+    return raw_params(P2, features=F2)
 
 
 def _mean_l1(hz, st, targets):
@@ -378,8 +369,8 @@ def test_color_refinement_freezes_the_geometry(kind):
     gen = torch.Generator(device=hz.dev).manual_seed(6)
     target = (torch.rand((hz.H, hz.W, 3), device=hz.dev, generator=gen) * 0.8).contiguous()
     mcmc = densify.MCMCConfig(relocate_start=0, relocate_frequency=1, add_start=0, add_frequency=1, perturb_start=0, noise_lr=5e3, seed=2)
-    st = hz.make(_raw_from(hz.P, hz.F), _decoder(), conf=conf, lambda_opacity=0.01, lambda_scale=0.01, densify_conf=mcmc)
-    plain = hz.make(_raw_from(hz.P, hz.F), _decoder(), conf=conf)
+    st = hz.make(raw_params(hz.P, features=hz.F), _decoder(), conf=conf, lambda_opacity=0.01, lambda_scale=0.01, densify_conf=mcmc)
+    plain = hz.make(raw_params(hz.P, features=hz.F), _decoder(), conf=conf)
     assert st.color_refine_start == 0
     geo = {k: st.params[k].clone() for k in GEOMETRY}
     feats, dec = st.params["features"].clone(), st.decoder.network.params.detach().clone()

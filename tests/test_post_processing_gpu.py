@@ -7,6 +7,7 @@ import pytest
 
 import post_processing_oracle as ppo
 from helpers import rel_l2
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -175,12 +176,11 @@ SH_CASES = [("gut", "white", True, (0.8, 0.2)), ("gut", "black", False, (1.0, 0.
 def test_sh_step_matches_autograd(kind, background, use_mask, weights):
     """GaussianTrainStep (3DGUT) and GaussianTrainStepGRT: exp_avg / (1 - b1) after one bias-corrected step against the autograd gradient,
     at the bars of test_loss_terms_step_gpu.py."""
-    from test_grt_train_step_gpu import _raw_from
     from test_loss_terms_step_gpu import _Harness, _step_against_autograd
 
     hz = _Harness(kind)
     H, W, dev = hz.H, hz.W, hz.dev
-    raw = _raw_from(hz.P, hz.S)
+    raw = raw_params(hz.P, hz.S)
     st = hz.make({k: v.clone() for k, v in raw.items()}, lambda_l1=weights[0], lambda_ssim=weights[1], background=background, background_seed=5,
                  post_processing=POST)
     target, mask = _target_and_mask(H, W, dev, use_mask)
@@ -215,14 +215,14 @@ def test_nht_step_matches_autograd(kind):
     import feature_decoder as fdm
     import train_step_nht as tsn
     from test_nht_train_step import _einsum_dirs
-    from test_nht_train_step_gpu import _decoder, _Harness, _raw_from
+    from test_nht_train_step_gpu import _decoder, _Harness
 
     hz = _Harness(kind)
     H, W, dev = hz.H, hz.W, hz.dev
     weights = (0.8, 0.2)
     dec = _decoder()
     params0 = dec.network.params.detach().clone()
-    raw = _raw_from(hz.P, hz.F)
+    raw = raw_params(hz.P, features=hz.F)
     st = hz.make({k: v.clone() for k, v in raw.items()}, dec, lambda_l1=weights[0], lambda_ssim=weights[1], background="white",
                  post_processing=POST)
     target, mask = _target_and_mask(H, W, dev, True)
@@ -264,7 +264,7 @@ def test_hybrid_step_matches_autograd(background):
     import threedgrt_tracer
     import threedgut_tracer
     import train_step_hybrid as th
-    from test_hybrid_train_step_gpu import CONFIGS, LRS, _Batch, _capture_adam, _Gaussians, _raw_from, _SecondaryBatch, _setup
+    from test_hybrid_train_step_gpu import CONFIGS, LRS, _Batch, _capture_adam, _Gaussians, _SecondaryBatch, _setup
 
     sc, rays_o, rays_d, P, S, poses, sensor = _setup()
     dev = P.device
@@ -272,7 +272,7 @@ def test_hybrid_step_matches_autograd(background):
     white = background != "black"
     weights = (0.8, 0.2) if white else (1.0, 0.0)
     target, mask = _target_and_mask(H, W, dev, white)
-    step = th.GaussianTrainStepHybrid(_raw_from(P, S), LRS, conf=CONFIGS["instances"], lambda_l1=weights[0], lambda_ssim=weights[1],
+    step = th.GaussianTrainStepHybrid(raw_params(P, S), LRS, conf=CONFIGS["instances"], lambda_l1=weights[0], lambda_ssim=weights[1],
                                       background="white" if white else "black", post_processing=POST)
     particles, sph = step.activated()
     seen = _capture_adam(step)
@@ -308,14 +308,14 @@ def test_hybrid_step_matches_autograd(background):
 def test_fit_to_srgb_targets(kind):
     """Targets rendered sRGB-encoded from the unperturbed scene; 90 steps of the perturbed scene with the encode in the loss bring the
     encoded L1 down by the factor of the existing fits."""
-    from test_grt_train_step_gpu import _perturb, _raw_from
+    from test_grt_train_step_gpu import _perturb
     from test_loss_terms_step_gpu import _Harness, _mean_composited_l1
 
     hz = _Harness(kind)
-    truth = hz.make(_raw_from(hz.P, hz.S), post_processing=POST)
+    truth = hz.make(raw_params(hz.P, hz.S), post_processing=POST)
     targets = [hz.render(truth, v)[0].clone() for v in range(6)]   # render() returns the encoded rgb
     P2, S2 = _perturb(hz.sc, hz.P.clone(), hz.S.clone())
-    fit = hz.make(_raw_from(P2, S2), post_processing=POST)
+    fit = hz.make(raw_params(P2, S2), post_processing=POST)
     before = _mean_composited_l1(hz, fit, targets)
     for it in range(90):
         hz.step(fit, it % 6, targets[it % 6])

@@ -25,12 +25,6 @@ STEPS, EVERY, N_VIEWS = 300, 50, 6
 LRS = dict(positions=1e-3, density=0.02, rotation=1e-3, scale=3e-3, features_albedo=5e-3, features_specular=2.5e-4)
 
 
-def _raw_from(particles, sph):
-    dns = np.clip(particles[:, 3:4], 1e-4, 1 - 1e-4)
-    return {"positions": particles[:, 0:3].copy(), "density": np.log(dns / (1 - dns)).astype(np.float32), "rotation": particles[:, 4:8].copy(),
-            "scale": np.log(particles[:, 8:11]).astype(np.float32), "features_albedo": sph[:, 0:3].copy(), "features_specular": sph[:, 3:48].copy()}
-
-
 def _activate(raw):
     """model.py:94-118 in numpy float32: [N,12] particles + [N,48] SH"""
     f32 = np.float32
@@ -50,7 +44,6 @@ def test_psnr_trajectories_match_the_oracle_driven_training():
     import train_step
     from oracle import adam_oracle as ao
     from oracle import gut_oracle as go
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1(n=600, width=96, height=96)
@@ -71,12 +64,10 @@ def test_psnr_trajectories_match_the_oracle_driven_training():
     P2[:, 0:3] += (0.02 * rng.normal(size=(sc.n, 3))).astype(np.float32)
     P2[:, 8:11] *= np.exp(0.2 * rng.normal(size=(sc.n, 3))).astype(np.float32)
     S2[:, 0:3] += (0.5 * rng.normal(size=(sc.n, 3))).astype(np.float32)
-    raw0 = _raw_from(P2, S2)
+    raw0 = {k: v.numpy() for k, v in train_step.raw_params(torch.from_numpy(P2), torch.from_numpy(S2)).items()}
 
     # ---- GPU arm
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     fit = train_step.GaussianTrainStep({k: torch.from_numpy(v.copy()).to(dev) for k, v in raw0.items()}, LRS, sph_degree=deg)
     t_targets = [torch.from_numpy(t).to(dev) for t in targets]

@@ -41,22 +41,14 @@ def _psnr(a, b):
     return float("inf") if mse == 0 else 10 * math.log10(255.0 ** 2 / mse)
 
 
-def _params(sc):
-    p = torch.from_numpy(sc.particles).cuda()
-    d = p[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    return {"positions": p[:, 0:3].contiguous(), "density": torch.log(d / (1 - d)), "rotation": p[:, 4:8].contiguous(),
-            "scale": torch.log(p[:, 8:11]).contiguous(), "features_albedo": torch.from_numpy(sc.sph[:, :3]).cuda().contiguous(),
-            "features_specular": torch.from_numpy(sc.sph[:, 3:]).cuda().contiguous()}
-
-
 @pytest.fixture(scope="module")
 def truth():
     """(3DGUT step, 3DGRT step) holding the ground-truth Gaussians."""
-    from train_step import GaussianTrainStep
+    from train_step import GaussianTrainStep, raw_params
     from train_step_grt import GaussianTrainStepGRT
 
     sc = scenes.scene_c1(n=1000)
-    params = _params(sc)
+    params = raw_params(torch.from_numpy(sc.particles).cuda(), torch.from_numpy(sc.sph).cuda())
     lrs = {k: 0.0 for k in params}
     grt_conf = {"render": run_conf("", "", method="3dgrt")["render"]}
     return sc, GaussianTrainStep(params, lrs, sph_degree=3), GaussianTrainStepGRT({k: v.clone() for k, v in params.items()}, lrs, conf=grt_conf,

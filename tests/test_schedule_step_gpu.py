@@ -11,6 +11,7 @@ import scenes
 from helpers import rel_l2
 from test_hybrid_train_step_gpu import _setup
 from test_schedule import BASE_MCMC, NHT_MCMC, _Reference, _with
+from train_step import raw_params
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -67,13 +68,7 @@ class _Run:
         return self.kind.endswith("nht")
 
     def raw(self, P, S, F):
-        dns = P[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        out = {"positions": P[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": P[:, 4:8].clone(), "scale": torch.log(P[:, 8:11])}
-        if self.nht:
-            out["features"] = F.clone()
-        else:
-            out.update(features_albedo=S[:, 0:3].clone(), features_specular=S[:, 3:48].clone())
-        return out
+        return raw_params(P, features=F) if self.nht else raw_params(P, S)
 
     def start(self):
         return self.raw(self.P2, self.S2, self.F2)

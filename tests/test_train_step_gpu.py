@@ -13,26 +13,17 @@ torch = pytest.importorskip("torch")
 @pytest.mark.parametrize("loss_weights", [(1.0, 0.0), (0.8, 0.2)])
 def test_short_fit_reduces_the_loss(loss_weights):
     import train_step
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1(n=600, width=96, height=96)
-    W, H = sc.width, sc.height
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     P = torch.from_numpy(sc.particles).to(dev)
     S = torch.from_numpy(sc.sph).to(dev)
 
-    def raw_from(particles, sph):
-        dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-                "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
     lrs = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
-    truth = train_step.GaussianTrainStep(raw_from(P, S), lrs)
+    truth = train_step.GaussianTrainStep(train_step.raw_params(P, S), lrs)
     views = [scenes.pose7_from_c2w(sc.camera(i, 6)) for i in range(6)]
     targets = [truth.render(rays_o, rays_d, sensor, p)[0][..., :3].clone() for p in views]
     gen = torch.Generator(device=dev).manual_seed(0)
@@ -40,7 +31,7 @@ def test_short_fit_reduces_the_loss(loss_weights):
     P2[:, 0:3] += 0.02 * torch.randn((sc.n, 3), device=dev, generator=gen)
     P2[:, 8:11] *= torch.exp(0.2 * torch.randn((sc.n, 3), device=dev, generator=gen))
     S2[:, 0:3] += 0.5 * torch.randn((sc.n, 3), device=dev, generator=gen)
-    fit = train_step.GaussianTrainStep(raw_from(P2, S2), lrs, lambda_l1=loss_weights[0], lambda_ssim=loss_weights[1])
+    fit = train_step.GaussianTrainStep(train_step.raw_params(P2, S2), lrs, lambda_l1=loss_weights[0], lambda_ssim=loss_weights[1])
 
     def mean_loss():
         return float(np.mean([float((fit.render(rays_o, rays_d, sensor, p)[0][..., :3] - t).abs().mean()) for p, t in zip(views, targets)]))
@@ -59,25 +50,16 @@ def test_fit_with_densification_changes_n_and_still_converges():
     the test): the number of Gaussians changes, every buffer follows, and the loss still goes down."""
     import densify
     import train_step
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1(n=600, width=96, height=96)
-    W, H = sc.width, sc.height
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     P, S = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
 
-    def raw_from(particles, sph):
-        dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-                "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
     lrs = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
-    truth = train_step.GaussianTrainStep(raw_from(P, S), lrs)
+    truth = train_step.GaussianTrainStep(train_step.raw_params(P, S), lrs)
     views = [scenes.pose7_from_c2w(sc.camera(i, 6)) for i in range(6)]
     targets = [truth.render(rays_o, rays_d, sensor, p)[0][..., :3].clone() for p in views]
     keep = torch.arange(sc.n, device=dev) % 3 != 0  # start from two thirds of the Gaussians: the fit has to grow some back
@@ -86,7 +68,7 @@ def test_fit_with_densification_changes_n_and_still_converges():
     conf = densify.DensifyConfig(clone_grad_threshold=2e-6, split_grad_threshold=2e-6, relative_size_threshold=0.03, prune_density_threshold=0.02,
                                  densify_start=10, densify_end=200, densify_frequency=30, prune_start=10, prune_end=200, prune_frequency=45,
                                  reset_start=-1, seed=1)
-    fit = train_step.GaussianTrainStep(raw_from(P2, S2), lrs, densify_conf=conf, scene_extent=3.0)
+    fit = train_step.GaussianTrainStep(train_step.raw_params(P2, S2), lrs, densify_conf=conf, scene_extent=3.0)
     n0 = fit.n
 
     def mean_loss():
@@ -108,25 +90,16 @@ def test_fit_with_mcmc_strategy_runs_on_the_gpu():
     """MCMC strategy (relocate / add / perturb) hooked into the training step: N grows by 5 % per add, buffers follow, the fit descends."""
     import densify
     import train_step
-    from threedgut_tracer.tracer import ShutterType, fromOpenCVPinholeCameraModelParameters
 
     dev = torch.device("cuda", 0)
     sc = scenes.scene_c1(n=600, width=96, height=96)
-    W, H = sc.width, sc.height
-    sensor = fromOpenCVPinholeCameraModelParameters(np.array([W, H]), ShutterType.GLOBAL, np.array([sc.cx, sc.cy], np.float32),
-                                                    np.array([sc.fx, sc.fy], np.float32), np.zeros(6, np.float32), np.zeros(2, np.float32),
-                                                    np.zeros(4, np.float32))
+    sensor = sc.pinhole_sensor()
     ro, rd = sc.rays()
     rays_o, rays_d = torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(dev)
     P, S = torch.from_numpy(sc.particles).to(dev), torch.from_numpy(sc.sph).to(dev)
 
-    def raw_from(particles, sph):
-        dns = particles[:, 3:4].clamp(1e-4, 1 - 1e-4)
-        return {"positions": particles[:, 0:3].clone(), "density": torch.log(dns / (1 - dns)), "rotation": particles[:, 4:8].clone(),
-                "scale": torch.log(particles[:, 8:11]), "features_albedo": sph[:, 0:3].clone(), "features_specular": sph[:, 3:48].clone()}
-
     lrs = dict(positions=2e-3, density=0.05, rotation=1e-3, scale=5e-3, features_albedo=1e-2, features_specular=5e-4)
-    truth = train_step.GaussianTrainStep(raw_from(P, S), lrs)
+    truth = train_step.GaussianTrainStep(train_step.raw_params(P, S), lrs)
     views = [scenes.pose7_from_c2w(sc.camera(i, 6)) for i in range(6)]
     targets = [truth.render(rays_o, rays_d, sensor, p)[0][..., :3].clone() for p in views]
     gen = torch.Generator(device=dev).manual_seed(0)
@@ -135,7 +108,7 @@ def test_fit_with_mcmc_strategy_runs_on_the_gpu():
     S2[:, 0:3] += 0.5 * torch.randn((sc.n, 3), device=dev, generator=gen)
     P2[::9, 3] = 0.001  # a few dead Gaussians for relocate()
     conf = densify.MCMCConfig(relocate_start=5, relocate_frequency=20, add_start=5, add_frequency=20, perturb_start=0, noise_lr=5e3, seed=2)
-    fit = train_step.GaussianTrainStep(raw_from(P2, S2), lrs, densify_conf=conf, lambda_l1=0.8, lambda_ssim=0.2)
+    fit = train_step.GaussianTrainStep(train_step.raw_params(P2, S2), lrs, densify_conf=conf, lambda_l1=0.8, lambda_ssim=0.2)
 
     def mean_loss():
         return float(np.mean([float((fit.render(rays_o, rays_d, sensor, p)[0][..., :3] - t).abs().mean()) for p, t in zip(views, targets)]))

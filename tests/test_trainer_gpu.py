@@ -22,13 +22,9 @@ W = H = 64
 
 
 def _truth_step(sc):
-    from train_step import GaussianTrainStep
+    from train_step import GaussianTrainStep, raw_params
 
-    p = torch.from_numpy(sc.particles).cuda()
-    d = p[:, 3:4].clamp(1e-4, 1 - 1e-4)
-    params = {"positions": p[:, 0:3].contiguous(), "density": torch.log(d / (1 - d)), "rotation": p[:, 4:8].contiguous(),
-              "scale": torch.log(p[:, 8:11]).contiguous(), "features_albedo": torch.from_numpy(sc.sph[:, :3]).cuda().contiguous(),
-              "features_specular": torch.from_numpy(sc.sph[:, 3:]).cuda().contiguous()}
+    params = raw_params(torch.from_numpy(sc.particles).cuda(), torch.from_numpy(sc.sph).cuda())
     return GaussianTrainStep(params, {k: 0.0 for k in params}, sph_degree=3)
 
 
